@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- CSPN propagation throughput on B200 (contract: see the task brief / DESIGN.md section 6).
+"""bench.py -- CSPN propagation throughput on an H100 (DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--algo auto|generic|cluster]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path (24-iteration 2D CSPN, '8sum', with sparse depth) over one batch of
 synthetic inputs of BASELINE.json configs[1]: 32 x 1216x352 (W x H) per GPU, fp32.  Weak scaling: every
 rank owns its own 32 images (N=8 is configs[4], 256 images); no data-path collective.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR also writes the result of the last timed step as DIR/out.npy
+(float32, 54.8 MB; with several GPUs rank 0's shard only): the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -38,17 +40,7 @@ def measured_hbm_peak():
         with open(p) as fh:
             return float(json.load(fh)['hbm_gbs']), 'measured (MEASURED_PEAKS.json, burst copy)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md)'
-
-
-def recorded_traffic(algo_name):
-    """dram bytes per launch of the dominant kernel from the committed ncu --set full capture, or None."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'traffic.json')) as fh:
-            t = json.load(fh)
-        return t.get(algo_name, {}).get('dram_bytes_per_launch')
-    except Exception:
-        return None
+        return 3350.0, 'H100 SXM data sheet (HBM3, 3.35 TB/s)'
 
 
 class ClockSampler:
@@ -203,8 +195,8 @@ def cpu_baseline_leg():
         gpu_eager = None
     return {'value': round(mpx4, 3), 'unit': 'Mpixels/s', 'cores': threads, 'kind': 'port',
             'sample': f'4x{W}x{H} images (B=4: BASELINE.md section 3), {ITERS} iters, {NORM}, with sparse depth: 1 warm-up + median of '
-                      f'3 forwards of oracle/cspn_torch_port.py (the reference op sequence of cspn.py:42-83 on CPU; '
-                      f'/root/reference is absent on this box); {threads} torch threads = the fastest of 8/16/32/64 on this host '
+                      f'3 forwards of oracle/cspn_torch_port.py (the reference op sequence of cspn.py:42-83 on CPU); '
+                      f'{threads} torch threads = the fastest of 8/16/32/64 on this host '
                       f'(warm-up + median of 3 each)',
             'ms_per_forward': round(t4 * 1e3, 1),
             'b1_value': round(mpx1, 3), 'b1_ms_per_forward': round(t1 * 1e3, 1),
@@ -293,8 +285,9 @@ def other_configs(dev, peak, sm_max_mhz):
     from cspn_b200.synth import make_inputs, make_inputs_3d
     L = _lib.lib()
     out = {}
-    fma_peak = 148 * 128 * (sm_max_mhz or 1965) * 1e6          # FMA/s at the maximum SM clock
-    # ---- configs[2]: 64 x 304x228, N in {4,8,16,24,48}; two input sets alternate (2 x 195 MB > 126 MB L2) ----------------
+    n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    fma_peak = n_sms * 128 * (sm_max_mhz or 1980) * 1e6        # FMA/s at the maximum SM clock (128 FP32 lanes per SM)
+    # ---- configs[2]: 64 x 304x228, N in {4,8,16,24,48}; two input sets alternate (2 x 195 MB > 50 MB L2) -----------------
     Bn, Hn, Wn = 64, 228, 304
     sets = [[t.to(dev) for t in make_inputs(sd, Bn, 1, Hn, Wn)] for sd in (1, 2)]
     px = Bn * Hn * Wn
@@ -326,9 +319,9 @@ def other_configs(dev, peak, sm_max_mhz):
                          'launches': launches, 'algo': algo_name}
         del graph
     out['cfg3_nyu_sweep'] = {'workload': f'2D CSPN 3x3, {NORM}, with sparse depth, batch {Bn}x{Wn}x{Hn} (BASELINE configs[2])',
-                             'timing': 'one CUDA graph of 10 calls alternating two input sets (2 x 195 MB > 126 MB L2), median of 7 '
+                             'timing': 'one CUDA graph of 10 calls alternating two input sets (2 x 195 MB > 50 MB L2), median of 7 '
                                        'CUDA-event timed replays after 2 warm-up, per call',
-                             'fp32_ceiling': f'148 SM x 128 FMA/clk x {sm_max_mhz} MHz / (8 N + 30) FMA per pixel (BASELINE.md section 2)',
+                             'fp32_ceiling': f'{n_sms} SM x 128 FMA/clk x {sm_max_mhz} MHz / (8 N + 30) FMA per pixel (BASELINE.md section 2)',
                              'by_iters': sweep}
     del sets
     # ---- configs[0]'s shape on the GPU: one 304x228 image, latency of the call ------------------------------------------
@@ -363,11 +356,9 @@ def other_configs(dev, peak, sm_max_mhz):
         t = ms[len(ms) // 2] * 1e-3
         r3[mode] = {'ms': round(t * 1e3, 3), 'mvox_s': round(vox / t / 1e6, 1), 'hbm_gbs': round(112 * vox / t / 1e9, 1),
                     'hbm_frac': round(112 * vox / t / 1e9 / peak, 4), 'launches': L.cspn_last_launches()}
-    tr = recorded_traffic('step3d')
     out['cfg4_3d'] = {'workload': f'3D CSPN 3x3x3, {N3} iters, volume {B3}x{D3}x{H3}x{W3} [B,D,H,W], 26-channel guidance (BASELINE configs[3])',
                       'unit': 'Mvoxels/s; algorithmic 112 B/voxel (26 guidance + 1 read + 1 write, fp32)', 'parity': 'unpinned (3D arithmetic '
                       'is not in the reference tree; checked against the repo\'s own restatement)', 'by_norm': r3,
-                      'traffic_per_step_launch_per_volume': tr,
                       'timing': 'median of 5 CUDA-event timed calls after 2 warm-up; inputs 1.7 GB > L2'}
     return out
 
@@ -375,14 +366,21 @@ def other_configs(dev, peak, sm_max_mhz):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=20)
+    ap.add_argument('--steps', type=int, default=20, help='timed steps (>= 1)')
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--algo', default='auto', choices=['auto', 'generic', 'cluster'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-other-configs', action='store_true')
     ap.add_argument('--e2e-steps', type=int, default=5)
+    ap.add_argument('--dump-outputs', metavar='DIR',
+                    help='write the last timed step\'s result to DIR/out.npy (float32); with --gpus N only rank 0\'s shard '
+                         '(its own 32 images) is written')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes what the CUDA path computed: it needs --impl ours')
     args.warmup = max(args.warmup, 3)
     quiet_stdout()
 
@@ -437,7 +435,7 @@ def main():
     algo_used = _lib.ALGO_NAMES[L.cspn_last_algo()]
     plan = cspn_b200.describe_plan(B_PER_GPU, 1, H, W, ITERS, algo)
 
-    # ---- timed region: K steps, inputs resident in HBM (602.7 MB per step > 126 MB L2) -------------
+    # ---- timed region: K steps, inputs resident in HBM (602.7 MB per step > 50 MB L2) --------------
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with ClockSampler(physical_gpu_index(local_rank)) as clocks:
         barrier()
@@ -452,6 +450,10 @@ def main():
     ms_total = float(ms.item())
     ms_per_step = ms_total / args.steps
     value = world * px / (ms_per_step * 1e-3) / 1e6
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'out.npy'), out.float().cpu().numpy())
 
     # ---- dominant-kernel roofline: events around each launch sequence of one step, averaged --------
     kern_ms = event_times(step, args.steps, 0)
@@ -459,7 +461,7 @@ def main():
     peak, peak_src = measured_hbm_peak()
     achieved = ALGO_BYTES_PER_PX * px / (kern_ms_avg * 1e-3) / 1e9
     roofline = {'bound': 'hbm', 'achieved': round(achieved, 1), 'peak': peak, 'unit': 'GB/s',
-                'frac': round(achieved / peak, 4), 'traffic': recorded_traffic(algo_used),
+                'frac': round(achieved / peak, 4),
                 'peak_source': peak_src, 'kernel': f'{algo_used} ({launches_per_step} launch(es) per step)',
                 'algorithmic_bytes_per_launch_sequence': ALGO_BYTES_PER_PX * px,
                 'launch_ms_avg': round(kern_ms_avg, 4), 'launch_ms_min': round(kern_ms[0], 4)}
@@ -529,7 +531,7 @@ def main():
         gather['best'] = best[1]
         gather['mpx_s_with_all_gather'] = round(world * px / (best[0] * 1e-3) / 1e6, 1)
         gather['limiter'] = (f'each GPU receives {(world - 1) * px * 4 / 1e6:.0f} MB per step over NVLink: '
-                             f'>= {(world - 1) * px * 4 / 900e9 * 1e3:.3f} ms at 900 GB/s per direction')
+                             f'>= {(world - 1) * px * 4 / 450e9 * 1e3:.3f} ms at 450 GB/s per direction (H100 NVLink)')
 
     cpu_baseline = None
     configs = None
@@ -546,7 +548,7 @@ def main():
             'warmup': args.warmup, 'ms_per_step': round(ms_per_step, 4), 'higher_is_better': True, 'scaling': 'weak',
             'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': cfg,
-            'detail': {'l2': 'inputs per step (602.7 MB/GPU) exceed the 126 MB L2; no flush needed', 'algo': algo_used, 'plan': plan},
+            'detail': {'l2': 'inputs per step (602.7 MB/GPU) exceed the 50 MB L2; no flush needed', 'algo': algo_used, 'plan': plan},
             'roofline': roofline, 'cpu_baseline': cpu_baseline, 'e2e': e2e,
             'gpu_launches': world * args.steps * launches_per_step,
             'clocks': clocks.summary(), 'e2e_matches_device_path': same,

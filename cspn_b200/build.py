@@ -1,8 +1,8 @@
-"""Build libcspn_b200.so (the C-ABI product library) in-tree with nvcc for sm_100a.
+"""Build libcspn_b200.so (the C-ABI product library) in-tree with nvcc for sm_90a (H100).
 
     python -m cspn_b200.build [--force]
 
-Output: cspn_b200/_build/libcspn_b200.so (git-ignored; travels to the GPU box with gpurun).
+Output: cspn_b200/_build/libcspn_b200.so (a build product, kept out of git).
 No torch headers are involved: the library is plain CUDA C++ behind include/cspn_b200.h.
 """
 import glob
@@ -19,7 +19,7 @@ LIB = os.path.join(OUT_DIR, 'libcspn_b200.so')
 STAMP = os.path.join(OUT_DIR, 'sources.sha256')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-std=c++17', '-lineinfo',
     '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden',
     '--expt-relaxed-constexpr',
@@ -86,7 +86,7 @@ def build(force=False, verbose=False, defines=(), out=None):
         fh.write('\n'.join(log))
     if verbose:
         print('\n'.join(log))
-    link = [nvcc] + ccbin + ['-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', lib] + objs
+    link = [nvcc] + ccbin + ['-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', lib] + objs
     subprocess.check_call(link, env=env)
     if not variant:
         with open(STAMP, 'w') as fh:

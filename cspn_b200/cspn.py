@@ -4,7 +4,7 @@ Mirrors /root/reference/cspn_pytorch/models/cspn.py (class Affinity_Propagate, :
 constructor, attributes, forward signature, assertion behaviour and return convention, so
 `import cspn as post_process` (torch_resnet_cspn_nyu.py:12) resolves to this file when it is
 placed first on sys.path (see INTEGRATION.md).  All arithmetic runs in libcspn_b200.so
-(hand-written sm_100a CUDA behind the C ABI of include/cspn_b200.h); PyTorch only supplies
+(hand-written sm_90a CUDA behind the C ABI of include/cspn_b200.h); PyTorch only supplies
 device memory, the current stream and autograd plumbing.  There is no CPU / eager fallback.
 """
 import torch

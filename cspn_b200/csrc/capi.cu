@@ -329,9 +329,8 @@ extern "C" CSPN_API int cspn2d_fwd_f32_host(const float* guidance, const float* 
     const size_t s_bytes = sparse ? align_up((size_t)nb * HW * sizeof(float), 256) : 0;
     const size_t ws_bytes = align_up(cspn2d_workspace_bytes(nb, C, H, W, iters, algo), 256);
     const size_t slot_bytes = g_bytes + d_bytes + s_bytes + ws_bytes;
-    // Results stay on the device until every chunk has been uploaded: on this platform an H2D and a D2H running
-    // concurrently each drop from 48-55 GB/s to 38 GB/s, and the output is only 1/10 of the input, so one D2H at the
-    // end (1 ms) beats overlapping it (measured: 17.8 ms -> see profiles/).
+    // Results stay on the device until every chunk has been uploaded: an H2D and a D2H running concurrently share the
+    // host link, and the output is only 1/10 of the input, so one D2H at the end beats overlapping it.
     rc = ensure_slot(pipe.result, (size_t)B * C * HW * sizeof(float));
     if (rc != CSPN_OK) return rc;
     float* dout_all = reinterpret_cast<float*>(pipe.result.buf);
@@ -349,8 +348,8 @@ extern "C" CSPN_API int cspn2d_fwd_f32_host(const float* guidance, const float* 
         float* dd = reinterpret_cast<float*>(s.buf + g_bytes);
         float* dsp = sparse ? reinterpret_cast<float*>(s.buf + g_bytes + d_bytes) : nullptr;
         void* dws = ws_bytes ? s.buf + g_bytes + d_bytes + s_bytes : nullptr;
-        // only channels 0..7 of the guidance are used (cspn.py:91-98): copy just those planes.  (A pitched 2D copy
-        // runs at ~20 GB/s on this platform against 48 GB/s for a linear one, so it is used only when needed.)
+        // only channels 0..7 of the guidance are used (cspn.py:91-98): copy just those planes, with one linear copy
+        // when the guidance has exactly 8 channels.
         if (guidance_channels == 8)
             CSPN_CUDA_TRY(cudaMemcpyAsync(dg, guidance + (size_t)b0 * 8 * HW, (size_t)n * 8 * HW * sizeof(float),
                                           cudaMemcpyHostToDevice, s.stream));

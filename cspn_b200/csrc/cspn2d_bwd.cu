@@ -15,12 +15,10 @@
 // The forward iterates d_1..d_{N-1} are recomputed and kept in the workspace ((N-1) B C H W floats).
 //
 // Two formulations:
-//  * cluster (default; validated on B200 in round 2 against fp64 autograd through the reference's op sequence and the
-//    gradient goldens): the forward cluster kernel in kStoreSteps mode writes every iterate, the same kernel in kAdjoint
+//  * cluster (default; checked against fp64 autograd through the reference's op sequence and the gradient goldens): the forward cluster kernel in kStoreSteps mode writes every iterate, the same kernel in kAdjoint
 //    mode runs the transposed stencil register-resident and writes every lambda_t, and one gather kernel forms
 //    Gw_k(p) = sum_t lambda_{t+1}(p) d_t(p + off_k), Gc = sum_t lambda_{t+1} straight into the finalize arithmetic:
-//    no Gw planes in memory, 2 N planes of workspace.  2.6x / 3.2x faster than the next one on the train-step shapes
-//    (profiles/r02_train_step_timing.txt).
+//    no Gw planes in memory, 2 N planes of workspace.
 //  * launch-per-step (W % 4 != 0, misaligned tensors, or CSPN_B200_BWD=steps): generic prep + N-1 forward steps, N adjoint
 //    steps that also read-modify-write the 8 planes of Gw, finalize.
 #include <cstdlib>

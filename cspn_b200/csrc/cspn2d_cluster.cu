@@ -1,4 +1,4 @@
-// 2D CSPN, all N iterations in ONE launch with HBM touched once per tile (sm_100a).
+// 2D CSPN, all N iterations in ONE launch with HBM touched once per tile (sm_90a: TMA, clusters, DSMEM, mbarrier).
 //
 // Reference arithmetic: /root/reference/cspn_pytorch/models/cspn.py:42-144 (see cspn2d_generic.cu
 // for the folded form d <- c' + sum_k w'_k shift_k(d)).
@@ -28,7 +28,6 @@
 //     exchange buffers written remotely through DSMEM with st.async, whose complete_tx lands on the consumer's
 //     mbarrier: pure dataflow, one mbarrier wait per iteration and no cluster-wide barrier inside the loop.
 // No tensor cores: a 9-point stencil with per-pixel weights is FMA-issue + HBM bound, not a contraction.
-// Tuning history and the measured dead ends (FFMA2, pairwise barriers, flags, ...): profiles/r01_tuning_log.md.
 #include <cstdlib>
 #include <mutex>
 #include <vector>
@@ -185,11 +184,7 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 //   then cbuf[RB][TW]         folded constant term c' of the current task
 //   then 3 mbarriers          tma, full[0], full[1]
 //
-// Arithmetic is scalar FFMA on purpose.  fma.rn.f32x2 (FFMA2, new on sm_100) was tried with pixel pairs in 64-bit
-// registers: with 160 weight registers live per thread it sustains only ~0.22 FFMA2/clk per sub-partition (715 cycles
-// for one 20-pixel step of two warps) against 489-550 cycles for the same step in scalar FFMA
-// (profiles/r01_stencil_probe_ffma_vs_ffma2.txt): three distinct 64-bit register operands per instruction starve on
-// register-file bandwidth.
+// Arithmetic is scalar FFMA: sm_90 has no packed FP32 FMA, and the stencil has no contraction for the tensor cores.
 template <int PR, int PC, int NW>
 struct Cfg {
     static constexpr int kThreads = 32 * NW;
@@ -218,7 +213,7 @@ struct Cfg {
     static_assert(TWP <= 256, "TMA box <= 256 columns");
     static_assert(RB <= 256 && RB % 4 == 0, "TMA box rows; plane size must stay a multiple of 128 B");
     static_assert(PR >= 2, "a patch needs distinct top and bottom rows");
-    static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared memory of an sm_100 CTA");
+    static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared memory of an sm_90 CTA");
 };
 
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -320,7 +315,7 @@ __device__ __forceinline__ void publish(const Xch& x, int wy, const float (&top)
 // Tile-edge lanes: the shuffled-in value of lane 0 (31) is meaningless; instead of zeroing it with a select per row and
 // step, the three taps that would consume it are predicated off (exactly the reference's zero padding, NaN-safe).
 // Measured alternatives (all own-row FMAs before the wait, wait forced late through a data dependency, source-major
-// order over all interior rows, two phase-shifted warp groups): profiles/r02_tuning_log.md.
+// order over all interior rows, two phase-shifted warp groups) were no faster.
 // scatter_row2: one source row into the accumulators of one destination row.  `src(jx)`, jx = -1..PC, is the extended
 // source row; it sits SRC_DY rows below the destination row whose weights are `w`.  The loop nest is SOURCE-major: the FMAs
 // that consume one source value are adjacent and write different accumulators (operand-reuse cache, no dependent pairs).
@@ -465,130 +460,6 @@ __device__ __forceinline__ void iterate3(const Xch& x, int wy, uint32_t phase, c
     }
 }
 
-// ---- the same step on FFMA2 (fma.rn.f32x2) ----------------------------------------------------------------------------
-// An FFMA reads three distinct registers over two register-file banks: two issue cycles each (profiles/r02_tuning_log.md).
-// fma.rn.f32x2 does two IEEE FMAs on 64-bit register pairs at one instruction per two cycles: the same pipe time for half
-// the instructions and no bank stalls -- provided every operand already IS an aligned register pair.  A thread's four
-// columns c0..c3 are therefore held as the STRIDED pairs S0 = (c0, c2) and S1 = (c1, c3).  A tap with dx = +-1 maps pairs
-// onto pairs: S0 reads (c-1, c1) =: T- , S0, S1 for dx = -1, 0, +1 and S1 reads S0, S1, (c2, c4) =: T+ ; T- and T+ cost one
-// shuffle (or one LDS.32 of the padded exchange row) plus one MOV each per source row.  Shared-memory rows that only this
-// kernel reads (c', exchange rows) keep every quad in the order (c0, c2, c1, c3), so an LDS.128 / STS.128 / st.async moves
-// two pairs; columns -1 and 4 of a quad are still the floats next to it.  Tile-edge lanes zero the shuffled-in half (a
-// select; half an FFMA2 cannot be predicated): the reference's zero padding, taken literally.
-// Everything that lives across steps is a 64-bit value (P2) so that the register allocator sees pairs, not two floats it
-// may place apart (with float2 it kept the rows in the quad order of the loads in front of the loop and rebuilt every
-// pair with two MOVs: 186 MOVs per two steps).
-typedef unsigned long long P2;
-__device__ __forceinline__ P2 pk(float lo, float hi) { P2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ float p_lo(P2 v) { float a, b; asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); return a; }
-__device__ __forceinline__ float p_hi(P2 v) { float a, b; asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); return b; }
-__device__ __forceinline__ P2 ffma2(P2 a, P2 b, P2 c) { P2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-struct RowP {
-    const P2 (&v)[2];
-    const P2 (&ed)[2];
-    __device__ __forceinline__ P2 operator()(int u) const { return u < 0 ? ed[0] : (u >= 2 ? ed[1] : v[u]); }
-};
-__device__ __forceinline__ void load_row_smem_p(const float* p, P2 (&v)[2]) {
-    asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(v[0]), "=l"(v[1]) : "r"(smem_u32(p)) : "memory");
-}
-// source pair u = q + dx feeds destination pair q; source-major order as in scatter_row2
-template <int SRC_DY, typename Src>
-__device__ __forceinline__ void scatter_row_p(const P2 (&w)[2][8], const Src& src, P2 (&acc)[2]) {
-#pragma unroll
-    for (int ux = 0; ux <= 3; ++ux) {
-        const int su = ux <= 1 ? ux : (ux == 2 ? -1 : 2);
-        const P2 xv = src(su);
-#pragma unroll
-        for (int dx = 1; dx >= -1; --dx) {
-            const int q = su - dx;
-            if (q < 0 || q >= 2) continue;
-            if (SRC_DY == 0 && dx == 0) continue;
-            acc[q] = ffma2(w[q][tap_of(SRC_DY, dx)], xv, acc[q]);
-        }
-    }
-}
-__device__ __forceinline__ void row_edges_p(const P2 (&v)[2], P2 (&ed)[2], bool first_lane, bool last_lane) {
-    const float l = __shfl_up_sync(0xffffffffu, p_hi(v[1]), 1);      // c3 of the lane to the left  = my column -1
-    const float r = __shfl_down_sync(0xffffffffu, p_lo(v[0]), 1);    // c0 of the lane to the right = my column 4
-    ed[0] = pk(first_lane ? 0.f : l, p_lo(v[1]));                    // T- = (c-1, c1)
-    ed[1] = pk(p_hi(v[0]), last_lane ? 0.f : r);                     // T+ = (c2, c4)
-}
-// publish() for rows held as pairs
-template <int PR, int NW, int PAR>
-__device__ __forceinline__ void publish_p(const Xch& x, int wy, const P2 (&top)[2], const P2 (&bot)[2]) {
-    using K = Cfg<PR, 4, NW>;
-    // (two 64-bit stores per row instead of one 128-bit store do not save the four MOVs that gather a row's two pairs into
-    // an aligned register quad: ptxas fuses them back into an STS.128)
-    const uint32_t p = smem_u32(x.base + (size_t)PAR * K::kSlots * K::TWX);
-    asm volatile("st.shared.v2.b64 [%0], {%1, %2};" ::"r"(p + (uint32_t)((1 + 2 * wy) * K::TWX * 4)), "l"(top[0]), "l"(top[1]) : "memory");
-    asm volatile("st.shared.v2.b64 [%0], {%1, %2};" ::"r"(p + (uint32_t)((2 + 2 * wy) * K::TWX * 4)), "l"(bot[0]), "l"(bot[1]) : "memory");
-    const uint32_t bar = x.bar_full0 + 8 * PAR;
-    if (x.remote_up)
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.b64 [%0], {%1, %2}, [%3];" ::"r"(
-                         x.up_data + PAR * (uint32_t)K::kXchParityBytes), "l"(top[0]), "l"(top[1]), "r"(x.up_bar + 8 * PAR) : "memory");
-    if (x.remote_dn)
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.b64 [%0], {%1, %2}, [%3];" ::"r"(
-                         x.dn_data + PAR * (uint32_t)K::kXchParityBytes), "l"(bot[0]), "l"(bot[1]), "r"(x.dn_bar + 8 * PAR) : "memory");
-    __syncwarp();
-    // one arrival per warp (lane 0); the first warp's also arms the bytes the neighbour CTAs will deliver (expect_tx of 0
-    // bytes is a plain arrival): one predicated instruction and one predicate instead of two of each
-    mbar_arrive_expect_tx_if(bar, x.my_tx, x.first_lane);
-}
-
-// Same phases as iterate3: A own-row taps of the boundary rows, B wait -> halo taps -> publish, C interior rows (seeded
-// with c' after the publish, which pins the order), D seeds of the next step's boundary rows.
-template <int PR, int NW, int PAR, bool PUBLISH>
-__device__ __forceinline__ void iterate_p(Xch& x, int wy, uint32_t phase, const P2 (&w)[PR][2][8], P2 (&din)[PR][2],
-                                          const P2 (&ein)[PR][2], P2 (&dout)[PR][2], P2 (&eout)[PR][2]) {
-    using K = Cfg<PR, 4, NW>;
-    scatter_row_p<0>(w[0], RowP{din[0], ein[0]}, dout[0]);
-    scatter_row_p<+1>(w[0], RowP{din[1], ein[1]}, dout[0]);
-    scatter_row_p<0>(w[PR - 1], RowP{din[PR - 1], ein[PR - 1]}, dout[PR - 1]);
-    scatter_row_p<-1>(w[PR - 1], RowP{din[PR - 2], ein[PR - 2]}, dout[PR - 1]);
-#ifndef CSPN_ABLATE_NO_SYNC
-    CSPN_STAMP(x, 5 + 3 * x.step);
-    mbar_wait(x.bar_full0 + 8 * PAR, phase);
-    CSPN_STAMP(x, 6 + 3 * x.step);
-#endif
-    {
-        const float* p = x.base + (size_t)PAR * K::kSlots * K::TWX;
-        const float* pu = p + (2 * wy) * K::TWX;          // row above my patch
-        const float* pd = p + (2 * wy + 3) * K::TWX;      // row below my patch
-        P2 u[2], ue[2], d[2], de[2];
-        load_row_smem_p(pu, u);
-        load_row_smem_p(pd, d);
-        ue[0] = pk(pu[-1], p_lo(u[1])); ue[1] = pk(p_hi(u[0]), pu[4]);   // pad floats are zero at the tile edges
-        de[0] = pk(pd[-1], p_lo(d[1])); de[1] = pk(p_hi(d[0]), pd[4]);
-        scatter_row_p<-1>(w[0], RowP{u, ue}, dout[0]);
-        scatter_row_p<+1>(w[PR - 1], RowP{d, de}, dout[PR - 1]);
-    }
-    if constexpr (PUBLISH) {
-#ifndef CSPN_ABLATE_NO_SYNC
-        publish_p<PR, NW, PAR ^ 1>(x, wy, dout[0], dout[PR - 1]);
-        CSPN_STAMP(x, 7 + 3 * x.step);
-#else
-        asm volatile("" ::: "memory");
-#endif
-        row_edges_p(dout[0], eout[0], x.first_lane, x.last_lane);
-        row_edges_p(dout[PR - 1], eout[PR - 1], x.first_lane, x.last_lane);
-    }
-#pragma unroll
-    for (int r = 1; r + 1 < PR; ++r) {
-        load_row_smem_p(x.cbuf + r * K::TW, dout[r]);
-        scatter_row_p<-1>(w[r], RowP{din[r - 1], ein[r - 1]}, dout[r]);
-        scatter_row_p<0>(w[r], RowP{din[r], ein[r]}, dout[r]);
-        scatter_row_p<+1>(w[r], RowP{din[r + 1], ein[r + 1]}, dout[r]);
-        if constexpr (PUBLISH) row_edges_p(dout[r], eout[r], x.first_lane, x.last_lane);
-    }
-    if constexpr (PUBLISH) {
-        load_row_smem_p(x.cbuf, din[0]);
-        load_row_smem_p(x.cbuf + (PR - 1) * K::TW, din[PR - 1]);
-    }
-#ifdef CSPN_TRACE
-    ++x.step;
-#endif
-}
-
 template <int PR, int PC, int NW, int PAR, bool PUBLISH, bool CHAIN = false>
 __device__ __forceinline__ void step_fwd(Xch& x, int wy, uint32_t phase, const float (&w)[PR][PC][8],
                                          float (&din)[PR][PC], float (&ein)[PR][2], float (&dout)[PR][PC],
@@ -684,14 +555,6 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                       const __grid_constant__ CUtensorMap tm_sparse, const __grid_constant__ ClusterParams prm) {
     using K = Cfg<PR, PC, NW>;
     constexpr int RB = K::RB, TW = K::TW, TWP = K::TWP, TWX = K::TWX;
-    // -DCSPN_PAIRS: the forward step on FFMA2 with strided column pairs (iterate_p); shared-memory rows are then kept in the
-    // quad order (c0, c2, c1, c3).  Measured 410 us against 404 us for the scalar step on cfg2 (profiles/r02_tuning_log.md):
-    // an FFMA2 with three distinct register pairs occupies the issue port for three cycles (profiles/r02_rfprobe.txt).
-#ifdef CSPN_PAIRS
-    constexpr bool kPairs = (MODE == kForward) && !CHAIN;
-#else
-    constexpr bool kPairs = false;
-#endif
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* stage = reinterpret_cast<float*>(smem_raw);
     float* xch = reinterpret_cast<float*>(smem_raw + K::kStageBytes);
@@ -924,12 +787,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
             if (r == 0 && early_publish) {
                 float bot[PC];
                 load_row_smem(my_c + (PR - 1) * TW, bot);
-                if constexpr (kPairs) {
-                    const float tp[PC] = {d[0][0], d[0][2], d[0][1], d[0][3]}, bp[PC] = {bot[0], bot[2], bot[1], bot[3]};
-                    publish<PR, PC, NW, 0>(xc, wy, tp, bp);
-                } else {
-                    publish<PR, PC, NW, 0>(xc, wy, d[0], bot);
-                }
+                publish<PR, PC, NW, 0>(xc, wy, d[0], bot);
             }
             float cj[PC];
             bool exact_div = false;
@@ -963,10 +821,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                 }
             }
             // only this thread ever reads these values back: no barrier needed
-            if constexpr (kPairs) {
-                const float cp[PC] = {cj[0], cj[2], cj[1], cj[3]};
-                store_row_smem(const_cast<float*>(xc.cbuf) + r * TW, cp);
-            } else if constexpr (MODE != kAdjoint) {
+            if constexpr (MODE != kAdjoint) {
                 store_row_smem(const_cast<float*>(xc.cbuf) + r * TW, cj);   // the adjoint has no constant term
             }
             // a pass after the first continues from the previous pass's result; c' above still used d_0
@@ -1040,49 +895,6 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                     for (int j = 0; j < PC; ++j) d[r][j] = d2[r][j];
             }
             cluster_arrive_relaxed();
-        } else if constexpr (kPairs) {
-        // FFMA2 formulation: the same loop on register pairs (see iterate_p)
-        P2 wp[PR][2][8], dp[PR][2], ep[PR][2], dp2[PR][2], ep2[PR][2];
-#pragma unroll
-        for (int r = 0; r < PR; ++r)
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                dp[r][q] = pk(d[r][q], d[r][q + 2]);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) wp[r][q][k] = pk(w[r][q][k], w[r][q + 2][k]);
-            }
-#ifndef CSPN_ABLATE_NO_SYNC
-        if (!early_publish) publish_p<PR, NW, 0>(xc, wy, dp[0], dp[PR - 1]);
-#endif
-#pragma unroll
-        for (int r = 0; r < PR; ++r) row_edges_p(dp[r], ep[r], xc.first_lane, xc.last_lane);
-#pragma unroll
-        for (int r = 0; r < PR; ++r) load_row_smem_p(xc.cbuf + r * TW, dp2[r]);   // accumulators of the first step start from c'
-        int it = 0;
-        for (; it + 2 < iters; it += 2) {   // steady state: every step publishes
-            iterate_p<PR, NW, 0, true>(xc, wy, ph0, wp, dp, ep, dp2, ep2);
-            ph0 ^= 1;
-            iterate_p<PR, NW, 1, true>(xc, wy, ph1, wp, dp2, ep2, dp, ep);
-            ph1 ^= 1;
-        }
-        if (iters - it == 2) {              // the last step of a task has nobody to publish to
-            iterate_p<PR, NW, 0, true>(xc, wy, ph0, wp, dp, ep, dp2, ep2);
-            ph0 ^= 1;
-            iterate_p<PR, NW, 1, false>(xc, wy, ph1, wp, dp2, ep2, dp, ep);
-            ph1 ^= 1;
-        } else if (iters - it == 1) {
-            iterate_p<PR, NW, 0, false>(xc, wy, ph0, wp, dp, ep, dp2, ep2);
-            ph0 ^= 1;
-        }
-        CSPN_STAMP(xc, kTraceEvents - 2);
-        cluster_arrive_relaxed();  // this CTA no longer reads its exchange buffers
-#pragma unroll
-        for (int r = 0; r < PR; ++r)
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                const P2 v = (iters & 1) ? dp2[r][q] : dp[r][q];
-                d[r][q] = p_lo(v); d[r][q + 2] = p_hi(v);
-            }
         } else {
 #ifndef CSPN_ABLATE_NO_SYNC
         if (!early_publish) publish<PR, PC, NW, 0>(xc, wy, d[0], d[PR - 1]);
@@ -1211,7 +1023,7 @@ KernelCfg make_cfg_chain() {
 // The menu the planner picks from.  Register budget per pixel: 8 weights + value + second value set (c' is in shared
 // memory); 8 warps (2 per SM sub-partition) may use 255 registers each -> up to 20 pixels per thread.
 #ifdef CSPN_DEV_SINGLE
-// developer build for offline SASS studies (tools/sass_excerpt.py on a 10-second compile): only the headline kernels
+// developer build for offline SASS studies (tools/sass_loop.py on a 10-second compile): only the headline kernels
 const std::vector<KernelCfg>& configs() {
     static const std::vector<KernelCfg> v = [] {
         KernelCfg k{5, 4, 8, {{nullptr, nullptr}, {nullptr, nullptr}}, {nullptr, nullptr}, {nullptr, nullptr}, {{nullptr, nullptr}, {nullptr, nullptr}},
@@ -1265,7 +1077,7 @@ int sm_count(int dev) {
     static int cached[16] = {};
     if (!cached[dev & 15]) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); n = 148; }
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); n = 132; }
         cached[dev & 15] = n;
     }
     return cached[dev & 15];
@@ -1348,15 +1160,15 @@ bool layout_1d(int L, int T, int halo, int align, int min_useful, int max_n, int
 
 // Best (configuration, cluster size, strips, bands) for one pass of `iters` steps: minimises SM time per image.
 // Deliberately independent of B and C, so the same image gets the same tiling (hence bit-identical results) whatever
-// batch it is part of.  `dev` < 0: no device query (planning on a CPU-only box): assume the B200 occupancy table
-// measured by tools/probe.
+// batch it is part of.  `dev` < 0: no device query (planning without a GPU): assume the H100 SXM occupancy table
+// measured by tools/probe.cu.
 bool plan_pass(int H, int W, int iters, int dev, int forced, bool chained, PassPlan& best) {
-    static const int kProbe256[17] = {0, 148, 74, 45, 33, 26, 22, 15, 15, 15, 11, 7, 7, 7, 7, 7, 7};
+    static const int kProbe256[17] = {0, 132, 66, 39, 30, 22, 17, 15, 15, 9, 7, 7, 7, 7, 7, 7, 7};
     const char* fcs = getenv("CSPN_B200_FORCE_CS");   // developer hook for tuning runs (with CSPN_B200_FORCE_PASSES)
     const int forced_cs = fcs ? atoi(fcs) : 0;
     best.cfg = -1;
     const auto& cf = configs();
-    const int n_sms = dev >= 0 ? sm_count(dev) : 148;
+    const int n_sms = dev >= 0 ? sm_count(dev) : 132;
     for (int ci = 0; ci < (int)cf.size(); ++ci) {
         if (forced >= 0 && ci != forced) continue;
         const KernelCfg& k = cf[ci];
@@ -1378,14 +1190,14 @@ bool plan_pass(int H, int W, int iters, int dev, int forced, bool chained, PassP
             const int mac = dev >= 0 ? max_active_clusters(ci, cs, dev, chained) : kProbe256[cs];
             if (mac <= 0) continue;
             // tasks x per-task work / co-resident clusters.  Per-task work: 8 FMA per pixel and step plus a fixed part
-            // (load, normalisation, store) worth ~15 steps (fit of the cfg3 sweep, profiles/r01_all_configs_timing.txt).
+            // (load, normalisation, store) worth ~15 steps (fit of the BASELINE configs[2] iteration sweep).
             // When a small configuration fits two CTAs per SM they share the SM's FMA pipe: count SMs, not CTAs.
             const int ctas_per_sm = (mac * cs + n_sms - 1) / n_sms;
             p.cost = (double)p.n_strips * p.n_bands * k.RB() * k.TW() * (8.0 * iters + 120.0) * ctas_per_sm / mac;
-            // row bands re-load their halo rows and multiply the task count; measured 7 % slower than this model says
-            // on cfg3 at N=4 (profiles/r01_plan_sweep.txt), so a banded plan has to win by a margin
+            // row bands re-load their halo rows and multiply the task count, which this model does not see, so a banded
+            // plan has to win by a margin
             if (p.n_bands > 1) p.cost *= 1.15;
-            // a chained task is measured ~18 % longer (recorded column: loads, selects, predicated stores per step; hand-over)
+            // a chained task is longer (recorded column: loads, selects, predicated stores per step; hand-over)
             if (chained) p.cost *= 1.20;
             p.cfg = ci; p.cs = cs; p.max_clusters = mac; p.iters = iters;
             if (best.cfg < 0 || p.cost < best.cost) best = p;
@@ -1682,10 +1494,10 @@ int launch_pass(const Problem2D& p, const PassPlan& pp, const void* fn, const fl
     prm.trace = g_trace;
     prm.hist = cb.hist; prm.flags = cb.flags; prm.chain_lane = pp.chain_lane;
     {
-        // group size: at least 1.5 x the co-resident clusters, the groups as equal as possible.  Measured on cfg2-shaped batches
-        // (profiles/r02_tuning_log.md): a strip's left neighbour only 16 tasks back (15 clusters) is not always finished when
-        // its flag is looked at (+4.6 %), 24 back it is, and the shared columns then come from L2 (-2 % against one group,
-        // DRAM reads 1.25 x -> 1.0 x algorithmic).  CSPN_B200_CHAIN_GROUP overrides (0 = one group).
+        // group size: at least 1.5 x the co-resident clusters, the groups as equal as possible.  A strip's left neighbour then
+        // runs at least one full round of clusters earlier, so its flag is normally set when it is first looked at, yet recently
+        // enough that the guidance columns the two tiles share still come from L2 instead of DRAM.  CSPN_B200_CHAIN_GROUP
+        // overrides (0 = one group).
         const long nq_all = (long)p.B * p.C * pp.n_bands;
         long min_g = pp.max_clusters + (pp.max_clusters + 1) / 2;
         if (const char* e = getenv("CSPN_B200_CHAIN_GROUP")) min_g = atol(e) > 0 ? atol(e) : nq_all;

@@ -6,7 +6,7 @@
 // (112 B of input per voxel); with N = 12 and a 3D halo no on-chip temporal blocking fits an
 // SM's 64K registers, so this path streams the normalised weights once per iteration from
 // L2/HBM.  Volumes are processed in groups (grid z carries the volume index): one step launch covers the whole
-// group, because a single volume's step lasts only ~46 us and launch gaps + ramp/tail cost 15 % at that size;
+// group, because a single volume's step is short enough that launch gaps and the grid's ramp / tail are a visible share;
 // the group is capped so that the 27*D*H*W-float workspace per volume stays below kMaxWorkspace3d.
 #include <cstdlib>
 

@@ -93,7 +93,7 @@ masked_l1_bwd_kernel(const float* __restrict__ pred, const float* __restrict__ g
 
 int grid_for(size_t n) {
     size_t b = (n + 255) / 256;
-    const size_t cap = 148 * 8;
+    const size_t cap = 132 * 8;   // 8 blocks per SM of an H100 SXM
     return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -1,7 +1,7 @@
 // torch.ops.cspn_b200.* -- the PyTorch operator registration of the CSPN propagation path.
 //
 // A thin C++ shim over the C ABI of include/cspn_b200.h (libcspn_b200.so): PyTorch supplies device memory, the current
-// stream and the dispatcher entry; every byte of arithmetic stays in the hand-written sm_100a kernels.  Registered as
+// stream and the dispatcher entry; every byte of arithmetic stays in the hand-written sm_90a kernels.  Registered as
 // dispatcher ops (TORCH_LIBRARY) so that torch.compile / torch.export trace the call the reference model makes at
 // /root/reference/cspn_pytorch/models/torch_resnet_cspn_nyu.py:375 as ONE opaque node; the fake (meta) kernels and the
 // autograd formulas are registered from Python (cspn_b200/torch_op.py) with torch.library.

@@ -1,4 +1,4 @@
-/* cspn_b200 -- C ABI of the B200-native CSPN propagation path.
+/* cspn_b200 -- C ABI of the H100-native CSPN propagation path.
  *
  * The reference (XinJCheng/CSPN) has no FFI: its hot path is a Python nn.Module,
  *   Affinity_Propagate.forward(guidance, blur_depth, sparse_depth=None)

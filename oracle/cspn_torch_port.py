@@ -1,13 +1,14 @@
 """PyTorch-op port of the reference's CPU/eager path.  TEST + BASELINE INFRASTRUCTURE ONLY.
 
 This is what `bench.py --impl reference` and bench.py's `cpu_baseline` leg time on the GPU
-box's host cores (/root/reference does not exist there): the same ATen op sequence per
-iteration as /root/reference/cspn_pytorch/models/cspn.py -- 8 zero-pads + cat
+machine's host cores: the same ATen op sequence per iteration as the reference's
+cspn_pytorch/models/cspn.py -- 8 zero-pads + cat
 (cspn.py:147-172), broadcast mul + ones-weight Conv3d as the 8-way sum (cspn.py:44-53,70),
 crop (cspn.py:71-72), centre term (cspn.py:76), mask replacement (cspn.py:81) -- so its cost
 profile (about 25-30 small ops and two (B,8,C,H+2,W+2) temporaries per iteration) is the
 reference's, minus the `.cuda()` call at cspn.py:50 that makes the original unusable on CPU.
-Validated against the real module in tests/test_oracle.py when /root/reference is present.
+Held bit for bit against outputs of the real module (stored under tests/golden/reference_forward/)
+in tests/test_oracle.py.
 Never imported by the product package.
 """
 import torch

@@ -13,12 +13,12 @@ GOLDEN_DIR = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box via gpurun)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu`-marked tests need a CUDA device: on a box without one they are skipped, not failed (the driver's CPU
-    round runs `-m "not gpu"`; a bare `pytest tests` must be green there too)."""
+    """`gpu`-marked tests need a CUDA device: on a machine without one they are skipped, not failed (a bare
+    `pytest tests` must be green there too)."""
     try:
         import torch
         has = torch.cuda.is_available()
@@ -26,7 +26,7 @@ def pytest_collection_modifyitems(config, items):
         has = False
     if has:
         return
-    skip = pytest.mark.skip(reason='no CUDA device on this box (GPU tests run through gpurun)')
+    skip = pytest.mark.skip(reason='no CUDA device on this machine')
     for item in items:
         if 'gpu' in item.keywords:
             item.add_marker(skip)

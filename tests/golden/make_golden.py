@@ -62,6 +62,24 @@ def main():
                         seed=0, B=1, C=1, H=4, W=5, gch=8, sparse='None', n_sample=0)
     print('zero_guidance_nan: all nan =', bool(torch.isnan(out).all()))
     special_cases()
+    reference_forward_cases()
+
+
+# The reference's forward on small signed-sparse inputs, 6 steps: tests/test_oracle.py holds the torch port (bit for bit) and
+# both oracles against these outputs.  Kept in their own directory: they are not cases of the generic golden sweep.
+REFERENCE_FORWARD_SHAPES = [(2, 3, 7, 9), (1, 1, 16, 33)]
+
+
+def reference_forward_cases():
+    out_dir = os.path.join(HERE, 'reference_forward')
+    os.makedirs(out_dir, exist_ok=True)
+    for norm in ('8sum', '8sum_abs'):
+        for (B, C, H, W) in REFERENCE_FORWARD_SHAPES:
+            g, d, s = make_inputs(123, B, C, H, W, 9, 'signed', 20)
+            out = ref_loader.reference_forward(g, d, s, 6, norm)
+            np.savez_compressed(os.path.join(out_dir, f'{norm}_{B}x{C}x{H}x{W}.npz'), guidance=g.numpy(), blur=d.numpy(),
+                                sparse_depth=s.numpy(), out=out.numpy(), prop_time=6, norm_type=norm)
+            print(f'reference_forward {norm} {B}x{C}x{H}x{W}: out shape {tuple(out.shape)}')
 
 
 def save_special(name, guidance, blur, sp, n, norm):

@@ -7,7 +7,7 @@ post_process_layer (torch_resnet_cspn_nyu.py:372-375) and what the model returns
 
 tests/golden/model/nyu_resnet50_tail.npz: guidance (1,8,228,304), blur (1,1,228,304), sparse_depth (1,1,228,304), out.
 The GPU box has no /root/reference: tests/test_reference_model_golden_gpu.py feeds these boundary tensors to the
-B200 module and must reproduce the reference MODEL's output -- the exit criterion of SURVEY.md section 7.2.
+CUDA module and must reproduce the reference MODEL's output -- the exit criterion of SURVEY.md section 7.2.
 float16-rounded storage would break bit-faithfulness of the inputs, so everything is stored as float32 (npz-compressed).
 """
 import importlib

@@ -1,8 +1,8 @@
-"""Model-level parity (SURVEY.md section 7.2's exit criterion) on the GPU box, where /root/reference does not exist:
+"""Model-level parity (SURVEY.md section 7.2's exit criterion) on the GPU, without the reference tree:
 tests/golden/model/nyu_resnet50_tail.npz holds what the reference's OWN model code (resnet50 + Gudi UNet decoder,
 torch_resnet_cspn_nyu.py, random seeded weights) handed to its post_process_layer (:372-375) and what that model
-returned with the reference's own cspn.py as the layer -- generated in the build container by
-tests/golden/make_golden_model.py.  Fed the same boundary tensors, the B200 module must return the reference MODEL's output."""
+returned with the reference's own cspn.py as the layer -- generated where the reference tree exists by
+tests/golden/make_golden_model.py.  Fed the same boundary tensors, the CUDA module must return the reference MODEL's output."""
 import os
 
 import numpy as np

@@ -1,5 +1,6 @@
-// Hardware probe run once on the B200 box: cluster occupancy for the cluster kernel's resource shape,
-// DRAM / L2 bandwidth, device attributes.  Output feeds the plan heuristics in cspn2d_cluster.cu / DESIGN.md.
+// Hardware probe: cluster occupancy for the cluster kernel's resource shape, DRAM / L2 bandwidth, device attributes.
+// Its occupancy lines are the table the planner in cspn2d_cluster.cu assumes when it plans without a GPU.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/_build/probe tools/probe.cu && tools/_build/probe
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <vector>
@@ -31,7 +32,7 @@ template <typename K>
 void occ(K kern, int threads, int smem, const char* name) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    for (int cs : {1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 14, 15, 16}) {
+    for (int cs = 1; cs <= 16; ++cs) {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(cs * 64);
         cfg.blockDim = dim3(threads);
@@ -68,15 +69,15 @@ int main() {
         float4 *a, *b; cudaMalloc(&a, bytes); cudaMalloc(&b, bytes);
         cudaMemset(a, 1, bytes);
         int reps = mb <= 128 ? 20 : 4;
-        read_kernel<<<148 * 8, 512>>>(a, n, sink, 2);
+        read_kernel<<<p.multiProcessorCount * 8, 512>>>(a, n, sink, 2);
         cudaEventRecord(e0);
-        read_kernel<<<148 * 8, 512>>>(a, n, sink, reps);
+        read_kernel<<<p.multiProcessorCount * 8, 512>>>(a, n, sink, reps);
         cudaEventRecord(e1); cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         double rd = (double)bytes * reps / (ms * 1e-3) / 1e9;
-        copy_kernel<<<148 * 8, 512>>>(a, b, n);
+        copy_kernel<<<p.multiProcessorCount * 8, 512>>>(a, b, n);
         cudaEventRecord(e0);
-        for (int r = 0; r < 5; ++r) copy_kernel<<<148 * 8, 512>>>(a, b, n);
+        for (int r = 0; r < 5; ++r) copy_kernel<<<p.multiProcessorCount * 8, 512>>>(a, b, n);
         cudaEventRecord(e1); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
         double cp = 2.0 * bytes * 5 / (ms * 1e-3) / 1e9;

@@ -11,7 +11,7 @@ What is supplied around it (nothing inside the reference tree is touched):
   * a checkpoint directory with a `best_model.pth` of seeded random weights in the reference's own format (DataParallel
     `module.` prefix plus the stray `post_process_layer.sum_conv.weight` every reference checkpoint carries);
   * `--cspn dropin`: `dropin/` goes on sys.path BEFORE the reference's ./models (eval.py:52 appends it), so
-    torch_resnet_cspn_nyu.py:12 (`import cspn as post_process`) resolves to the B200 module: needs a GPU.
+    torch_resnet_cspn_nyu.py:12 (`import cspn as post_process`) resolves to the CUDA module: needs a GPU.
     `--cspn reference`: the reference's own cspn.py (CPU works: `.cuda()` becomes the identity where CUDA is absent).
 Returns / prints the model outputs eval.py computed, so the two choices can be compared: same weights, same samples.
 """

@@ -5,7 +5,7 @@
 Prints: registers / spills are in ptxas.log; here the SASS of the kernel is split at its back edges, the longest loop body
 (two propagation steps) is taken, and its instruction mix, the positions of the exchange instructions (SYNCS wait /
 arrive, STS, STAS, LDS, SHFL) along the instruction stream and the share of FFMAs that can take an operand from the
-reuse cache are listed.  profiles/r02_sass_*.txt are outputs of this script.
+reuse cache are listed.
 """
 import collections
 import re
