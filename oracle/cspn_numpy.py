@@ -81,6 +81,13 @@ def affinity_normalization_2d(guidance: np.ndarray, norm_type: str):
     return gate_wb, gate_sum[:, None]
 
 
+def sparse_mask(sparse_depth, dtype=np.float32):
+    """m = sign(sparse_depth), cspn.py:63-64, as torch.sign computes it on the CPU and on CUDA: 0 for NaN (np.sign gives
+    NaN), so a NaN sparse pixel masks nothing."""
+    sp = np.asarray(sparse_depth, dtype=dtype)
+    return (sp > 0).astype(dtype) - (sp < 0).astype(dtype)
+
+
 def cspn2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum',
            dtype=np.float32):
     """Affinity_Propagate.forward, cspn.py:42-83, op for op (unfolded mask / centre term).
@@ -95,7 +102,7 @@ def cspn2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8su
     result = raw                                             # cspn.py:61
     mask = None
     if sparse_depth is not None:
-        mask = np.sign(np.asarray(sparse_depth, dtype=dtype))            # cspn.py:63-64
+        mask = sparse_mask(sparse_depth, dtype)
     with np.errstate(invalid='ignore'):
         for _ in range(prop_time):                           # cspn.py:66
             acc = np.zeros_like(result)

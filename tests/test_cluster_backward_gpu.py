@@ -6,29 +6,11 @@ import pytest
 import torch
 
 import cspn_b200
-from cspn_b200 import _lib
 from cspn_b200.synth import make_inputs
+from forced_plans import backward as grads
 from oracle import cspn_torch_port as tp
 
 pytestmark = pytest.mark.gpu
-
-
-def grads(g, d, s, go, n, norm):
-    """The C ABI's backward called directly (ctypes, this thread): autograd would run it on the engine's worker thread,
-    where the thread-local cspn_last_launches() of this thread does not see it."""
-    L = _lib.lib()
-    gc, dc, goc = g.cuda().contiguous(), d.cuda().contiguous(), go.cuda().contiguous()
-    sc = None if s is None else s.cuda().contiguous()
-    B, C, H, W = dc.shape
-    gg, gd = torch.empty_like(gc), torch.empty_like(dc)
-    ws_bytes = L.cspn2d_bwd_workspace_bytes(B, C, H, W, n)
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device='cuda')
-    rc = L.cspn2d_bwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), goc.data_ptr(), gg.data_ptr(),
-                          gd.data_ptr(), B, C, H, W, gc.shape[1], n, _lib.NORM2D[norm], ws.data_ptr(), ws_bytes,
-                          torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, 'cspn2d_bwd_f32')
-    torch.cuda.synchronize()
-    return gg.double().cpu(), gd.double().cpu(), L.cspn_last_launches()
 
 
 @pytest.mark.parametrize('norm', ['8sum', '8sum_abs'])

@@ -12,6 +12,7 @@ import cspn_b200
 from conftest import golden_names, load_golden
 from cspn_b200 import _lib
 from cspn_b200.synth import make_inputs
+from forced_plans import SPECIAL
 from oracle import c_oracle, cspn_numpy as onp
 
 pytestmark = pytest.mark.gpu
@@ -115,9 +116,18 @@ def test_nan_semantics_match_reference(algo):
     assert_parity(run(g, d, s, 3, '8sum', algo), ref, 'partial NaN')
 
 
-SPECIAL = ['nan_zero_guidance_4x8', 'nan_zero_patch_12x16_n1', 'nan_zero_patch_12x16_n2', 'nan_zero_patch_12x16_n3',
-           'nan_zero_patch_40x132_n6', 'subnormal_affinity_8x8', 'huge_affinity_8x12', 'inf_guidance_8x12',
-           'inf_guidance_abs_8x12']
+@pytest.mark.parametrize('algo', ALGOS)
+def test_nan_sparse_pixel_masks_nothing(algo):
+    """torch.sign(NaN) is 0 on CUDA as on the CPU (the reference's mask, cspn.py:64): a NaN sparse pixel is not a sparse
+    pixel, and both algorithms agree with the torch port there."""
+    from oracle import cspn_torch_port as tp
+    assert torch.sign(torch.tensor([float('nan')], device='cuda')).item() == 0
+    g, d, s = make_inputs(5, 1, 1, 12, 16, 8, 'bernoulli', 10)
+    s[0, 0, 6, 7] = float('nan')
+    ref = tp.cspn2d_torch(g, d, s, 3, '8sum').numpy()
+    out = run(g, d, s, 3, '8sum', algo)
+    assert not np.isnan(out).any()
+    assert_parity(out, ref, 'NaN sparse pixel')
 
 
 @pytest.mark.parametrize('algo', ALGOS)

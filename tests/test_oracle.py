@@ -54,6 +54,22 @@ def test_oracles_and_torch_port_match_reference_outputs(norm, shape):
         assert ok and ratio < 0.05
 
 
+def test_nan_sparse_pixel_masks_nothing_in_every_oracle():
+    """sign(NaN) is 0 in torch (the reference's mask, cspn.py:64), in the C oracle and in the kernels: a NaN in
+    sparse_depth is not a sparse pixel and poisons nothing."""
+    import torch
+    from oracle import cspn_torch_port as tp
+    from cspn_b200.synth import make_inputs
+    g, d, s = make_inputs(5, 1, 1, 12, 16, 8, 'bernoulli', 10)
+    s[0, 0, 6, 7] = float('nan')
+    assert torch.sign(s).isnan().sum() == 0
+    port = tp.cspn2d_torch(g, d, s, 3, '8sum').numpy()
+    assert not np.isnan(port).any()
+    for out in (onp.cspn2d(g.numpy(), d.numpy(), s.numpy(), 3, '8sum'), c_oracle.cspn2d(g.numpy(), d.numpy(), s.numpy(), 3, '8sum')):
+        ok, ratio, _ = onp.parity_ok(out, port)
+        assert ok and ratio < 0.05, ratio
+
+
 def test_semantics_pinned_by_reference():
     """Facts SURVEY.md 8(a) lists, checked on the oracle: sparse pixels return the BLUR depth
     (not the sparse value); prop_time=0 is the identity; extra guidance channels are ignored;

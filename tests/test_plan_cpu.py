@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 from hypothesis import given, settings, strategies as st
 
+import forced_plans as fpl
+from conftest import load_golden
 from cspn_b200 import _lib
 from oracle import cspn_numpy as onp
 
@@ -75,7 +77,7 @@ def replay_chained(info, guidance, blur, sparse, norm):
     f64 = np.float64
     gate_wb, gate_sum = onp.affinity_normalization_2d(guidance.astype(f64), norm)
     raw = blur.astype(f64)
-    mask = None if sparse is None else np.sign(sparse.astype(f64))
+    mask = None if sparse is None else onp.sparse_mask(sparse, f64)
     H, W = raw.shape[-2:]
     cur = raw
     for p in info['passes']:
@@ -111,7 +113,7 @@ def replay(info, guidance, blur, sparse, norm):
     f64 = np.float64
     gate_wb, gate_sum = onp.affinity_normalization_2d(guidance.astype(f64), norm)
     raw = blur.astype(f64)
-    mask = None if sparse is None else np.sign(sparse.astype(f64))
+    mask = None if sparse is None else onp.sparse_mask(sparse, f64)
     H, W = raw.shape[-2:]
     cur = raw
     for p in info['passes']:
@@ -161,3 +163,86 @@ def test_replaying_the_plan_on_the_oracle_reproduces_the_untiled_result(H, W, n,
         out = replay_chained(cinfo, g, d, s, norm)
         assert not np.isnan(out).any()
         np.testing.assert_allclose(out, ref, rtol=1e-12, atol=1e-12)
+
+
+# ---- the forced-plan matrix of tests/test_forced_plans_gpu.py (tests/forced_plans.py), checked without a GPU ----------
+
+@pytest.mark.parametrize('index', range(len(fpl.CONFIGS) + 1))
+def test_forced_configuration_index_gives_the_pinned_menu(index, monkeypatch):
+    """configs() of cspn2d_cluster.cu is exactly the menu the forced-plan matrix covers: a configuration added there
+    fails here until tests/forced_plans.py covers it."""
+    monkeypatch.setenv('CSPN_B200_FORCE_CFG', str(index))
+    info = _lib.plan_info(37, 260, 7)
+    chained = _lib.plan_info(37, 260, 7, True)
+    if index == len(fpl.CONFIGS):
+        assert not info['supported'] and not chained['supported']
+        return
+    assert {(p['PR'], p['NW']) for p in info['passes']} == {fpl.CONFIGS[index]}
+    assert chained['supported'] == (index in fpl.CHAINED)
+
+
+@pytest.mark.parametrize('name', sorted(fpl.PROBLEMS))
+def test_forced_matrix_is_honoured_and_replays_on_the_oracle(name, monkeypatch):
+    """Every forced combination of the GPU matrix is a valid plan of the forced shape (the H100 can then only refuse it
+    through its occupancy query), and replaying it tile by tile reproduces the untiled result."""
+    pb = fpl.PROBLEMS[name]
+    rng = np.random.default_rng(pb.H + pb.n)
+    g = rng.standard_normal((1, 8, pb.H, pb.W))
+    d = rng.uniform(0, 10, (1, 1, pb.H, pb.W))
+    s = None
+    if pb.sparse:
+        s = rng.uniform(-1 if pb.sparse == 'signed' else 0, 10, (1, 1, pb.H, pb.W)) * (rng.uniform(size=d.shape) < 0.05)
+    ref = onp.cspn2d(g, d, s, pb.n, pb.norm, dtype=np.float64)
+    for plan in dict.fromkeys(pb.fwd + pb.bwd):
+        fpl.force(monkeypatch, plan)
+        info = check_plan(pb.H, pb.W, pb.n, fpl.chains(plan))
+        fpl.check_honoured(plan, info)
+        banded = any(len(p['bands']) > 1 for p in info['passes'])
+        assert banded == (plan.cs * fpl.rows(plan.cfg) < pb.H), plan
+        out = (replay_chained if fpl.chains(plan) else replay)(info, g, d, s, pb.norm)
+        np.testing.assert_allclose(out, ref, rtol=1e-12, atol=1e-12, err_msg=str(plan))
+
+
+def test_special_value_and_nan_patch_plans_are_honoured(monkeypatch):
+    cases = []
+    for name in fpl.SPECIAL:
+        c = load_golden(name)
+        H, W = c['blur'].shape[-2:]
+        cases.append((H, W, c['prop_time'], fpl.special_plans(name, H)))
+    cases += [(12, 16, n, fpl.NAN_PATCH_PLANS) for n in (1, 2, 3)]
+    for H, W, n, plans in cases:
+        for plan in plans:
+            fpl.force(monkeypatch, plan)
+            fpl.check_honoured(plan, check_plan(H, W, n))
+
+
+def test_forced_matrix_reaches_every_configuration_in_every_mode(monkeypatch):
+    """The axes every configuration must meet at least once (forward, chained, backward), read off the plans the planner
+    makes for the matrix."""
+    seen = {ci: set() for ci in range(len(fpl.CONFIGS))}
+    for pb in fpl.PROBLEMS.values():
+        for kind, plans in (('fwd', pb.fwd), ('bwd', pb.bwd)):
+            for plan in plans:
+                fpl.force(monkeypatch, plan)
+                info = fpl.plan_info(plan, pb.H, pb.W, pb.n)
+                n_pass = fpl.check_honoured(plan, info)
+                banded = any(len(p['bands']) > 1 for p in info['passes'])
+                unequal = len({p['iters'] for p in info['passes']}) > 1
+                tags = {f'cs{plan.cs}' if plan.cs in (1, 16) else 'cs_mid'}
+                tags |= {'banded'} if banded else ({'cs16_one_band'} if plan.cs == 16 else set())
+                tags |= {f'{n_pass}_unequal_passes'} if unequal else set()
+                tags |= {'bands_x_passes'} if banded and n_pass > 1 else set()
+                tags |= {'general'} if banded or n_pass > 1 else {'plain'}
+                tags |= {'strips'} if len(info['passes'][0]['strips']) > 1 else set()
+                tags |= {pb.norm, f'sparse_{pb.sparse}', f'C{pb.C}', f'gch{pb.gch}'}
+                if plan.chain:
+                    tags = {f'chained_{t}' for t in tags} if fpl.chains(plan) else {'chain_falls_back'}
+                seen[plan.cfg] |= {f'{kind}_{t}' for t in tags}
+    axes = {'cs1', 'cs_mid', 'cs16', 'cs16_one_band', 'banded', '2_unequal_passes', '3_unequal_passes', 'bands_x_passes',
+            'general', 'plain', 'strips', '8sum', '8sum_abs', 'sparse_signed', 'sparse_None', 'C2', 'gch9'}
+    fwd = {f'fwd_{a}' for a in axes}
+    bwd = {f'bwd_{a}' for a in ('cs1', 'cs_mid', 'cs16_one_band', 'banded', '3_unequal_passes', 'bands_x_passes', 'C2')}
+    chained = {'fwd_chained_cs1', 'fwd_chained_cs16', 'fwd_chained_2_unequal_passes', 'fwd_chained_8sum', 'fwd_chained_8sum_abs'}
+    for ci in seen:
+        need = fwd | bwd | (chained if ci in fpl.CHAINED else {'fwd_chain_falls_back'})
+        assert need <= seen[ci], (fpl.CONFIGS[ci], sorted(need - seen[ci]))

@@ -12,7 +12,7 @@ from oracle import cspn_numpy as onp, cspn_torch_port as tp
 
 def folded(guidance, sparse, norm):
     gate_wb, gate_sum = onp.affinity_normalization_2d(guidance, norm)          # w_k, s
-    m = np.zeros_like(gate_sum) if sparse is None else np.sign(sparse)
+    m = np.zeros_like(gate_sum) if sparse is None else onp.sparse_mask(sparse, sparse.dtype)
     return (1 - m) * gate_wb, (1 - m) * (1 - gate_sum) + m, m                  # w', kappa, m
 
 
