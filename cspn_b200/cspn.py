@@ -272,3 +272,121 @@ class Affinity_Propagate3D(nn.Module):
         if torch.is_grad_enabled() and (guidance.requires_grad or feat.requires_grad) and self.prop_time > 0:
             return _Propagate3dFn.apply(guidance, feat, self.prop_time, self.norm_type)
         return propagate3d(guidance, feat, self.prop_time, self.norm_type)
+
+
+# ---- 2D with a K x K affinity kernel (K in {3, 5, 7}) ----------------------------------------------------------------
+KERNEL_SIZES_2D = (3, 5, 7)
+
+
+def norm_code_2d_k(prop_kernel, norm_type=None):
+    """The norm names of a K x K kernel follow the 3D naming, f'{K*K-1}sum' / f'{K*K-1}sum_abs' ('8sum', '24sum',
+    '48sum', ...); returns the cspn_norm2d code (0 signed, 1 abs).  Raises AssertionError for another K or name."""
+    assert prop_kernel in KERNEL_SIZES_2D, f'prop_kernel must be 3, 5 or 7, got {prop_kernel}'
+    nt = prop_kernel * prop_kernel - 1
+    names = {f'{nt}sum': 0, f'{nt}sum_abs': 1}
+    norm_type = norm_type or f'{nt}sum'
+    assert norm_type in names, f'norm_type of a {prop_kernel}x{prop_kernel} kernel is one of {sorted(names)}, got {norm_type!r}'
+    return names[norm_type]
+
+
+def _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel):
+    nt = prop_kernel * prop_kernel - 1
+    if guidance.dim() == 4 and guidance.shape[1] < nt:
+        raise ValueError(f'a {prop_kernel}x{prop_kernel} kernel needs guidance (B,>={nt},H,W), got {tuple(guidance.shape)}')
+    _check_inputs_2d(guidance, blur_depth, sparse_depth)
+    if not (guidance.is_cuda and blur_depth.is_cuda):
+        raise _lib.CspnError(f'the {prop_kernel}x{prop_kernel} propagation takes CUDA tensors only '
+                             '(there is no host-buffer entry point for it)')
+
+
+def propagate2d_k(guidance, blur_depth, sparse_depth=None, prop_kernel=5, prop_time=24, norm_type=None, out=None):
+    """2D CSPN with a K x K affinity kernel, forward only (no autograd), CUDA tensors only, enqueued on the current stream.
+    guidance (B, >=K*K-1, H, W): channels 0..K*K-2 are used, shared by the C channels of blur_depth (B, C, H, W);
+    norm_type f'{K*K-1}sum' (default) or f'{K*K-1}sum_abs'.  K = 3 is propagate2d itself (same kernels, same bits)."""
+    code = norm_code_2d_k(prop_kernel, norm_type)
+    _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel)
+    if prop_kernel == 3:
+        return propagate2d(guidance, blur_depth, sparse_depth, prop_time, ('8sum', '8sum_abs')[code], ALGO_AUTO, out)
+    if prop_time == 0:
+        if out is None:
+            return blur_depth
+        _check_out(out, blur_depth, guidance, sparse_depth)
+        out.copy_(blur_depth)
+        return out
+    L = _lib.lib()
+    B, C, H, W = blur_depth.shape
+    g, d = guidance.contiguous(), blur_depth.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    if out is None:
+        out = torch.empty_like(d)
+    _check_out(out, d, g, s)
+    with torch.cuda.device(d.device):
+        ws_bytes = L.cspn2d_k_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+        rc = L.cspn2d_k_fwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(out), B, C, H, W, g.shape[1], prop_kernel, int(prop_time),
+                                code, _ptr(ws), ws_bytes, _stream(d.device))
+    _lib.check(rc, 'cspn2d_k_fwd_f32')
+    return out
+
+
+class _Propagate2dKFn(torch.autograd.Function):
+    """autograd seam of the K x K operator without the torch-op shim: native forward + native adjoint (cspn2d_k_bwd_f32)."""
+
+    @staticmethod
+    def forward(ctx, guidance, blur_depth, sparse_depth, prop_kernel, prop_time, norm_type):
+        ctx.save_for_backward(guidance, blur_depth, sparse_depth)
+        ctx.cfg = (prop_kernel, prop_time, norm_type)
+        return propagate2d_k(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, norm_type)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        guidance, blur_depth, sparse_depth = ctx.saved_tensors
+        prop_kernel, prop_time, norm_type = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        B, C, H, W = blur_depth.shape
+        g, d, go = guidance.contiguous(), blur_depth.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        need_g, need_d = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        gg = torch.empty_like(g) if need_g else None
+        gd = torch.empty_like(d) if need_d else None
+        with torch.cuda.device(d.device):
+            ws_bytes = L.cspn2d_k_bwd_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+            rc = L.cspn2d_k_bwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(go), _ptr(gg), _ptr(gd), B, C, H, W, g.shape[1],
+                                    prop_kernel, int(prop_time), norm_code_2d_k(prop_kernel, norm_type), _ptr(ws), ws_bytes,
+                                    _stream(d.device))
+        _lib.check(rc, 'cspn2d_k_bwd_f32')
+        return gg, gd, None, None, None, None
+
+
+class Affinity_PropagateK(nn.Module):
+    """2D CSPN with a K x K affinity kernel, K in {3, 5, 7}: Affinity_Propagate with K*K-1 neighbours instead of 8
+    (cspn.py with its pad tuples generalised; DESIGN.md section 4.8).  forward(guidance (B, >=K*K-1, H, W),
+    blur_depth (B, C, H, W), sparse_depth (B, 1, H, W) or None).  norm_type defaults to f'{K*K-1}sum'; the other is
+    f'{K*K-1}sum_abs'.  No parameters, no buffers; prop_time == 0 returns blur_depth itself.  Forward and backward run
+    in CUDA kernels (K = 3 in those of Affinity_Propagate, with the same bits)."""
+
+    def __init__(self, prop_time, prop_kernel, norm_type=None):
+        super().__init__()
+        norm_code_2d_k(prop_kernel, norm_type)      # AssertionError for K not in {3, 5, 7} or a name that does not match K
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+        self.norm_type = norm_type or f'{prop_kernel * prop_kernel - 1}sum'
+        self._use_op = _use_torch_op()
+
+    def forward(self, guidance, blur_depth, sparse_depth=None):
+        if self.prop_time == 0:
+            return blur_depth
+        sd = None if sparse_depth is None else sparse_depth.detach()
+        code = norm_code_2d_k(self.prop_kernel, self.norm_type)
+        if self._use_op and blur_depth.is_cuda:
+            return torch.ops.cspn_b200.propagate2d_k(guidance, blur_depth, sd, self.prop_kernel, self.prop_time, code)
+        if torch.is_grad_enabled() and (guidance.requires_grad or blur_depth.requires_grad):
+            return _Propagate2dKFn.apply(guidance, blur_depth, sd, self.prop_kernel, self.prop_time, self.norm_type)
+        return propagate2d_k(guidance, blur_depth, sparse_depth, self.prop_kernel, self.prop_time, self.norm_type)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'

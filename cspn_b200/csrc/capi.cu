@@ -176,6 +176,70 @@ int cspn2d_bwd_f32(const float* guidance, const float* blur, const float* sparse
     return rc;
 }
 
+// ---- K x K kernels: K = 3 is the operator above, K = 5 / 7 run in cspn2d_wide.cu ----------------------------------
+static bool kernel_size_ok(int K) { return K == 3 || K == 5 || K == 7; }
+
+static int check2d_k(const float* guidance, const float* blur, const void* out, int B, int C, int H, int W, int gch, int K,
+                     int iters, int norm_type) {
+    if (!guidance || !blur || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!kernel_size_ok(K)) { set_error("kernel size must be 3, 5 or 7, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (gch < K * K - 1) { set_error("a %dx%d kernel needs >= %d guidance channels, got %d", K, K, K * K - 1, gch); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (norm_type != CSPN_NORM_8SUM && norm_type != CSPN_NORM_8SUM_ABS) { set_error("unknown norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+size_t cspn2d_k_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
+    if (K == 3) return cspn2d_workspace_bytes(B, C, H, W, iters, CSPN_ALGO_AUTO);
+    return widek_workspace_bytes(B, C, H, W, K, iters);
+}
+
+int cspn2d_k_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out, int B, int C, int H, int W,
+                     int guidance_channels, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                     cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_k(guidance, blur, out, B, C, H, W, guidance_channels, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return cspn2d_fwd_f32(guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_AUTO,
+                              workspace, workspace_bytes, stream);
+    DeviceGuard guard(device_of(blur));
+    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    int launches = 0;
+    rc = widek_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn2d_k_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters < 0 || !kernel_size_ok(K)) return 0;
+    if (K == 3) return cspn2d_bwd_workspace_bytes(B, C, H, W, iters);
+    return widek_bwd_workspace_bytes(B, C, H, W, K, iters);
+}
+
+int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
+                     float* grad_guidance, float* grad_blur, int B, int C, int H, int W, int guidance_channels, int K,
+                     int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_k(guidance, blur, grad_out, B, C, H, W, guidance_channels, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return cspn2d_bwd_f32(guidance, blur, sparse, grad_out, grad_guidance, grad_blur, B, C, H, W, guidance_channels,
+                              iters, norm_type, workspace, workspace_bytes, stream);
+    DeviceGuard guard(device_of(blur));
+    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    int launches = 0;
+    rc = widek_backward(p, K, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
 size_t cspn3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
     if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0) return 0;
     return generic3d_workspace_bytes(B, C, D, H, W, iters);

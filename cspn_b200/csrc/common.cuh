@@ -78,6 +78,13 @@ size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters);
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
           size_t ws_bytes, cudaStream_t stream, int* launches);
 
+// K x K kernels, K in {5, 7} (cspn2d_wide.cu)
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
+                   size_t ws_bytes, cudaStream_t stream, int* launches);
+
 size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters);
 int generic3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W,
                       int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);

@@ -1,0 +1,414 @@
+// 2D CSPN with a K x K affinity kernel, K = 2R+1 in {5, 7} (K*K-1 = 24 / 48 neighbours), forward and backward.
+// The 3x3 operator keeps its own kernels (cspn2d_cluster.cu, cspn2d_generic.cu, cspn2d_bwd.cu); K = 3 is delegated to
+// them by the C ABI.
+//
+// Arithmetic: cspn2d_generic.cu with K*K-1 taps.  Tap k enumerates (t, l) over [0,K)^2 in raster order without the
+// centre (R, R) and reads the source at (dy, dx) = (R-t, R-l) (oracle/cspn_numpy_k.py::offsets_2d):
+//   a_k(p) = ghat_k(p + off_k) (0 outside),  w_k = a_k / sum_j |a_j|,  s = sum_k w_k,  m = sign(sparse)
+//   folded: w'_k = (1-m) w_k,  kappa = (1-m)(1-s) + m,   d_{t+1} = kappa d0 + sum_k w'_k shift_k(d_t).
+//
+// Why not the cluster kernel's design: it keeps 8 weights per pixel in registers for the whole run.  24 or 48 weights
+// per pixel do not fit (a KITTI image's 24 folded planes, ~41 MB, exceed the register file of the whole GPU), so this
+// path stores the folded weights (K*K planes per image, the last one kappa) and streams them once per step:
+//   prep    one launch per group of images: gather, normalise, fold the mask;
+//   step    one launch per step and group (grid z = image*channel).  The CTA stages its tile of d_t with an R-pixel halo
+//           in shared memory (zeros outside the image); each weight plane is read once per step, as LDG.128 when
+//           W % 4 == 0 and the pointers are 16-byte aligned (4 pixels of a row per thread), else one pixel per thread.
+//   groups  the launches cover the whole batch: one prep, then N steps.  (Splitting the batch into groups whose weight
+//           planes fit the L2 measured slower; see group_size.)
+// Backward, in the staged form of cspn2d_bwd.cu: prep, N-1 forward steps that keep d_1..d_{N-1}, N adjoint steps
+//   lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k) (lambda_{t+1} tile + halo in shared memory), and one
+//   gather-finalize kernel (Gw_k, Gc in registers, then the chain rule of cspn2d_bwd.cu with K*K-1 taps).
+#include <cstdlib>
+#include <cstring>
+
+#include "common.cuh"
+
+namespace cspn {
+
+namespace {
+
+template <int R>
+struct Taps {
+    static constexpr int K = 2 * R + 1;
+    static constexpr int NT = K * K - 1;   // neighbours
+    static constexpr int NP = K * K;       // planes per image in the workspace: w'_0..w'_{NT-1}, kappa
+    __host__ __device__ static constexpr int idx(int k) { return k >= NT / 2 ? k + 1 : k; }
+    __host__ __device__ static constexpr int dy(int k) { return R - idx(k) / K; }
+    __host__ __device__ static constexpr int dx(int k) { return R - idx(k) % K; }
+};
+
+__device__ __forceinline__ bool inside(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
+
+// ---- prep: prep2d_kernel with NT taps.  grid z = image of the group (pointers offset to the group) ----------------
+template <int R>
+__global__ void __launch_bounds__(256)
+prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ sparse, float* __restrict__ wk, int H, int W,
+             int gch, int norm_abs) {
+    using T = Taps<R>;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    const int b = blockIdx.z;
+    if (x >= W || y >= H) return;
+    const size_t HW = (size_t)H * W;
+    const float* g = guidance + (size_t)b * gch * HW;
+    float a[T::NT], S = 0.f;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        const int yy = y + T::dy(k), xx = x + T::dx(k);
+        float v = 0.f;
+        if (inside(yy, xx, H, W)) {
+            v = __ldg(g + k * HW + (size_t)yy * W + xx);
+            if (norm_abs) v = fabsf(v);
+        }
+        a[k] = v;
+        S += fabsf(v);
+    }
+    const size_t p = (size_t)y * W + x;
+    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    const float om = 1.f - m;
+    float s = 0.f;
+    float* o = wk + (size_t)b * T::NP * HW + p;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        const float w = __fdiv_rn(a[k], S);   // IEEE: 0/0 -> NaN, x/inf -> 0, subnormal S divides exactly
+        s += w;
+        o[k * HW] = om * w;
+    }
+    o[T::NT * HW] = om * (1.f - s) + m;
+}
+
+// ---- step, 4 pixels of a row per thread (W % 4 == 0, 16-byte aligned cur / d0 / dst / wk) -------------------------
+// Tile 64 x 16 pixels per CTA of 16 x 16 threads.  The shared tile holds rows y0-R .. y0+15+R and columns x0-4 ..
+// x0+67 as float4 (the halo is rounded up to 4 columns so every row of a thread's window is three aligned LDS.128).
+constexpr int kVecTW = 64, kVecTH = 16;
+
+template <int R>
+__global__ void __launch_bounds__(256)
+stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                 float* __restrict__ dst, int C, int H, int W) {
+    using T = Taps<R>;
+    constexpr int SH = kVecTH + 2 * R, SQ = kVecTW / 4 + 2;
+    __shared__ float4 tile[SH][SQ];
+    const int x0 = blockIdx.x * kVecTW, y0 = blockIdx.y * kVecTH, bc = blockIdx.z;
+    const size_t HW = (size_t)H * W;
+    const float* c = cur + (size_t)bc * HW;
+    for (int i = threadIdx.y * 16 + threadIdx.x; i < SH * SQ; i += 256) {
+        const int r = i / SQ, q = i % SQ;
+        const int gy = y0 - R + r, gx = x0 - 4 + 4 * q;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (inside(gy, gx, H, W)) v = __ldg(reinterpret_cast<const float4*>(c + (size_t)gy * W + gx));   // W % 4 == 0
+        tile[r][q] = v;
+    }
+    __syncthreads();
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const int x = x0 + 4 * tx, y = y0 + ty;
+    if (x >= W || y >= H) return;
+    const size_t p = (size_t)y * W + x;
+    const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
+    const float4 kap = __ldg(reinterpret_cast<const float4*>(w + T::NT * HW));
+    const float4 dd = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)bc * HW + p));
+    float acc0 = kap.x * dd.x, acc1 = kap.y * dd.y, acc2 = kap.z * dd.z, acc3 = kap.w * dd.w;
+#pragma unroll
+    for (int t = 0; t < T::K; ++t) {
+        const int r = ty + R + (R - t);                      // tile row of source row y + dy, dy = R - t
+        const float4 A = tile[r][tx], B = tile[r][tx + 1], Cq = tile[r][tx + 2];
+        const float row[12] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w, Cq.x, Cq.y, Cq.z, Cq.w};   // columns x-4 .. x+7
+#pragma unroll
+        for (int l = 0; l < T::K; ++l) {
+            if (t == R && l == R) continue;
+            const int k = t * T::K + l - (t * T::K + l > T::NT / 2 ? 1 : 0);
+            const int dx = R - l;
+            const float4 wv = __ldg(reinterpret_cast<const float4*>(w + k * HW));
+            acc0 = fmaf(wv.x, row[4 + dx], acc0);
+            acc1 = fmaf(wv.y, row[5 + dx], acc1);
+            acc2 = fmaf(wv.z, row[6 + dx], acc2);
+            acc3 = fmaf(wv.w, row[7 + dx], acc3);
+        }
+    }
+    *reinterpret_cast<float4*>(dst + (size_t)bc * HW + p) = make_float4(acc0, acc1, acc2, acc3);
+}
+
+// ---- step / adjoint, one pixel per thread (any W, any alignment).  Tile 32 x 8 pixels + R halo --------------------
+constexpr int kSclTW = 32, kSclTH = 8;
+
+template <int R>
+__device__ __forceinline__ void load_tile_scalar(float (*tile)[kSclTW + 2 * R], const float* __restrict__ src, int x0, int y0,
+                                                 int H, int W) {
+    constexpr int SH = kSclTH + 2 * R, SW = kSclTW + 2 * R;
+    for (int i = threadIdx.y * kSclTW + threadIdx.x; i < SH * SW; i += kSclTW * kSclTH) {
+        const int r = i / SW, q = i % SW;
+        const int gy = y0 - R + r, gx = x0 - R + q;
+        tile[r][q] = inside(gy, gx, H, W) ? __ldg(src + (size_t)gy * W + gx) : 0.f;
+    }
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                    float* __restrict__ dst, int C, int H, int W) {
+    using T = Taps<R>;
+    __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
+    const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, bc = blockIdx.z;
+    const size_t HW = (size_t)H * W;
+    load_tile_scalar<R>(tile, cur + (size_t)bc * HW, x0, y0, H, W);
+    __syncthreads();
+    const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
+    if (x >= W || y >= H) return;
+    const size_t p = (size_t)y * W + x;
+    const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
+    float acc = __ldg(w + T::NT * HW) * __ldg(d0 + (size_t)bc * HW + p);
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
+    dst[(size_t)bc * HW + p] = acc;
+}
+
+// lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only
+template <int R>
+__global__ void __launch_bounds__(256)
+adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out, int C, int H,
+            int W) {
+    using T = Taps<R>;
+    __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
+    const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, bc = blockIdx.z;
+    const size_t HW = (size_t)H * W;
+    load_tile_scalar<R>(tile, lam_in + (size_t)bc * HW, x0, y0, H, W);
+    __syncthreads();
+    const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
+    if (x >= W || y >= H) return;
+    const float* w = wk + (size_t)(bc / C) * T::NP * HW;
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        const int ys = y - T::dy(k), xs = x - T::dx(k);
+        if (inside(ys, xs, H, W))
+            acc = fmaf(__ldg(w + k * HW + (size_t)ys * W + xs), tile[ty + R - T::dy(k)][tx + R - T::dx(k)], acc);
+    }
+    lam_out[(size_t)bc * HW + (size_t)y * W + x] = acc;
+}
+
+// Gw_k(p) = sum_t lambda_{t+1}(p) d_t(p + off_k) with d_t staged tile by tile, Gc = sum_t lambda_{t+1}; then the finalize
+// arithmetic of cspn2d_bwd.cu.  steps[t] = d_{t+1}, lam[t] = lambda_t (planes n floats apart), lambda_N = grad_out.
+// grid z = image of the group; every pointer is offset to the group's first image.
+template <int R>
+__global__ void __launch_bounds__(256)
+gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+               const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
+               const float* __restrict__ grad_out, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+               long long n, int N, int C, int H, int W, int gch, int norm_abs) {
+    using T = Taps<R>;
+    __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
+    const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, b = blockIdx.z;
+    const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
+    const bool in = x < W && y < H;
+    const size_t HW = (size_t)H * W, p = in ? (size_t)y * W + x : 0;
+    float gw[T::NT];
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) gw[k] = 0.f;
+    const float kappa = in ? __ldg(wk + ((size_t)b * T::NP + T::NT) * HW + p) : 0.f;
+    float gkappa = 0.f;
+    for (int c = 0; c < C; ++c) {
+        const size_t plane = ((size_t)b * C + c) * HW;
+        float gc = 0.f;
+        for (int t = 0; t < N; ++t) {
+            __syncthreads();
+            load_tile_scalar<R>(tile, (t == 0 ? blur : steps + (size_t)(t - 1) * n) + plane, x0, y0, H, W);
+            __syncthreads();
+            if (!in) continue;
+            const float lp = __ldg((t == N - 1 ? grad_out : lam + (size_t)(t + 1) * n) + plane + p);
+            gc += lp;
+#pragma unroll
+            for (int k = 0; k < T::NT; ++k)   // taps outside the image take no gradient (they read the zero padding)
+                if (inside(y + T::dy(k), x + T::dx(k), H, W))
+                    gw[k] = fmaf(lp, tile[ty + R + T::dy(k)][tx + R + T::dx(k)], gw[k]);
+        }
+        if (!in) continue;
+        gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
+        if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
+    }
+    if (!in || !grad_guidance) return;
+    const float* g = guidance + (size_t)b * gch * HW;
+    float a[T::NT], S = 0.f;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        const int yy = y + T::dy(k), xx = x + T::dx(k);
+        float v = 0.f;
+        if (inside(yy, xx, H, W)) {
+            v = __ldg(g + k * HW + (size_t)yy * W + xx);
+            if (norm_abs) v = fabsf(v);
+        }
+        a[k] = v;
+        S += fabsf(v);
+    }
+    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    const float om = 1.f - m;
+    float Tsum = 0.f;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        gw[k] = om * (gw[k] - gkappa);                          // H_k = dL/dw_k
+        Tsum = fmaf(gw[k], __fdiv_rn(a[k], S), Tsum);
+    }
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        const int yy = y + T::dy(k), xx = x + T::dx(k);
+        if (inside(yy, xx, H, W)) {
+            const size_t q = (size_t)yy * W + xx;
+            const float ga = __fdiv_rn(gw[k] - signf(a[k]) * Tsum, S);
+            // d|g|/dg = sign(g) (0 at 0, like torch.abs) in the _abs norm
+            const float sg = norm_abs ? signf(__ldg(g + k * HW + q)) : 1.f;
+            grad_guidance[((size_t)b * gch + k) * HW + q] = ga * sg;
+        }
+    }
+}
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Images per launch group: the whole batch.  Groups sized so that their weight planes fit the L2 (steps 2..N reading
+// the weights from L2 instead of HBM) measured slower than one group on an H100 at 3 of the 4 shapes of
+// tools/time_kxk.py (DESIGN.md section 4.8), so they are not used.  CSPN_B200_KXK_GROUP=<images> splits the batch
+// (developer hook: the tests check that an image's bits do not depend on its group; time_kxk.py compares the two).
+int group_size(int B) {
+    if (const char* e = getenv("CSPN_B200_KXK_GROUP")) {
+        const int v = atoi(e);
+        if (v > 0) return v < B ? v : B;
+    }
+    return B;
+}
+
+template <int R>
+void launch_prep(const float* guidance, const float* sparse, float* wk, int nimg, int H, int W, int gch, int norm_abs,
+                 cudaStream_t s) {
+    prepk_kernel<R><<<dim3((W + 31) / 32, (H + 7) / 8, nimg), dim3(32, 8), 0, s>>>(guidance, sparse, wk, H, W, gch, norm_abs);
+}
+
+template <int R>
+void launch_step(bool vec, const float* wk, const float* d0, const float* cur, float* dst, int nbc, int C, int H, int W,
+                 cudaStream_t s) {
+    if (vec)
+        stepk_vec_kernel<R><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
+            wk, d0, cur, dst, C, H, W);
+    else
+        stepk_scalar_kernel<R><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
+            wk, d0, cur, dst, C, H, W);
+}
+
+template <int R>
+int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) {
+    constexpr int NP = Taps<R>::NP;
+    const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
+    float* wk_all = static_cast<float*>(ws);
+    float* tmp_all = wk_all + (size_t)p.B * NP * HW;
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(p.out) && aligned16(ws);
+    const int G = group_size(p.B);
+    for (int b0 = 0; b0 < p.B; b0 += G) {
+        const int nimg = p.B - b0 < G ? p.B - b0 : G;
+        float* wk = wk_all + (size_t)b0 * NP * HW;
+        const float* blur = p.blur + (size_t)b0 * plane;
+        float* out = p.out + (size_t)b0 * plane;
+        float* tmp = tmp_all + (size_t)b0 * plane;
+        launch_prep<R>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr, wk, nimg, p.H,
+                       p.W, p.gch, p.norm_abs, stream);
+        ++*launches;
+        const float* cur = blur;
+        float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
+        for (int it = 0; it < p.iters; ++it) {
+            launch_step<R>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
+            ++*launches;
+            cur = dst;
+            dst = (dst == out) ? tmp : out;
+        }
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
+template <int R>
+int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
+               cudaStream_t stream, int* launches) {
+    constexpr int NP = Taps<R>::NP;
+    const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
+    const long long n = (long long)p.B * plane;
+    float* wk_all = static_cast<float*>(ws);
+    float* steps = wk_all + (size_t)p.B * NP * HW;   // steps[t] = d_{t+1}, t < N-1
+    float* lam = steps + (size_t)p.iters * n;        // lam[t]   = lambda_t
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(ws);
+    const int G = group_size(p.B);
+    for (int b0 = 0; b0 < p.B; b0 += G) {
+        const int nimg = p.B - b0 < G ? p.B - b0 : G;
+        const size_t off = (size_t)b0 * plane;
+        float* wk = wk_all + (size_t)b0 * NP * HW;
+        const float* blur = p.blur + off;
+        const float* guidance = p.guidance + (size_t)b0 * p.gch * HW;
+        const float* sparse = p.sparse ? p.sparse + (size_t)b0 * HW : nullptr;
+        launch_prep<R>(guidance, sparse, wk, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+        ++*launches;
+        for (int t = 0; t + 1 < p.iters; ++t) {        // d_{t+1} = step(d_t)
+            launch_step<R>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
+                           nimg * p.C, p.C, p.H, p.W, stream);
+            ++*launches;
+        }
+        const dim3 grid((p.W + kSclTW - 1) / kSclTW, (p.H + kSclTH - 1) / kSclTH, nimg * p.C);
+        for (int t = p.iters - 1; t >= 0; --t) {        // lambda_t from lambda_{t+1}
+            const float* lin = (t == p.iters - 1 ? grad_out : lam + (size_t)(t + 1) * n) + off;
+            adjk_kernel<R><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lam + (size_t)t * n + off, p.C, p.H, p.W);
+            ++*launches;
+        }
+        gatherk_kernel<R><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
+            guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off,
+            grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr, grad_blur ? grad_blur + off : nullptr, n,
+            p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
+        ++*launches;
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
+}  // namespace
+
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (iters <= 0) return 0;
+    const size_t HW = (size_t)H * W;
+    return sizeof(float) * ((size_t)B * K * K * HW + (size_t)B * C * HW);
+}
+
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (iters <= 0) return 0;
+    const size_t HW = (size_t)H * W;
+    return sizeof(float) * ((size_t)B * K * K * HW + 2 * (size_t)iters * B * C * HW);
+}
+
+int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const size_t n = (size_t)p.B * p.C * p.H * p.W;
+    if (p.iters == 0) {
+        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
+    if (!ws || ws_bytes < need) {
+        set_error("%dx%d 2D path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
+    return K == 5 ? forward_k<2>(p, ws, stream, launches) : forward_k<3>(p, ws, stream, launches);
+}
+
+int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
+                   size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
+    if (grad_guidance)   // channels >= K*K-1 and taps that read the padding get zero gradient
+        CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
+    if (p.iters == 0) {
+        if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
+    if (!ws || ws_bytes < need) {
+        set_error("%dx%d 2D backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D backward: B*C exceeds gridDim.z", K, K); return CSPN_ERR_UNSUPPORTED; }
+    return K == 5 ? backward_k<2>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
+                  : backward_k<3>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+}
+
+}  // namespace cspn

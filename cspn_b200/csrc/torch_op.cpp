@@ -10,6 +10,10 @@
 //   propagate2d(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int prop_time, int norm_type, int algo) -> Tensor
 //   propagate2d_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int prop_time,
 //                        int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)
+//   propagate2d_k(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int kernel_size, int prop_time, int norm_type)
+//       -> Tensor                                                    (K x K kernel, K in {3, 5, 7}; K = 3 is propagate2d)
+//   propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size,
+//                          int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)
 //   propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor
 //   propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type,
 //                        bool need_guidance, bool need_feat) -> (Tensor, Tensor)
@@ -102,6 +106,59 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_backward_cuda(const at::Tensor& g
     return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
 }
 
+// K x K kernels: K = 3 is the 3x3 operator above (same kernels, same bits); K = 5 / 7 go through cspn2d_k_*_f32
+void check2d_k(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse, int64_t K) {
+    TORCH_CHECK(K == 3 || K == 5 || K == 7, "kernel_size must be 3, 5 or 7, got ", K);
+    check2d(guidance, blur, sparse);
+    TORCH_CHECK(guidance.size(1) >= K * K - 1, "a ", K, "x", K, " kernel needs guidance (B,>=", K * K - 1, ",H,W), got ",
+                guidance.sizes());
+}
+
+at::Tensor propagate2d_k_cuda(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                              int64_t K, int64_t prop_time, int64_t norm_type) {
+    check2d_k(guidance, blur, sparse, K);
+    if (K == 3) return propagate2d_cuda(guidance, blur, sparse, prop_time, norm_type, CSPN_ALGO_AUTO);
+    if (prop_time == 0) return blur.clone();
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(d);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const size_t ws_bytes = cspn2d_k_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
+    check_rc(cspn2d_k_fwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, out.data_ptr<float>(), B, C, H, W,
+                              (int)g.size(1), (int)K, (int)prop_time, (int)norm_type, ws_bytes ? ws.data_ptr() : nullptr,
+                              ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn2d_k_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> propagate2d_k_backward_cuda(const at::Tensor& guidance, const at::Tensor& blur,
+                                                               const std::optional<at::Tensor>& sparse, const at::Tensor& grad_out,
+                                                               int64_t K, int64_t prop_time, int64_t norm_type, bool need_g,
+                                                               bool need_d) {
+    check2d_k(guidance, blur, sparse, K);
+    if (K == 3) return propagate2d_backward_cuda(guidance, blur, sparse, grad_out, prop_time, norm_type, need_g, need_d);
+    TORCH_CHECK(grad_out.sizes() == blur.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == blur.device(),
+                "grad_out must match blur_depth");
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
+    at::Tensor gd = need_d ? at::empty_like(d) : at::Tensor();
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const size_t ws_bytes = cspn2d_k_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
+    check_rc(cspn2d_k_bwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
+                              need_d ? gd.data_ptr<float>() : nullptr, B, C, H, W, (int)g.size(1), (int)K, (int)prop_time,
+                              (int)norm_type, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
+                              (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn2d_k_bwd_f32");
+    return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
+}
+
 void check3d(const at::Tensor& guidance, const at::Tensor& feat) {
     TORCH_CHECK(guidance.dim() == 5 && feat.dim() == 5, "guidance and feat must be (B,C,D,H,W)");
     TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
@@ -159,6 +216,10 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate2d(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int prop_time, int norm_type, int algo) -> Tensor");
     m.def("propagate2d_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int prop_time, "
           "int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)");
+    m.def("propagate2d_k(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int kernel_size, int prop_time, "
+          "int norm_type) -> Tensor");
+    m.def("propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size, "
+          "int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)");
     m.def("propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor");
     m.def("propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -167,6 +228,8 @@ TORCH_LIBRARY(cspn_b200, m) {
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d", &propagate2d_cuda);
     m.impl("propagate2d_backward", &propagate2d_backward_cuda);
+    m.impl("propagate2d_k", &propagate2d_k_cuda);
+    m.impl("propagate2d_k_backward", &propagate2d_k_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);
     m.impl("propagate3d_backward", &propagate3d_backward_cuda);
 }

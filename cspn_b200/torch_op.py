@@ -53,6 +53,20 @@ def _register():
         gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
         return gg, gd
 
+    @lib.register_fake('cspn_b200::propagate2d_k')
+    def _(guidance, blur_depth, sparse_depth, kernel_size, prop_time, norm_type):
+        torch._check(guidance.dim() == 4 and blur_depth.dim() == 4, lambda: 'guidance and blur_depth must be (B,C,H,W)')
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        torch._check(guidance.shape[1] >= kernel_size * kernel_size - 1,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs >= {kernel_size * kernel_size - 1} guidance channels')
+        return torch.empty_like(blur_depth, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_k_backward')
+    def _(guidance, blur_depth, sparse_depth, grad_out, kernel_size, prop_time, norm_type, need_guidance, need_blur):
+        gg = torch.empty_like(guidance, memory_format=torch.contiguous_format) if need_guidance else guidance.new_empty(0)
+        gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
+        return gg, gd
+
     @lib.register_fake('cspn_b200::propagate3d')
     def _(guidance, feat, prop_time, norm_type):
         torch._check(guidance.dim() == 5 and feat.dim() == 5, lambda: 'guidance and feat must be (B,C,D,H,W)')
@@ -78,6 +92,21 @@ def _register():
         return (gg if need_g else None), (gd if need_d else None), None, None, None, None
 
     lib.register_autograd('cspn_b200::propagate2d', backward2d, setup_context=setup2d)
+
+    def setup2d_k(ctx, inputs, output):
+        guidance, blur_depth, sparse_depth, kernel_size, prop_time, norm_type = inputs
+        ctx.save_for_backward(guidance, blur_depth, sparse_depth)
+        ctx.cfg = (kernel_size, prop_time, norm_type)
+
+    def backward2d_k(ctx, grad_out):
+        guidance, blur_depth, sparse_depth = ctx.saved_tensors
+        kernel_size, prop_time, norm_type = ctx.cfg
+        need_g, need_d = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        gg, gd = torch.ops.cspn_b200.propagate2d_k_backward(guidance, blur_depth, sparse_depth, grad_out.contiguous(),
+                                                            kernel_size, prop_time, norm_type, need_g, need_d)
+        return (gg if need_g else None), (gd if need_d else None), None, None, None, None
+
+    lib.register_autograd('cspn_b200::propagate2d_k', backward2d_k, setup_context=setup2d_k)
 
     def setup3d(ctx, inputs, output):
         guidance, feat, prop_time, norm_type = inputs

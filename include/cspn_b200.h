@@ -114,6 +114,29 @@ CSPN_API int cspn2d_bwd_f32(const float* guidance, const float* blur, const floa
                    int B, int C, int H, int W, int guidance_channels, int iters, int norm_type,
                    void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D with a K x K affinity kernel, K in {3, 5, 7} (K*K-1 = 8, 24, 48 neighbours) ----------------------------
+ * cspn.py with its pad tuples generalised (DESIGN.md section 4.8): tap k enumerates (t, l) over [0,K)^2 in raster order
+ * without the centre and reads the source at (dy, dx) = ((K-1)/2 - t, (K-1)/2 - l).
+ * guidance [B][guidance_channels >= K*K-1][H][W] (channels 0..K*K-2 used, shared across the C channels of blur);
+ * blur / sparse / out / grad_* and norm_type (cspn_norm2d: 0 signed, 1 abs) as in the 3x3 calls above.
+ * K = 3 IS the 3x3 operator: the calls delegate to cspn2d_fwd_f32 (CSPN_ALGO_AUTO) / cspn2d_bwd_f32 and the workspace
+ * queries return theirs.  K = 5 / 7: forward workspace B*K*K*H*W + B*C*H*W floats, backward B*K*K*H*W + 2*iters*B*C*H*W
+ * floats (0 for iters == 0); the size does not depend on the device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5, 7},
+ * guidance_channels < K*K-1, an unknown norm, iters < 0, a non-positive shape or a null guidance / blur / out
+ * (grad_out in the backward; grad_guidance and grad_blur may be NULL). */
+CSPN_API size_t cspn2d_k_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_k_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out,
+                     int B, int C, int H, int W, int guidance_channels, int K, int iters, int norm_type,
+                     void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_k_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
+                     float* grad_guidance, float* grad_blur, int B, int C, int H, int W,
+                     int guidance_channels, int K, int iters, int norm_type,
+                     void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 3D: replaces CSPN.cspn(guide, feat) (cspn_paddle/demo.py:20-54) ------------------------
  * guidance [B][26][D][H][W], feat/out [B][C][D][H][W] (gate shared across C, cspn_paddle/README.md:56)
  */
