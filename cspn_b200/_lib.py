@@ -32,6 +32,10 @@ SIGNATURES = {
     'cspn3d_fwd_f32_host': (_i, [_vp] * 3 + [_i] * 8),
     'cspn3d_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn3d_bwd_f32': (_i, [_vp] * 5 + [_i] * 7 + [_vp, _sz, _vp]),
+    'cspn3d_k_workspace_bytes': (_sz, [_i] * 7),
+    'cspn3d_k_fwd_f32': (_i, [_vp] * 3 + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn3d_k_bwd_workspace_bytes': (_sz, [_i] * 7),
+    'cspn3d_k_bwd_f32': (_i, [_vp] * 5 + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn_depth_metrics_workspace_bytes': (_sz, []),
     'cspn_depth_metrics_f32': (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     'cspn_masked_l1_bwd_f32': (_i, [_vp] * 5 + [_sz, _vp]),

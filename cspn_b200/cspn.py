@@ -242,6 +242,18 @@ class _Propagate3dFn(torch.autograd.Function):
         return gg, gf, None, None
 
 
+def _per_channel_gate_views(guidance, feat, nt):
+    """Per-channel gates, the feat.shape[1] > 1 branch of CSPN.cspn (cspn_paddle/demo.py:28-45): with guidance
+    (B, nt*C, D, H, W), channel c of feat is propagated with guide channels [nt*c, nt*c+nt).  In memory that IS a batch of
+    B*C single-channel volumes with nt-channel gates, so the views returned cost nothing (contiguous inputs) and the same
+    kernels run.  None when the shapes are not of that form."""
+    if feat.dim() == 5 and guidance.dim() == 5 and feat.shape[1] > 1 and guidance.shape[1] == nt * feat.shape[1]:
+        B, C = feat.shape[:2]
+        return (guidance.contiguous().view(B * C, nt, *guidance.shape[2:]),
+                feat.contiguous().view(B * C, 1, *feat.shape[2:]))
+    return None
+
+
 class Affinity_Propagate3D(nn.Module):
     """3D (3x3x3, 26 neighbours) counterpart; the reference has only call sites for it
     (cspn_paddle/demo.py:20-54: CSPN.cspn(guide, feat)).  norm_type:
@@ -259,14 +271,9 @@ class Affinity_Propagate3D(nn.Module):
         self._use_op = _use_torch_op()
 
     def forward(self, guidance, feat):
-        if feat.dim() == 5 and guidance.dim() == 5 and feat.shape[1] > 1 and guidance.shape[1] == 26 * feat.shape[1]:
-            # per-channel gates, the feat.shape[1] > 1 branch of CSPN.cspn (cspn_paddle/demo.py:28-45): channel c of feat is
-            # propagated with guide channels [26c, 26c+26).  In memory that IS a batch of B*C single-channel volumes with
-            # 26-channel gates, so the views below cost nothing (contiguous inputs) and the same kernels run.
-            B, C = feat.shape[:2]
-            out = self.forward(guidance.contiguous().view(B * C, 26, *guidance.shape[2:]),
-                               feat.contiguous().view(B * C, 1, *feat.shape[2:]))
-            return out.view(feat.shape)
+        views = _per_channel_gate_views(guidance, feat, 26)
+        if views is not None:
+            return self.forward(*views).view(feat.shape)
         if self._use_op and feat.is_cuda and self.prop_time > 0:
             return torch.ops.cspn_b200.propagate3d(guidance, feat, self.prop_time, NORM3D[self.norm_type])
         if torch.is_grad_enabled() and (guidance.requires_grad or feat.requires_grad) and self.prop_time > 0:
@@ -387,6 +394,126 @@ class Affinity_PropagateK(nn.Module):
         if torch.is_grad_enabled() and (guidance.requires_grad or blur_depth.requires_grad):
             return _Propagate2dKFn.apply(guidance, blur_depth, sd, self.prop_kernel, self.prop_time, self.norm_type)
         return propagate2d_k(guidance, blur_depth, sparse_depth, self.prop_kernel, self.prop_time, self.norm_type)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'
+
+
+# ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
+KERNEL_SIZES_3D = (3, 5)
+
+
+def norm_code_3d_k(prop_kernel, norm_type=None):
+    """The norm names of a K x K x K kernel follow the 3D naming, f'{K**3-1}sum' / f'{K**3-1}sum_abs' ('26sum', '124sum',
+    ...) and 'paddle'; returns the cspn_norm3d code (0 signed, 1 abs, 2 paddle).  The default is f'{K**3-1}sum_abs', as in
+    Affinity_Propagate3D.  Raises AssertionError for another K or name."""
+    assert prop_kernel in KERNEL_SIZES_3D, f'prop_kernel must be 3 or 5 in 3D, got {prop_kernel}'
+    nt = prop_kernel ** 3 - 1
+    names = {f'{nt}sum': 0, f'{nt}sum_abs': 1, 'paddle': 2}
+    norm_type = norm_type or f'{nt}sum_abs'
+    assert norm_type in names, (f'norm_type of a {prop_kernel}x{prop_kernel}x{prop_kernel} kernel is one of {sorted(names)}, '
+                                f'got {norm_type!r}')
+    return names[norm_type]
+
+
+def _check_shapes_3d_k(guidance, feat, prop_kernel):
+    nt = prop_kernel ** 3 - 1
+    if guidance.dim() != 5 or feat.dim() != 5:
+        raise ValueError('guidance and feat must be (B,C,D,H,W)')
+    if guidance.dtype != torch.float32 or feat.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    B, C, D, H, W = feat.shape
+    if guidance.shape != (B, nt, D, H, W):
+        raise ValueError(f'a {prop_kernel}x{prop_kernel}x{prop_kernel} kernel needs guidance (B,{nt},D,H,W) or, with C > 1 '
+                         f'feature channels, (B,{nt}*C,D,H,W); got {tuple(guidance.shape)} for feat {tuple(feat.shape)}')
+    if guidance.device != feat.device:
+        raise RuntimeError('guidance and feat are on different devices')
+
+
+def propagate3d_k(guidance, feat, prop_kernel=5, prop_time=12, norm_type=None):
+    """3D CSPN with a K x K x K affinity kernel, forward only (no autograd), CUDA tensors only, enqueued on the current
+    stream.  guidance (B, K**3-1, D, H, W), one gate shared by the C channels of feat (B, C, D, H, W); norm_type
+    f'{K**3-1}sum', f'{K**3-1}sum_abs' (default) or 'paddle'.  K = 3 is propagate3d itself (same kernels, same bits)."""
+    code = norm_code_3d_k(prop_kernel, norm_type)
+    _check_shapes_3d_k(guidance, feat, prop_kernel)
+    if not (guidance.is_cuda and feat.is_cuda):
+        raise _lib.CspnError(f'the {prop_kernel}x{prop_kernel}x{prop_kernel} propagation takes CUDA tensors only '
+                             '(there is no host-buffer entry point for it)')
+    if prop_time == 0:
+        return feat
+    if prop_kernel == 3:
+        return propagate3d(guidance, feat, prop_time, ('26sum', '26sum_abs', 'paddle')[code])
+    L = _lib.lib()
+    B, C, D, H, W = feat.shape
+    g, f = guidance.contiguous(), feat.contiguous()
+    out = torch.empty_like(f)
+    with torch.cuda.device(f.device):
+        ws_bytes = L.cspn3d_k_workspace_bytes(B, C, D, H, W, prop_kernel, int(prop_time))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+        rc = L.cspn3d_k_fwd_f32(_ptr(g), _ptr(f), _ptr(out), B, C, D, H, W, prop_kernel, int(prop_time), code, _ptr(ws),
+                                ws_bytes, _stream(f.device))
+    _lib.check(rc, 'cspn3d_k_fwd_f32')
+    return out
+
+
+class _Propagate3dKFn(torch.autograd.Function):
+    """autograd seam of the K x K x K operator without the torch-op shim: native forward + native adjoint (cspn3d_k_bwd_f32)."""
+
+    @staticmethod
+    def forward(ctx, guidance, feat, prop_kernel, prop_time, norm_type):
+        ctx.save_for_backward(guidance, feat)
+        ctx.cfg = (prop_kernel, prop_time, norm_type)
+        return propagate3d_k(guidance, feat, prop_kernel, prop_time, norm_type)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        guidance, feat = ctx.saved_tensors
+        prop_kernel, prop_time, norm_type = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        B, C, D, H, W = feat.shape
+        g, f, go = guidance.contiguous(), feat.contiguous(), grad_out.contiguous()
+        gg = torch.empty_like(g) if ctx.needs_input_grad[0] else None
+        gf = torch.empty_like(f) if ctx.needs_input_grad[1] else None
+        with torch.cuda.device(f.device):
+            ws_bytes = L.cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, prop_kernel, int(prop_time))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+            rc = L.cspn3d_k_bwd_f32(_ptr(g), _ptr(f), _ptr(go), _ptr(gg), _ptr(gf), B, C, D, H, W, prop_kernel, int(prop_time),
+                                    norm_code_3d_k(prop_kernel, norm_type), _ptr(ws), ws_bytes, _stream(f.device))
+        _lib.check(rc, 'cspn3d_k_bwd_f32')
+        return gg, gf, None, None, None
+
+
+class Affinity_Propagate3DK(nn.Module):
+    """3D CSPN with a K x K x K affinity kernel, K in {3, 5}: Affinity_Propagate3D with K**3-1 neighbours instead of 26
+    (DESIGN.md section 4.9).  forward(guidance, feat (B, C, D, H, W)): guidance is (B, K**3-1, D, H, W), one gate shared by
+    the C channels, or (B, (K**3-1)*C, D, H, W) with C > 1, one gate per channel (cspn_paddle/demo.py:28-45).  norm_type
+    defaults to f'{K**3-1}sum_abs'; the others are f'{K**3-1}sum' and 'paddle'.  No parameters, no buffers; prop_time == 0
+    returns feat itself.  Forward and backward run in CUDA kernels (K = 3 in those of Affinity_Propagate3D, same bits)."""
+
+    def __init__(self, prop_time, prop_kernel, norm_type=None):
+        super().__init__()
+        norm_code_3d_k(prop_kernel, norm_type)      # AssertionError for K not in {3, 5} or a name that does not match K
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+        self.norm_type = norm_type or f'{prop_kernel ** 3 - 1}sum_abs'
+        self._use_op = _use_torch_op()
+
+    def forward(self, guidance, feat):
+        if self.prop_time == 0:
+            return feat
+        views = _per_channel_gate_views(guidance, feat, self.prop_kernel ** 3 - 1)
+        if views is not None:
+            return self.forward(*views).view(feat.shape)
+        _check_shapes_3d_k(guidance, feat, self.prop_kernel)
+        code = norm_code_3d_k(self.prop_kernel, self.norm_type)
+        if self._use_op and feat.is_cuda:
+            return torch.ops.cspn_b200.propagate3d_k(guidance, feat, self.prop_kernel, self.prop_time, code)
+        if torch.is_grad_enabled() and (guidance.requires_grad or feat.requires_grad):
+            return _Propagate3dKFn.apply(guidance, feat, self.prop_kernel, self.prop_time, self.norm_type)
+        return propagate3d_k(guidance, feat, self.prop_kernel, self.prop_time, self.norm_type)
 
     def extra_repr(self):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'

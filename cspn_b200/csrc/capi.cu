@@ -284,6 +284,64 @@ int cspn3d_bwd_f32(const float* guidance, const float* feat, const float* grad_o
     return rc;
 }
 
+// ---- K x K x K kernels: K = 3 is the 3D operator above, K = 5 runs in cspn3d_wide.cu ------------------------------
+static int check3d_k(const float* guidance, const float* feat, const void* out, int B, int C, int D, int H, int W, int K,
+                     int iters, int norm_type) {
+    if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d D=%d H=%d W=%d", B, C, D, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (K != 3 && K != 5) { set_error("3D kernel size must be 3 or 5, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (norm_type < CSPN_NORM_26SUM || norm_type > CSPN_NORM_PADDLE) { set_error("unknown 3D norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+size_t cspn3d_k_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
+    if (K == 3) return cspn3d_workspace_bytes(B, C, D, H, W, iters);
+    return widek3d_workspace_bytes(B, C, D, H, W, K, iters);
+}
+
+int cspn3d_k_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
+                     int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check3d_k(guidance, feat, out, B, C, D, H, W, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3) return cspn3d_fwd_f32(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, norm_type, workspace, workspace_bytes, (cudaStream_t)stream,
+                         &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn3d_k_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
+    if (K == 3) return cspn3d_bwd_workspace_bytes(B, C, D, H, W, iters);
+    return widek3d_bwd_workspace_bytes(C, D, H, W, K, iters);
+}
+
+int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
+                     int B, int C, int D, int H, int W, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                     cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check3d_k(guidance, feat, grad_out, B, C, D, H, W, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return cspn3d_bwd_f32(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace,
+                              workspace_bytes, stream);
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = widek3d_backward(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, K, iters, norm_type, workspace,
+                          workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

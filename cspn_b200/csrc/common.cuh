@@ -85,6 +85,8 @@ size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                    size_t ws_bytes, cudaStream_t stream, int* launches);
 
+// volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
+int group3d(int B, int C, int D, int H, int W, int iters, int planes);
 size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters);
 int generic3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W,
                       int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
@@ -92,5 +94,14 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
 size_t bwd3d_workspace_bytes(int C, int D, int H, int W, int iters);
 int bwd3d(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat, int B, int C,
           int D, int H, int W, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+
+// K x K x K kernels, K = 5 (cspn3d_wide.cu)
+size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
+                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters);
+int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
+                     int D, int H, int W, int K, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream,
+                     int* launches);
 
 }  // namespace cspn

@@ -308,11 +308,12 @@ step3d_gather_vec4_kernel(const float* __restrict__ g, const float* __restrict__
 
 }  // namespace
 
-// Volumes per launch group: as many as keep the group's workspace under kMaxWorkspace3d (and gridDim.z legal).
+// Volumes per launch group: as many as keep the group's workspace (`planes` weight planes per volume plus the ping-pong
+// buffer) under kMaxWorkspace3d (and gridDim.z legal).  27 planes here, K^3 in cspn3d_wide.cu.
 constexpr size_t kMaxWorkspace3d = (size_t)4 << 30;
-static int group3d(int B, int C, int D, int H, int W, int iters) {
+int group3d(int B, int C, int D, int H, int W, int iters, int planes) {
     const size_t V = (size_t)D * H * W;
-    const size_t per_vol = sizeof(float) * (27 * V + (iters > 1 ? (size_t)C * V : 0));
+    const size_t per_vol = sizeof(float) * ((size_t)planes * V + (iters > 1 ? (size_t)C * V : 0));
     size_t cap = kMaxWorkspace3d;
     if (const char* e = getenv("CSPN_B200_MAX_WS3D_KB"))   // developer hook: tests force small / ragged groups
         if (atof(e) > 0) cap = (size_t)(atof(e) * 1024.0);
@@ -326,7 +327,7 @@ static int group3d(int B, int C, int D, int H, int W, int iters) {
 size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
     if (iters <= 0) return 0;
     const size_t V = (size_t)D * H * W;
-    return sizeof(float) * (size_t)group3d(B, C, D, H, W, iters) * (27 * V + (iters > 1 ? (size_t)C * V : 0));
+    return sizeof(float) * (size_t)group3d(B, C, D, H, W, iters, 27) * (27 * V + (iters > 1 ? (size_t)C * V : 0));
 }
 
 int generic3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W,
@@ -368,7 +369,7 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
         CSPN_CUDA_TRY(cudaGetLastError());
         return CSPN_OK;
     }
-    const int G = group3d(B, C, D, H, W, iters);
+    const int G = group3d(B, C, D, H, W, iters, 27);
     float* wk = static_cast<float*>(ws);          // [G][27][V]
     float* tmp = wk + (size_t)G * 27 * V;         // [G][C][V]
     const dim3 block(32, 8);

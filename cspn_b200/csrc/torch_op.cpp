@@ -17,6 +17,10 @@
 //   propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor
 //   propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type,
 //                        bool need_guidance, bool need_feat) -> (Tensor, Tensor)
+//   propagate3d_k(Tensor guidance, Tensor feat, int kernel_size, int prop_time, int norm_type) -> Tensor
+//       (K x K x K kernel, K in {3, 5}; K = 3 is propagate3d)
+//   propagate3d_k_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, int norm_type,
+//                          bool need_guidance, bool need_feat) -> (Tensor, Tensor)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -210,6 +214,58 @@ std::tuple<at::Tensor, at::Tensor> propagate3d_backward_cuda(const at::Tensor& g
     return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
 }
 
+// K x K x K kernels: K = 3 is the 3D operator above (same kernels, same bits); K = 5 goes through cspn3d_k_*_f32
+void check3d_k(const at::Tensor& guidance, const at::Tensor& feat, int64_t K) {
+    TORCH_CHECK_VALUE(K == 3 || K == 5, "3D kernel_size must be 3 or 5, got ", K);
+    TORCH_CHECK_VALUE(guidance.dim() == 5 && feat.dim() == 5, "guidance and feat must be (B,C,D,H,W)");
+    TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    const int64_t nt = K * K * K - 1;
+    TORCH_CHECK_VALUE(guidance.size(0) == feat.size(0) && guidance.size(1) == nt && guidance.size(2) == feat.size(2) &&
+                          guidance.size(3) == feat.size(3) && guidance.size(4) == feat.size(4),
+                      "a ", K, "x", K, "x", K, " kernel needs guidance (B,", nt, ",D,H,W), got ", guidance.sizes(), " for feat ",
+                      feat.sizes());
+    TORCH_CHECK(guidance.device() == feat.device(), "guidance and feat are on different devices");
+}
+
+at::Tensor propagate3d_k_cuda(const at::Tensor& guidance, const at::Tensor& feat, int64_t K, int64_t prop_time, int64_t norm_type) {
+    check3d_k(guidance, feat, K);
+    if (K == 3) return propagate3d_cuda(guidance, feat, prop_time, norm_type);
+    if (prop_time == 0) return feat.clone();
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor g = guidance.contiguous(), f = feat.contiguous();
+    at::Tensor out = at::empty_like(f);
+    const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
+    const size_t ws_bytes = cspn3d_k_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
+    check_rc(cspn3d_k_fwd_f32(fptr(g), fptr(f), out.data_ptr<float>(), B, C, D, H, W, (int)K, (int)prop_time, (int)norm_type,
+                              ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn3d_k_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> propagate3d_k_backward_cuda(const at::Tensor& guidance, const at::Tensor& feat,
+                                                               const at::Tensor& grad_out, int64_t K, int64_t prop_time,
+                                                               int64_t norm_type, bool need_g, bool need_f) {
+    check3d_k(guidance, feat, K);
+    if (K == 3) return propagate3d_backward_cuda(guidance, feat, grad_out, prop_time, norm_type, need_g, need_f);
+    TORCH_CHECK(grad_out.sizes() == feat.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == feat.device(),
+                "grad_out must match feat");
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor g = guidance.contiguous(), f = feat.contiguous(), go = grad_out.contiguous();
+    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
+    at::Tensor gf = need_f ? at::empty_like(f) : at::Tensor();
+    const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
+    const size_t ws_bytes = cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
+    check_rc(cspn3d_k_bwd_f32(fptr(g), fptr(f), fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
+                              need_f ? gf.data_ptr<float>() : nullptr, B, C, D, H, W, (int)K, (int)prop_time, (int)norm_type,
+                              ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn3d_k_bwd_f32");
+    return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -223,6 +279,9 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor");
     m.def("propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
+    m.def("propagate3d_k(Tensor guidance, Tensor feat, int kernel_size, int prop_time, int norm_type) -> Tensor");
+    m.def("propagate3d_k_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, int norm_type, "
+          "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -232,4 +291,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_k_backward", &propagate2d_k_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);
     m.impl("propagate3d_backward", &propagate3d_backward_cuda);
+    m.impl("propagate3d_k", &propagate3d_k_cuda);
+    m.impl("propagate3d_k_backward", &propagate3d_k_backward_cuda);
 }

@@ -78,6 +78,20 @@ def _register():
         gf = torch.empty_like(feat, memory_format=torch.contiguous_format) if need_feat else feat.new_empty(0)
         return gg, gf
 
+    @lib.register_fake('cspn_b200::propagate3d_k')
+    def _(guidance, feat, kernel_size, prop_time, norm_type):
+        torch._check(guidance.dim() == 5 and feat.dim() == 5, lambda: 'guidance and feat must be (B,C,D,H,W)')
+        torch._check(kernel_size in (3, 5), lambda: '3D kernel_size must be 3 or 5')
+        torch._check(guidance.shape[1] == kernel_size ** 3 - 1,
+                     lambda: f'a {kernel_size}x{kernel_size}x{kernel_size} kernel needs {kernel_size ** 3 - 1} guidance channels')
+        return torch.empty_like(feat, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate3d_k_backward')
+    def _(guidance, feat, grad_out, kernel_size, prop_time, norm_type, need_guidance, need_feat):
+        gg = torch.empty_like(guidance, memory_format=torch.contiguous_format) if need_guidance else guidance.new_empty(0)
+        gf = torch.empty_like(feat, memory_format=torch.contiguous_format) if need_feat else feat.new_empty(0)
+        return gg, gf
+
     def setup2d(ctx, inputs, output):
         guidance, blur_depth, sparse_depth, prop_time, norm_type, algo = inputs
         ctx.save_for_backward(guidance, blur_depth, sparse_depth)
@@ -122,6 +136,21 @@ def _register():
         return (gg if need_g else None), (gf if need_f else None), None, None
 
     lib.register_autograd('cspn_b200::propagate3d', backward3d, setup_context=setup3d)
+
+    def setup3d_k(ctx, inputs, output):
+        guidance, feat, kernel_size, prop_time, norm_type = inputs
+        ctx.save_for_backward(guidance, feat)
+        ctx.cfg = (kernel_size, prop_time, norm_type)
+
+    def backward3d_k(ctx, grad_out):
+        guidance, feat = ctx.saved_tensors
+        kernel_size, prop_time, norm_type = ctx.cfg
+        need_g, need_f = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        gg, gf = torch.ops.cspn_b200.propagate3d_k_backward(guidance, feat, grad_out.contiguous(), kernel_size, prop_time,
+                                                            norm_type, need_g, need_f)
+        return (gg if need_g else None), (gf if need_f else None), None, None, None
+
+    lib.register_autograd('cspn_b200::propagate3d_k', backward3d_k, setup_context=setup3d_k)
 
 
 def propagate2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum', algo=_lib.ALGO_AUTO):

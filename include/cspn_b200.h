@@ -158,6 +158,30 @@ CSPN_API int cspn3d_bwd_f32(const float* guidance, const float* feat, const floa
                    int B, int C, int D, int H, int W, int iters, int norm_type,
                    void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 3D with a K x K x K affinity kernel, K in {3, 5} (K^3-1 = 26, 124 neighbours) ---------------------------------
+ * Tap k enumerates (f, t, l) over [0,K)^3 in raster order without the centre and reads the source at
+ * (dz, dy, dx) = ((K-1)/2 - f, (K-1)/2 - t, (K-1)/2 - l) (DESIGN.md section 4.9).
+ * guidance [B][K^3-1][D][H][W] (one gate shared by the C channels of feat), feat / out / grad_* [B][C][D][H][W];
+ * norm_type is a cspn_norm3d (0 gathered signed, 1 gathered abs, 2 own-location 'paddle').
+ * K = 3 IS the 3D operator: the calls delegate to cspn3d_fwd_f32 / cspn3d_bwd_f32 and the workspace queries return theirs.
+ * K = 5: forward workspace G*(125 + (iters > 1 ? C : 0))*D*H*W floats, with G the volumes per launch group (all B unless
+ * that exceeds 4 GiB or gridDim.z); backward (125 + (2*iters-1)*C)*D*H*W floats; 0 for iters == 0; neither depends on the
+ * device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5}, an unknown norm, iters < 0, a non-positive shape or a null
+ * guidance / feat / out (grad_out in the backward; grad_guidance and grad_feat may be NULL).  CSPN_ERR_UNSUPPORTED for a
+ * shape the launch grid cannot take (D*C > 65535). */
+CSPN_API size_t cspn3d_k_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+
+CSPN_API int cspn3d_k_fwd_f32(const float* guidance, const float* feat, float* out,
+                     int B, int C, int D, int H, int W, int K, int iters, int norm_type,
+                     void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn3d_k_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+
+CSPN_API int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const float* grad_out,
+                     float* grad_guidance, float* grad_feat,
+                     int B, int C, int D, int H, int W, int K, int iters, int norm_type,
+                     void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):

@@ -42,3 +42,18 @@ g3.requires_grad_(True); f3.requires_grad_(True)
 cspn_b200.Affinity_Propagate3D(3, 3, '26sum_abs')(g3, f3).sum().backward()
 torch.cuda.synchronize()
 print('3D fwd+bwd', float(g3.grad.abs().sum()), float(f3.grad.sum()), flush=True)
+
+# 5x5x5 kernels (cspn3d_wide.cu): every norm, direct / vectorised and scalar paths, forward and backward
+for mode in ('124sum', '124sum_abs', 'paddle'):
+    for W in (16, 13):
+        g5 = torch.rand(2, 124, 5, 7, W, device='cuda')
+        f5 = torch.rand(2, 2, 5, 7, W, device='cuda')
+        out = cspn_b200.propagate3d_k(g5, f5, 5, 3, mode)
+        torch.cuda.synchronize()
+        print('3D 5x5x5', mode, W, _lib.lib().cspn_last_launches(), float(out.sum()), flush=True)
+        g5.requires_grad_(True); f5.requires_grad_(True)
+        m = cspn_b200.Affinity_Propagate3DK(3, 5, mode)
+        m._use_op = False
+        m(g5, f5).sum().backward()
+        torch.cuda.synchronize()
+        print('3D 5x5x5 fwd+bwd', mode, W, float(g5.grad.abs().sum()), float(f5.grad.sum()), flush=True)
