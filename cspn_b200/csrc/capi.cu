@@ -52,9 +52,9 @@ int check2d(const float* guidance, const float* blur, float* out, int B, int C, 
 }
 
 // Picks the algorithm actually run for `algo` on this problem.  AUTO prefers the cluster kernel.
-int resolve_algo(const Problem2D& p, int algo, char* why, int why_len) {
+int resolve_algo(const Problem2D& p, int algo, char* why, int why_len, const void* ws = nullptr) {
     if (algo == CSPN_ALGO_GENERIC) return CSPN_ALGO_GENERIC;
-    if (cluster2d_supported(p, why, why_len)) return CSPN_ALGO_CLUSTER;
+    if (cluster2d_supported(p, why, why_len, ws)) return CSPN_ALGO_CLUSTER;
     return algo == CSPN_ALGO_CLUSTER ? (int)CSPN_ERR_UNSUPPORTED : (int)CSPN_ALGO_GENERIC;
 }
 
@@ -105,7 +105,7 @@ int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse
     if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
     Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
     char why[256] = "";
-    const int chosen = (iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why));
+    const int chosen = (iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why), workspace);
     if (chosen < 0) { set_error("cluster kernel unsupported for this problem: %s", why); return chosen; }
     g_last_algo = chosen;
     int launches = 0;
@@ -115,7 +115,7 @@ int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse
         const size_t need = generic2d_workspace_bytes(B, C, H, W, iters);
         if (!workspace || workspace_bytes < need) {
             set_error("CSPN_ALGO_AUTO falls back to the generic path here (%s), which needs %zu workspace bytes (got %zu): "
-                      "query cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors",
+                      "query cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors and workspace",
                       why[0] ? why : "cluster kernel declined", need, workspace ? workspace_bytes : (size_t)0);
             return CSPN_ERR_WORKSPACE;
         }
@@ -142,7 +142,7 @@ int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, const float*
     if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
     Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
     char why[256] = "";
-    if (!cluster2d_supported(p, why, sizeof(why))) {
+    if (!cluster2d_supported(p, why, sizeof(why), workspace)) {
         set_error("the fused gather runs in the cluster kernel's epilogue, which cannot take this problem: %s", why);
         return CSPN_ERR_UNSUPPORTED;
     }

@@ -58,7 +58,9 @@ struct Problem2D {
 size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters);
 int generic2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 
-bool cluster2d_supported(const Problem2D& p, char* why, int why_len);
+// ws: the caller's workspace (nullptr when not known yet); a plan of several passes keeps its intermediate result there
+// with float4 stores and loads, so it declines a workspace that is not 16-byte aligned
+bool cluster2d_supported(const Problem2D& p, char* why, int why_len, const void* ws = nullptr);
 size_t cluster2d_workspace_bytes(int B, int C, int H, int W, int iters);
 // peer_out / mc_out: additional destinations of the final result (fused gather), see cspn2d_fwd_gather_f32
 int cluster2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,

@@ -1283,7 +1283,7 @@ extern "C" __attribute__((visibility("default"))) void cspn_debug_set_trace(void
 extern "C" __attribute__((visibility("default"))) int cspn_debug_trace_events() { return kTraceEvents; }
 #endif
 
-bool cluster2d_supported(const Problem2D& p, char* why, int why_len) {
+bool cluster2d_supported(const Problem2D& p, char* why, int why_len, const void* ws) {
     if (p.iters <= 0) { snprintf(why, why_len, "iters == 0"); return false; }
     if ((reinterpret_cast<uintptr_t>(p.guidance) | reinterpret_cast<uintptr_t>(p.blur) | reinterpret_cast<uintptr_t>(p.sparse) |
          reinterpret_cast<uintptr_t>(p.out)) & 15) {
@@ -1295,6 +1295,11 @@ bool cluster2d_supported(const Problem2D& p, char* why, int why_len) {
     std::lock_guard<std::mutex> lock(g_mu);
     Plan plan;
     if (!make_plan(p.H, p.W, p.iters, dev, plan, why, why_len)) return false;
+    if (plan.n_pass > 1 && (reinterpret_cast<uintptr_t>(ws) & 15)) {
+        snprintf(why, why_len, "%d passes keep their intermediate result in the workspace, which must then be 16-byte aligned",
+                 plan.n_pass);
+        return false;
+    }
     for (int i = 0; i < 2; ++i) {
         const PassPlan& pp = i ? plan.shortp : plan.longp;
         if (pp.cfg >= 0 && (long)p.B * p.C * pp.n_strips * pp.n_bands > 2147483647L) {
@@ -1584,6 +1589,10 @@ int cluster2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_
         set_error("cluster path splits %d steps into %d passes and needs %zu workspace bytes, got %zu", p.iters, plan.n_pass,
                   d_bytes, ws ? ws_bytes : (size_t)0);
         return CSPN_ERR_WORKSPACE;
+    }
+    if (plan.n_pass > 1 && (reinterpret_cast<uintptr_t>(ws) & 15)) {   // the callers decline this in cluster2d_supported
+        set_error("cluster path splits %d steps into %d passes and needs a 16-byte aligned workspace", p.iters, plan.n_pass);
+        return CSPN_ERR_UNSUPPORTED;
     }
     const float* prev = nullptr;   // result of the previous pass
     for (int ip = 0; ip < plan.n_pass; ++ip) {

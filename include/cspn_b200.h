@@ -79,7 +79,10 @@ typedef enum {
 /* Workspace for `algo`.  CSPN_ALGO_AUTO assumes what the cluster kernel needs of its tensors -- W % 4 == 0 and 16-byte
  * aligned base pointers (every allocator's default) -- because the query cannot see the pointers; if a call then has to
  * take the generic path (misaligned views), cspn2d_fwd_f32 returns CSPN_ERR_WORKSPACE with a message naming
- * cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) as the size to provide. */
+ * cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) as the size to provide.  The workspace should be 16-byte aligned too:
+ * a cluster plan of several passes keeps its intermediate result there with 16-byte stores, so it declines a misaligned
+ * workspace -- CSPN_ALGO_AUTO then takes the generic path as above, CSPN_ALGO_CLUSTER and cspn2d_fwd_gather_f32 return
+ * CSPN_ERR_UNSUPPORTED.  The generic path takes any 4-byte aligned workspace. */
 CSPN_API size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo);
 
 CSPN_API int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out,

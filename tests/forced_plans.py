@@ -19,6 +19,8 @@ import torch
 
 from cspn_b200 import _lib
 
+import memory_contract as mc
+
 # configs() of cspn_b200/csrc/cspn2d_cluster.cu by index: (PR rows per thread, NW warps); a CTA covers PR*NW rows x 128
 CONFIGS = [(5, 8), (4, 8), (3, 8), (2, 8), (5, 4)]
 CHAINED = (0, 1, 2)        # the configurations that have chained-strip forward kernels
@@ -139,18 +141,22 @@ def bit_group(plan, info):
 
 def backward(g, d, s, go, n, norm):
     """The C ABI's backward called directly (ctypes, this thread): autograd would run it on the engine's worker thread,
-    where the thread-local cspn_last_launches() of this thread does not see it.  Returns (grad_guidance, grad_blur) in
-    float64 on the CPU and the launch count."""
+    where the thread-local cspn_last_launches() of this thread does not see it.  Both gradients and a workspace of exactly
+    the queried size sit in sentinel-filled guarded buffers (tests/memory_contract.py), checked to be fully written and
+    stored within.  Returns (grad_guidance, grad_blur) in float64 on the CPU and the launch count."""
     L = _lib.lib()
     gc, dc, goc = g.cuda().contiguous(), d.cuda().contiguous(), go.cuda().contiguous()
     sc = None if s is None else s.cuda().contiguous()
     B, C, H, W = dc.shape
-    gg, gd = torch.empty_like(gc), torch.empty_like(dc)
+    gg, gd = mc.guarded(gc.shape), mc.guarded(dc.shape)
     ws_bytes = L.cspn2d_bwd_workspace_bytes(B, C, H, W, n)
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device='cuda')
-    rc = L.cspn2d_bwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), goc.data_ptr(), gg.data_ptr(),
-                          gd.data_ptr(), B, C, H, W, gc.shape[1], n, _lib.NORM2D[norm], ws.data_ptr(), ws_bytes,
+    ws = mc.workspace(ws_bytes)
+    rc = L.cspn2d_bwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), goc.data_ptr(), gg.ptr(),
+                          gd.ptr(), B, C, H, W, gc.shape[1], n, _lib.NORM2D[norm], ws.ptr(), ws_bytes,
                           torch.cuda.current_stream().cuda_stream)
     _lib.check(rc, 'cspn2d_bwd_f32')
     torch.cuda.synchronize()
-    return gg.double().cpu(), gd.double().cpu(), L.cspn_last_launches()
+    mc.assert_written(gg, 'grad_guidance')
+    mc.assert_written(gd, 'grad_blur')
+    assert ws.guards_intact(), 'a store landed past the workspace'
+    return gg.t.double().cpu(), gd.t.double().cpu(), L.cspn_last_launches()

@@ -15,6 +15,7 @@ import torch
 from cspn_b200 import _lib
 from cspn_b200.synth import make_inputs
 from conftest import load_golden
+import memory_contract as mc
 from forced_plans import (NAN_PATCH_PLANS, NORMS, PROBLEMS, SPECIAL, backward, bit_group, chains, check_honoured, force,
                           plan_info, special_plans)
 from oracle import c_oracle, cspn_numpy as onp, cspn_torch_port as tp
@@ -28,20 +29,24 @@ def inputs(pb, seed):
 
 
 def _forward(g, d, s, n, norm):
-    """The C ABI on this thread (cspn_last_* are thread-local), with a workspace prefilled with 0xA5 bytes."""
+    """The C ABI on this thread (cspn_last_* are thread-local).  `out` and a workspace of exactly the queried size sit in
+    sentinel-filled guarded buffers (tests/memory_contract.py): every plan must store all of `out` and nothing outside it
+    or past the workspace.  Returns the workspace's interior."""
     L = _lib.lib()
     gc, dc = g.cuda().contiguous(), d.cuda().contiguous()
     sc = None if s is None else s.cuda().contiguous()
     B, C, H, W = dc.shape
     ws_bytes = L.cspn2d_workspace_bytes(B, C, H, W, n, _lib.ALGO_CLUSTER)
-    ws = torch.full((max(ws_bytes, 16),), 0xA5, dtype=torch.uint8, device='cuda')
-    out = torch.empty_like(dc)
-    rc = L.cspn2d_fwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), out.data_ptr(), B, C, H, W,
-                          gc.shape[1], n, _lib.NORM2D[norm], _lib.ALGO_CLUSTER, ws.data_ptr(), ws_bytes,
+    ws = mc.workspace(ws_bytes)
+    out = mc.guarded(dc.shape)
+    rc = L.cspn2d_fwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), out.ptr(), B, C, H, W,
+                          gc.shape[1], n, _lib.NORM2D[norm], _lib.ALGO_CLUSTER, ws.ptr(), ws_bytes,
                           torch.cuda.current_stream().cuda_stream)
     _lib.check(rc, 'cspn2d_fwd_f32')
     torch.cuda.synchronize()
-    return out.cpu(), L.cspn_last_algo(), L.cspn_last_launches(), ws
+    mc.assert_written(out, 'out')
+    assert ws.guards_intact(), 'a store landed past the workspace'
+    return out.t.cpu(), L.cspn_last_algo(), L.cspn_last_launches(), ws.t
 
 
 def chain_flags(info, B, C, H, W, ws):
