@@ -27,6 +27,10 @@ SIGNATURES = {
     'cspn2d_k_fwd_f32': (_i, [_vp] * 4 + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn2d_k_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_k_bwd_f32': (_i, [_vp] * 6 + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn2d_paddle_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_paddle_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_paddle_bwd_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_paddle_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn3d_workspace_bytes': (_sz, [_i] * 6),
     'cspn3d_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_fwd_f32_host': (_i, [_vp] * 3 + [_i] * 8),

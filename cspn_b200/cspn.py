@@ -517,3 +517,109 @@ class Affinity_Propagate3DK(nn.Module):
 
     def extra_repr(self):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'
+
+
+# ---- 2D with the Paddle module's own-location gates (K in {3, 5, 7}) -------------------------------------------------
+def _check_inputs_2d_paddle(guidance, feat, prop_kernel):
+    """Shapes of CSPN.cspn with dim_num = 2 (cspn_paddle/demo.py:20-54).  guidance (B, K*K-1, H, W) is one gate shared by
+    the C channels of feat (B, C, H, W); (B, (K*K-1)*C, H, W) with C > 1 gives channel c the guide channels
+    [nt*c, nt*c+nt) (demo.py:28-45), which in memory is B*C single-channel images.  Any other channel count is a
+    ValueError: demo.py normalises over every guide channel it is given.  Returns the (images, channels) of the C ABI."""
+    assert prop_kernel in KERNEL_SIZES_2D, f'prop_kernel must be 3, 5 or 7, got {prop_kernel}'
+    nt = prop_kernel * prop_kernel - 1
+    if guidance.dim() != 4 or feat.dim() != 4:
+        raise ValueError('guidance and feat must be (B,C,H,W)')
+    if guidance.dtype != torch.float32 or feat.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    B, C, H, W = feat.shape
+    per_channel = C > 1 and guidance.shape[1] == nt * C
+    if guidance.shape[0] != B or guidance.shape[2:] != (H, W) or not (guidance.shape[1] == nt or per_channel):
+        raise ValueError(f"a {prop_kernel}x{prop_kernel} 'paddle' kernel needs guidance (B,{nt},H,W) or, with C > 1 feature "
+                         f'channels, (B,{nt}*C,H,W); got {tuple(guidance.shape)} for feat {tuple(feat.shape)}')
+    if guidance.device != feat.device:
+        raise RuntimeError('guidance and feat are on different devices')
+    if not (guidance.is_cuda and feat.is_cuda):
+        raise _lib.CspnError(f"the {prop_kernel}x{prop_kernel} 'paddle' propagation takes CUDA tensors only "
+                             '(there is no host-buffer entry point for it)')
+    return (B * C, 1) if per_channel else (B, C)
+
+
+def propagate2d_paddle(guidance, feat, prop_kernel=3, prop_time=24):
+    """CSPN.cspn of the Paddle module with dim_num = 2, forward only (no autograd), CUDA tensors only, enqueued on the
+    current stream: w_k = |g_k| / sum_j |g_j| at each pixel's own location, then prop_time steps
+    d <- sum_k w_k shift_k(d) (zero padding, no centre term).  Shapes as in Affinity_Propagate2DPaddle."""
+    Bi, Ci = _check_inputs_2d_paddle(guidance, feat, prop_kernel)
+    if prop_time == 0:
+        return feat
+    L = _lib.lib()
+    H, W = feat.shape[2:]
+    g, f = guidance.contiguous(), feat.contiguous()
+    out = torch.empty_like(f)
+    with torch.cuda.device(f.device):
+        ws_bytes = L.cspn2d_paddle_workspace_bytes(Bi, Ci, H, W, prop_kernel, int(prop_time))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+        rc = L.cspn2d_paddle_fwd_f32(_ptr(g), _ptr(f), _ptr(out), Bi, Ci, H, W, prop_kernel, int(prop_time), _ptr(ws), ws_bytes,
+                                     _stream(f.device))
+    _lib.check(rc, 'cspn2d_paddle_fwd_f32')
+    return out
+
+
+class _Propagate2dPaddleFn(torch.autograd.Function):
+    """autograd seam of the 2D 'paddle' operator without the torch-op shim: native forward + native adjoint
+    (cspn2d_paddle_bwd_f32)."""
+
+    @staticmethod
+    def forward(ctx, guidance, feat, prop_kernel, prop_time):
+        ctx.save_for_backward(guidance, feat)
+        ctx.cfg = (prop_kernel, prop_time)
+        return propagate2d_paddle(guidance, feat, prop_kernel, prop_time)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        guidance, feat = ctx.saved_tensors
+        prop_kernel, prop_time = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        Bi, Ci = _check_inputs_2d_paddle(guidance, feat, prop_kernel)
+        L = _lib.lib()
+        H, W = feat.shape[2:]
+        g, f, go = guidance.contiguous(), feat.contiguous(), grad_out.contiguous()
+        gg = torch.empty_like(g) if ctx.needs_input_grad[0] else None
+        gf = torch.empty_like(f) if ctx.needs_input_grad[1] else None
+        with torch.cuda.device(f.device):
+            ws_bytes = L.cspn2d_paddle_bwd_workspace_bytes(Bi, Ci, H, W, prop_kernel, int(prop_time))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+            rc = L.cspn2d_paddle_bwd_f32(_ptr(g), _ptr(f), _ptr(go), _ptr(gg), _ptr(gf), Bi, Ci, H, W, prop_kernel,
+                                         int(prop_time), _ptr(ws), ws_bytes, _stream(f.device))
+        _lib.check(rc, 'cspn2d_paddle_bwd_f32')
+        return gg, gf, None, None
+
+
+class Affinity_Propagate2DPaddle(nn.Module):
+    """The 2D half of the Paddle module (cspn_paddle/demo.py --dimNum=2): CSPN.cspn(guide, feat) with dim_num = 2,
+    K in {3, 5, 7} (demo.py:65, guide_chan = K*K-1).  forward(guidance, feat (B, C, H, W)): guidance (B, K*K-1, H, W), one
+    gate shared by the C channels, or (B, (K*K-1)*C, H, W) with C > 1, one gate per channel.  The gates are |guidance|
+    normalised over the channels at each pixel's own location; each of prop_time steps is sum_k w_k shift_k(feat), with
+    zero padding, no centre term and no sparse replacement (DESIGN.md section 4.10).  No parameters, no buffers;
+    prop_time == 0 returns feat itself.  Forward and backward run in CUDA kernels."""
+
+    def __init__(self, prop_time, prop_kernel=3):
+        super().__init__()
+        assert prop_kernel in KERNEL_SIZES_2D, f'prop_kernel must be 3, 5 or 7, got {prop_kernel}'
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+        self._use_op = _use_torch_op()
+
+    def forward(self, guidance, feat):
+        if self.prop_time == 0:
+            return feat
+        _check_inputs_2d_paddle(guidance, feat, self.prop_kernel)
+        if self._use_op:
+            return torch.ops.cspn_b200.propagate2d_paddle(guidance, feat, self.prop_kernel, self.prop_time)
+        if torch.is_grad_enabled() and (guidance.requires_grad or feat.requires_grad):
+            return _Propagate2dPaddleFn.apply(guidance, feat, self.prop_kernel, self.prop_time)
+        return propagate2d_paddle(guidance, feat, self.prop_kernel, self.prop_time)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'

@@ -240,6 +240,58 @@ int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const float* spar
     return rc;
 }
 
+// ---- 2D 'paddle' (own-location norm), K in {3, 5, 7}: every K in cspn2d_wide.cu ------------------------------------
+static int check2d_paddle(const float* guidance, const float* feat, const void* out, int B, int C, int H, int W, int K,
+                          int iters) {
+    if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!kernel_size_ok(K)) { set_error("kernel size must be 3, 5 or 7, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+size_t cspn2d_paddle_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
+    return widek_workspace_bytes(B, C, H, W, K, iters);
+}
+
+int cspn2d_paddle_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int H, int W, int K, int iters,
+                          void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_paddle(guidance, feat, out, B, C, H, W, K, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
+    int launches = 0;
+    rc = widek_paddle_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn2d_paddle_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
+    return widek_bwd_workspace_bytes(B, C, H, W, K, iters);
+}
+
+int cspn2d_paddle_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
+                          int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                          cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_paddle(guidance, feat, grad_out, B, C, H, W, K, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, feat, nullptr, nullptr, B, C, H, W, K * K - 1, iters, 0};
+    int launches = 0;
+    rc = widek_paddle_backward(p, K, grad_out, grad_guidance, grad_feat, workspace, workspace_bytes, (cudaStream_t)stream,
+                               &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
 size_t cspn3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
     if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0) return 0;
     return generic3d_workspace_bytes(B, C, D, H, W, iters);

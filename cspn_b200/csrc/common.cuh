@@ -86,6 +86,10 @@ int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStre
 size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                    size_t ws_bytes, cudaStream_t stream, int* launches);
+// 'paddle' own-location norm, K in {3, 5, 7}, on the same kernels and workspaces (p.sparse null, p.gch == K*K-1)
+int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
+                          size_t ws_bytes, cudaStream_t stream, int* launches);
 
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);

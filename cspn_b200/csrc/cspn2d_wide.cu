@@ -19,6 +19,13 @@
 // Backward, in the staged form of cspn2d_bwd.cu: prep, N-1 forward steps that keep d_1..d_{N-1}, N adjoint steps
 //   lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k) (lambda_{t+1} tile + halo in shared memory), and one
 //   gather-finalize kernel (Gw_k, Gc in registers, then the chain rule of cspn2d_bwd.cu with K*K-1 taps).
+//
+// 'paddle' (cspn_paddle/demo.py with dimNum = 2), K = 2R+1 in {3, 5, 7}, on the same launches:
+//   w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location,   d_{t+1} = sum_k w_k d_t(p + off_k)
+// with no centre term and no sparse replacement.  Its prep (prepk_paddle_kernel) writes w_k and a zero kappa plane; the
+// step kernels' PADDLE flag drops the kappa d0 term and the d0 load; the adjoint step is shared as it is; the gather's
+// PADDLE flag applies the own-location chain rule (grad_g_j at p, grad_feat = lambda_0).  K = 3 runs here too: the
+// cluster kernel keeps the folded 3x3 form only.
 #include <cstdlib>
 #include <cstring>
 
@@ -78,12 +85,36 @@ prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ spars
     o[T::NT * HW] = om * (1.f - s) + m;
 }
 
+// 'paddle' prep: w_k = |g_k(p)| / sum_j |g_j(p)|, kappa = 0.  guidance [image][NT][H][W]; grid z = image of the group
+template <int R>
+__global__ void __launch_bounds__(256)
+prepk_paddle_kernel(const float* __restrict__ guidance, float* __restrict__ wk, int H, int W) {
+    using T = Taps<R>;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    const int b = blockIdx.z;
+    if (x >= W || y >= H) return;
+    const size_t HW = (size_t)H * W, p = (size_t)y * W + x;
+    const float* g = guidance + (size_t)b * T::NT * HW + p;
+    float a[T::NT], S = 0.f;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) {
+        a[k] = fabsf(__ldg(g + k * HW));
+        S += a[k];
+    }
+    float* o = wk + (size_t)b * T::NP * HW + p;
+#pragma unroll
+    for (int k = 0; k < T::NT; ++k) o[k * HW] = __fdiv_rn(a[k], S);   // IEEE: 0/0 -> NaN, x/inf -> 0, subnormal S exact
+    o[T::NT * HW] = 0.f;
+}
+
 // ---- step, 4 pixels of a row per thread (W % 4 == 0, 16-byte aligned cur / d0 / dst / wk) -------------------------
 // Tile 64 x 16 pixels per CTA of 16 x 16 threads.  The shared tile holds rows y0-R .. y0+15+R and columns x0-4 ..
 // x0+67 as float4 (the halo is rounded up to 4 columns so every row of a thread's window is three aligned LDS.128).
+// PADDLE: no kappa d0 term (d0 is not read).
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R>
+template <int R, bool PADDLE = false>
 __global__ void __launch_bounds__(256)
 stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
                  float* __restrict__ dst, int C, int H, int W) {
@@ -106,9 +137,12 @@ stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, con
     if (x >= W || y >= H) return;
     const size_t p = (size_t)y * W + x;
     const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
-    const float4 kap = __ldg(reinterpret_cast<const float4*>(w + T::NT * HW));
-    const float4 dd = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)bc * HW + p));
-    float acc0 = kap.x * dd.x, acc1 = kap.y * dd.y, acc2 = kap.z * dd.z, acc3 = kap.w * dd.w;
+    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;
+    if (!PADDLE) {
+        const float4 kap = __ldg(reinterpret_cast<const float4*>(w + T::NT * HW));
+        const float4 dd = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)bc * HW + p));
+        acc0 = kap.x * dd.x; acc1 = kap.y * dd.y; acc2 = kap.z * dd.z; acc3 = kap.w * dd.w;
+    }
 #pragma unroll
     for (int t = 0; t < T::K; ++t) {
         const int r = ty + R + (R - t);                      // tile row of source row y + dy, dy = R - t
@@ -143,7 +177,7 @@ __device__ __forceinline__ void load_tile_scalar(float (*tile)[kSclTW + 2 * R], 
     }
 }
 
-template <int R>
+template <int R, bool PADDLE = false>
 __global__ void __launch_bounds__(256)
 stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
                     float* __restrict__ dst, int C, int H, int W) {
@@ -157,7 +191,7 @@ stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, 
     if (x >= W || y >= H) return;
     const size_t p = (size_t)y * W + x;
     const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
-    float acc = __ldg(w + T::NT * HW) * __ldg(d0 + (size_t)bc * HW + p);
+    float acc = PADDLE ? 0.f : __ldg(w + T::NT * HW) * __ldg(d0 + (size_t)bc * HW + p);
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
     dst[(size_t)bc * HW + p] = acc;
@@ -190,7 +224,9 @@ adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, floa
 // Gw_k(p) = sum_t lambda_{t+1}(p) d_t(p + off_k) with d_t staged tile by tile, Gc = sum_t lambda_{t+1}; then the finalize
 // arithmetic of cspn2d_bwd.cu.  steps[t] = d_{t+1}, lam[t] = lambda_t (planes n floats apart), lambda_N = grad_out.
 // grid z = image of the group; every pointer is offset to the group's first image.
-template <int R>
+// PADDLE (sparse null, gch = NT): the own-location chain rule of cspn3d_wide.cu's fin3k_kernel mode 2 -- no centre term,
+// grad_g_j lands at p, grad_blur = lambda_0.
+template <int R, bool PADDLE = false>
 __global__ void __launch_bounds__(256)
 gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
                const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
@@ -205,7 +241,7 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
     float gw[T::NT];
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) gw[k] = 0.f;
-    const float kappa = in ? __ldg(wk + ((size_t)b * T::NP + T::NT) * HW + p) : 0.f;
+    const float kappa = in && !PADDLE ? __ldg(wk + ((size_t)b * T::NP + T::NT) * HW + p) : 0.f;
     float gkappa = 0.f;
     for (int c = 0; c < C; ++c) {
         const size_t plane = ((size_t)b * C + c) * HW;
@@ -223,11 +259,29 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
                     gw[k] = fmaf(lp, tile[ty + R + T::dy(k)][tx + R + T::dx(k)], gw[k]);
         }
         if (!in) continue;
+        if (PADDLE) {
+            if (grad_blur) grad_blur[plane + p] = __ldg(lam + plane + p);
+            continue;
+        }
         gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
         if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
     }
     if (!in || !grad_guidance) return;
     const float* g = guidance + (size_t)b * gch * HW;
+    if (PADDLE) {
+        float S = 0.f;
+#pragma unroll
+        for (int k = 0; k < T::NT; ++k) S += fabsf(__ldg(g + k * HW + p));
+        float Tsum = 0.f;
+#pragma unroll
+        for (int k = 0; k < T::NT; ++k) Tsum = fmaf(gw[k], __fdiv_rn(fabsf(__ldg(g + k * HW + p)), S), Tsum);
+#pragma unroll
+        for (int k = 0; k < T::NT; ++k) {   // d|g|/dg = sign(g), 0 at 0 like torch.abs
+            const float v = __ldg(g + k * HW + p);
+            grad_guidance[((size_t)b * gch + k) * HW + p] = __fdiv_rn(gw[k] - signf(fabsf(v)) * Tsum, S) * signf(v);
+        }
+        return;
+    }
     float a[T::NT], S = 0.f;
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) {
@@ -275,24 +329,26 @@ int group_size(int B) {
     return B;
 }
 
-template <int R>
+template <int R, bool PADDLE>
 void launch_prep(const float* guidance, const float* sparse, float* wk, int nimg, int H, int W, int gch, int norm_abs,
                  cudaStream_t s) {
-    prepk_kernel<R><<<dim3((W + 31) / 32, (H + 7) / 8, nimg), dim3(32, 8), 0, s>>>(guidance, sparse, wk, H, W, gch, norm_abs);
+    const dim3 grid((W + 31) / 32, (H + 7) / 8, nimg), block(32, 8);
+    if constexpr (PADDLE) prepk_paddle_kernel<R><<<grid, block, 0, s>>>(guidance, wk, H, W);
+    else prepk_kernel<R><<<grid, block, 0, s>>>(guidance, sparse, wk, H, W, gch, norm_abs);
 }
 
-template <int R>
+template <int R, bool PADDLE>
 void launch_step(bool vec, const float* wk, const float* d0, const float* cur, float* dst, int nbc, int C, int H, int W,
                  cudaStream_t s) {
     if (vec)
-        stepk_vec_kernel<R><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
+        stepk_vec_kernel<R, PADDLE><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
             wk, d0, cur, dst, C, H, W);
     else
-        stepk_scalar_kernel<R><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
+        stepk_scalar_kernel<R, PADDLE><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
             wk, d0, cur, dst, C, H, W);
 }
 
-template <int R>
+template <int R, bool PADDLE>
 int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) {
     constexpr int NP = Taps<R>::NP;
     const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
@@ -306,13 +362,13 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) 
         const float* blur = p.blur + (size_t)b0 * plane;
         float* out = p.out + (size_t)b0 * plane;
         float* tmp = tmp_all + (size_t)b0 * plane;
-        launch_prep<R>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr, wk, nimg, p.H,
-                       p.W, p.gch, p.norm_abs, stream);
+        launch_prep<R, PADDLE>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr, wk, nimg,
+                               p.H, p.W, p.gch, p.norm_abs, stream);
         ++*launches;
         const float* cur = blur;
         float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < p.iters; ++it) {
-            launch_step<R>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
+            launch_step<R, PADDLE>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
             ++*launches;
             cur = dst;
             dst = (dst == out) ? tmp : out;
@@ -322,7 +378,7 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) 
     return CSPN_OK;
 }
 
-template <int R>
+template <int R, bool PADDLE>
 int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                cudaStream_t stream, int* launches) {
     constexpr int NP = Taps<R>::NP;
@@ -340,10 +396,10 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
         const float* blur = p.blur + off;
         const float* guidance = p.guidance + (size_t)b0 * p.gch * HW;
         const float* sparse = p.sparse ? p.sparse + (size_t)b0 * HW : nullptr;
-        launch_prep<R>(guidance, sparse, wk, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+        launch_prep<R, PADDLE>(guidance, sparse, wk, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
         ++*launches;
         for (int t = 0; t + 1 < p.iters; ++t) {        // d_{t+1} = step(d_t)
-            launch_step<R>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
+            launch_step<R, PADDLE>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
                            nimg * p.C, p.C, p.H, p.W, stream);
             ++*launches;
         }
@@ -353,7 +409,7 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
             adjk_kernel<R><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lam + (size_t)t * n + off, p.C, p.H, p.W);
             ++*launches;
         }
-        gatherk_kernel<R><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
+        gatherk_kernel<R, PADDLE><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
             guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off,
             grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr, grad_blur ? grad_blur + off : nullptr, n,
             p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
@@ -389,7 +445,7 @@ int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStre
         return CSPN_ERR_WORKSPACE;
     }
     if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
-    return K == 5 ? forward_k<2>(p, ws, stream, launches) : forward_k<3>(p, ws, stream, launches);
+    return K == 5 ? forward_k<2, false>(p, ws, stream, launches) : forward_k<3, false>(p, ws, stream, launches);
 }
 
 int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
@@ -407,8 +463,44 @@ int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad
         return CSPN_ERR_WORKSPACE;
     }
     if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D backward: B*C exceeds gridDim.z", K, K); return CSPN_ERR_UNSUPPORTED; }
-    return K == 5 ? backward_k<2>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
-                  : backward_k<3>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+    return K == 5 ? backward_k<2, false>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
+                  : backward_k<3, false>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+}
+
+// 'paddle': p.sparse is null and p.gch == K*K-1 (the C ABI sets both); same workspaces as the K x K path
+int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+    if (p.iters == 0) {
+        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
+    if (!ws || ws_bytes < need) {
+        set_error("%dx%d 2D 'paddle' path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D 'paddle' path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
+    if (K == 3) return forward_k<1, true>(p, ws, stream, launches);
+    return K == 5 ? forward_k<2, true>(p, ws, stream, launches) : forward_k<3, true>(p, ws, stream, launches);
+}
+
+int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
+                          size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
+    if (p.iters == 0) {   // the identity: no dependence on the guidance
+        if (grad_guidance) CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
+        if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
+    if (!ws || ws_bytes < need) {
+        set_error("%dx%d 2D 'paddle' backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D 'paddle' backward: B*C exceeds gridDim.z", K, K); return CSPN_ERR_UNSUPPORTED; }
+    // every guidance gradient is written by the finalize (each g_j(p) feeds pixel p alone): no zero fill
+    if (K == 3) return backward_k<1, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+    return K == 5 ? backward_k<2, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
+                  : backward_k<3, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
 }
 
 }  // namespace cspn

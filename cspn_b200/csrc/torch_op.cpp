@@ -14,6 +14,10 @@
 //       -> Tensor                                                    (K x K kernel, K in {3, 5, 7}; K = 3 is propagate2d)
 //   propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size,
 //                          int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)
+//   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
+//       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
+//   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
+//                               bool need_guidance, bool need_feat) -> (Tensor, Tensor)
 //   propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor
 //   propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type,
 //                        bool need_guidance, bool need_feat) -> (Tensor, Tensor)
@@ -29,6 +33,7 @@
 
 #include <optional>
 #include <tuple>
+#include <utility>
 
 #include "../../include/cspn_b200.h"
 
@@ -163,6 +168,60 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_k_backward_cuda(const at::Tensor&
     return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
 }
 
+// 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
+// (B, (K*K-1)*C, H, W) with C > 1 gives channel c its own gate (demo.py:28-45), which in memory is B*C images of one
+// channel.  Returns the (images, channels) the C ABI is called with.
+std::pair<int, int> check2d_paddle(const at::Tensor& guidance, const at::Tensor& feat, int64_t K) {
+    TORCH_CHECK_VALUE(K == 3 || K == 5 || K == 7, "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK_VALUE(guidance.dim() == 4 && feat.dim() == 4, "guidance and feat must be (B,C,H,W)");
+    TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    const int64_t nt = K * K - 1, B = feat.size(0), C = feat.size(1);
+    const bool shape_ok = guidance.size(0) == B && guidance.size(2) == feat.size(2) && guidance.size(3) == feat.size(3);
+    const bool per_channel = C > 1 && guidance.size(1) == nt * C;
+    TORCH_CHECK_VALUE(shape_ok && (guidance.size(1) == nt || per_channel), "a ", K, "x", K, " 'paddle' kernel needs guidance (B,",
+                      nt, ",H,W) or, with C > 1 feature channels, (B,", nt, "*C,H,W); got ", guidance.sizes(), " for feat ",
+                      feat.sizes());
+    TORCH_CHECK(guidance.device() == feat.device(), "guidance and feat are on different devices");
+    return per_channel ? std::make_pair((int)(B * C), 1) : std::make_pair((int)B, (int)C);
+}
+
+at::Tensor propagate2d_paddle_cuda(const at::Tensor& guidance, const at::Tensor& feat, int64_t K, int64_t prop_time) {
+    const auto [B, C] = check2d_paddle(guidance, feat, K);
+    if (prop_time == 0) return feat.clone();
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor g = guidance.contiguous(), f = feat.contiguous();
+    at::Tensor out = at::empty_like(f);
+    const int H = (int)f.size(2), W = (int)f.size(3);
+    const size_t ws_bytes = cspn2d_paddle_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
+    check_rc(cspn2d_paddle_fwd_f32(fptr(g), fptr(f), out.data_ptr<float>(), B, C, H, W, (int)K, (int)prop_time,
+                                   ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn2d_paddle_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> propagate2d_paddle_backward_cuda(const at::Tensor& guidance, const at::Tensor& feat,
+                                                                    const at::Tensor& grad_out, int64_t K, int64_t prop_time,
+                                                                    bool need_g, bool need_f) {
+    const auto [B, C] = check2d_paddle(guidance, feat, K);
+    TORCH_CHECK(grad_out.sizes() == feat.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == feat.device(),
+                "grad_out must match feat");
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor g = guidance.contiguous(), f = feat.contiguous(), go = grad_out.contiguous();
+    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
+    at::Tensor gf = need_f ? at::empty_like(f) : at::Tensor();
+    const int H = (int)f.size(2), W = (int)f.size(3);
+    const size_t ws_bytes = cspn2d_paddle_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
+    check_rc(cspn2d_paddle_bwd_f32(fptr(g), fptr(f), fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
+                                   need_f ? gf.data_ptr<float>() : nullptr, B, C, H, W, (int)K, (int)prop_time,
+                                   ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn2d_paddle_bwd_f32");
+    return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+}
+
 void check3d(const at::Tensor& guidance, const at::Tensor& feat) {
     TORCH_CHECK(guidance.dim() == 5 && feat.dim() == 5, "guidance and feat must be (B,C,D,H,W)");
     TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
@@ -276,6 +335,9 @@ TORCH_LIBRARY(cspn_b200, m) {
           "int norm_type) -> Tensor");
     m.def("propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size, "
           "int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)");
+    m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
+    m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
+          "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
     m.def("propagate3d(Tensor guidance, Tensor feat, int prop_time, int norm_type) -> Tensor");
     m.def("propagate3d_backward(Tensor guidance, Tensor feat, Tensor grad_out, int prop_time, int norm_type, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -289,6 +351,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_backward", &propagate2d_backward_cuda);
     m.impl("propagate2d_k", &propagate2d_k_cuda);
     m.impl("propagate2d_k_backward", &propagate2d_k_backward_cuda);
+    m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
+    m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);
     m.impl("propagate3d_backward", &propagate3d_backward_cuda);
     m.impl("propagate3d_k", &propagate3d_k_cuda);

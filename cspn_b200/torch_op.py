@@ -67,6 +67,21 @@ def _register():
         gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
         return gg, gd
 
+    @lib.register_fake('cspn_b200::propagate2d_paddle')
+    def _(guidance, feat, kernel_size, prop_time):
+        torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        nt = kernel_size * kernel_size - 1
+        torch._check(guidance.shape[1] == nt or (feat.shape[1] > 1 and guidance.shape[1] == nt * feat.shape[1]),
+                     lambda: f'a {kernel_size}x{kernel_size} \'paddle\' kernel needs {nt} or {nt}*C guidance channels')
+        return torch.empty_like(feat, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_paddle_backward')
+    def _(guidance, feat, grad_out, kernel_size, prop_time, need_guidance, need_feat):
+        gg = torch.empty_like(guidance, memory_format=torch.contiguous_format) if need_guidance else guidance.new_empty(0)
+        gf = torch.empty_like(feat, memory_format=torch.contiguous_format) if need_feat else feat.new_empty(0)
+        return gg, gf
+
     @lib.register_fake('cspn_b200::propagate3d')
     def _(guidance, feat, prop_time, norm_type):
         torch._check(guidance.dim() == 5 and feat.dim() == 5, lambda: 'guidance and feat must be (B,C,D,H,W)')
@@ -121,6 +136,21 @@ def _register():
         return (gg if need_g else None), (gd if need_d else None), None, None, None, None
 
     lib.register_autograd('cspn_b200::propagate2d_k', backward2d_k, setup_context=setup2d_k)
+
+    def setup2d_paddle(ctx, inputs, output):
+        guidance, feat, kernel_size, prop_time = inputs
+        ctx.save_for_backward(guidance, feat)
+        ctx.cfg = (kernel_size, prop_time)
+
+    def backward2d_paddle(ctx, grad_out):
+        guidance, feat = ctx.saved_tensors
+        kernel_size, prop_time = ctx.cfg
+        need_g, need_f = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        gg, gf = torch.ops.cspn_b200.propagate2d_paddle_backward(guidance, feat, grad_out.contiguous(), kernel_size, prop_time,
+                                                                 need_g, need_f)
+        return (gg if need_g else None), (gf if need_f else None), None, None
+
+    lib.register_autograd('cspn_b200::propagate2d_paddle', backward2d_paddle, setup_context=setup2d_paddle)
 
     def setup3d(ctx, inputs, output):
         guidance, feat, prop_time, norm_type = inputs

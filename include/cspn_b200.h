@@ -140,6 +140,27 @@ CSPN_API int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const fl
                      int guidance_channels, int K, int iters, int norm_type,
                      void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
+ * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
+ * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
+ * K x K calls above.  guidance [B][K*K-1][H][W], one gate shared by the C channels of feat [B][C][H][W]; per-channel gates
+ * (demo.py:28-45, guidance [B][(K*K-1)*C][H][W]) are the same memory as B*C images with C = 1.  out / grad_feat
+ * [B][C][H][W], grad_guidance [B][K*K-1][H][W]; either gradient may be NULL.  K = 3 runs on the K x K kernels too.
+ * Workspace: forward B*K*K*H*W + B*C*H*W floats, backward B*K*K*H*W + 2*iters*B*C*H*W floats, 0 for iters == 0; neither
+ * depends on the device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5, 7}, iters < 0, a non-positive shape or a null
+ * guidance / feat / out (grad_out in the backward); CSPN_ERR_UNSUPPORTED for B*C > 65535. */
+CSPN_API size_t cspn2d_paddle_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_paddle_fwd_f32(const float* guidance, const float* feat, float* out,
+                          int B, int C, int H, int W, int K, int iters,
+                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_paddle_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_paddle_bwd_f32(const float* guidance, const float* feat, const float* grad_out,
+                          float* grad_guidance, float* grad_feat, int B, int C, int H, int W, int K, int iters,
+                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 3D: replaces CSPN.cspn(guide, feat) (cspn_paddle/demo.py:20-54) ------------------------
  * guidance [B][26][D][H][W], feat/out [B][C][D][H][W] (gate shared across C, cspn_paddle/README.md:56)
  */
