@@ -31,6 +31,14 @@ SIGNATURES = {
     'cspn2d_paddle_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_paddle_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_paddle_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_gates_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_gates_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_gates_bwd_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_gates_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn3d_gates_workspace_bytes': (_sz, [_i] * 7),
+    'cspn3d_gates_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _sz, _vp]),
+    'cspn3d_gates_bwd_workspace_bytes': (_sz, [_i] * 7),
+    'cspn3d_gates_bwd_f32': (_i, [_vp] * 5 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_workspace_bytes': (_sz, [_i] * 6),
     'cspn3d_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_fwd_f32_host': (_i, [_vp] * 3 + [_i] * 8),

@@ -623,3 +623,103 @@ class Affinity_Propagate2DPaddle(nn.Module):
 
     def extra_repr(self):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'
+
+
+# ---- caller-supplied gates: fluid.layers.affinity_propagate itself (2D K in {3, 5, 7}, 3D K in {3, 5}) ----------------
+def _check_gates(input, gate_weight, kernel_size, prop_step):
+    """Shapes of fluid.layers.affinity_propagate(input, gate_weight, kernel_size) (cspn_paddle/demo.py:41-43, 51-52): a 4-D
+    input (B, C, H, W) is 2D, a 5-D one (B, C, D, H, W) is 3D.  gate_weight (B, K**d-1, ...) is one gate shared by the C
+    channels; (B, (K**d-1)*C, ...) with C > 1 gives channel c the gate channels [nt*c, nt*c+nt) (demo.py:28-45), which in
+    memory is B*C single-channel images.  Returns (d, images, channels) of the C ABI."""
+    if input.dim() not in (4, 5):
+        raise ValueError(f'input must be (B,C,H,W) or (B,C,D,H,W), got {tuple(input.shape)}')
+    nd = input.dim() - 2
+    sizes = KERNEL_SIZES_2D if nd == 2 else KERNEL_SIZES_3D
+    assert kernel_size in sizes, f'kernel_size of a {nd}D affinity_propagate must be one of {sizes}, got {kernel_size}'
+    nt = kernel_size ** nd - 1
+    if gate_weight.dim() != input.dim():
+        raise ValueError(f'gate_weight must have the dimensions of input, got {tuple(gate_weight.shape)} for {tuple(input.shape)}')
+    if prop_step < 0:
+        raise ValueError(f'prop_step must be >= 0, got {prop_step}')
+    if input.dtype != torch.float32 or gate_weight.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    B, C = input.shape[:2]
+    per_channel = C > 1 and gate_weight.shape[1] == nt * C
+    if gate_weight.shape[0] != B or gate_weight.shape[2:] != input.shape[2:] or not (gate_weight.shape[1] == nt or per_channel):
+        raise ValueError(f'a {"x".join([str(kernel_size)] * nd)} kernel needs gate_weight (B,{nt},...) or, with C > 1 input '
+                         f'channels, (B,{nt}*C,...); got {tuple(gate_weight.shape)} for input {tuple(input.shape)}')
+    if gate_weight.device != input.device:
+        raise RuntimeError('input and gate_weight are on different devices')
+    if not (input.is_cuda and gate_weight.is_cuda):
+        raise _lib.CspnError('affinity_propagate takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return (nd,) + ((B * C, 1) if per_channel else (B, C))
+
+
+def _affinity_propagate_fwd(input, gate_weight, kernel_size, prop_step):
+    """Forward only (no autograd) through cspn{2,3}d_gates_fwd_f32, enqueued on the current stream."""
+    nd, Bi, Ci = _check_gates(input, gate_weight, kernel_size, prop_step)
+    if prop_step == 0:
+        return input
+    L = _lib.lib()
+    g, x = gate_weight.contiguous(), input.contiguous()
+    out = torch.empty_like(x)
+    name = f'cspn{nd}d_gates'
+    with torch.cuda.device(x.device):
+        ws_bytes = getattr(L, f'{name}_workspace_bytes')(Bi, Ci, *x.shape[2:], kernel_size, int(prop_step))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
+        rc = getattr(L, f'{name}_fwd_f32')(_ptr(g), _ptr(x), _ptr(out), Bi, Ci, *x.shape[2:], kernel_size, int(prop_step),
+                                           _ptr(ws), ws_bytes, _stream(x.device))
+    _lib.check(rc, f'{name}_fwd_f32')
+    return out
+
+
+class _AffinityPropagateFn(torch.autograd.Function):
+    """autograd seam of affinity_propagate without the torch-op shim: native forward + native adjoint
+    (cspn{2,3}d_gates_bwd_f32)."""
+
+    @staticmethod
+    def forward(ctx, input, gate_weight, kernel_size, prop_step):
+        ctx.save_for_backward(input, gate_weight)
+        ctx.cfg = (kernel_size, prop_step)
+        return _affinity_propagate_fwd(input, gate_weight, kernel_size, prop_step)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        input, gate_weight = ctx.saved_tensors
+        kernel_size, prop_step = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        nd, Bi, Ci = _check_gates(input, gate_weight, kernel_size, prop_step)
+        L = _lib.lib()
+        x, g, go = input.contiguous(), gate_weight.contiguous(), grad_out.contiguous()
+        gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        gg = torch.empty_like(g) if ctx.needs_input_grad[1] else None
+        name = f'cspn{nd}d_gates'
+        with torch.cuda.device(x.device):
+            ws_bytes = getattr(L, f'{name}_bwd_workspace_bytes')(Bi, Ci, *x.shape[2:], kernel_size, int(prop_step))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
+            rc = getattr(L, f'{name}_bwd_f32')(_ptr(g), _ptr(x), _ptr(go), _ptr(gg), _ptr(gx), Bi, Ci, *x.shape[2:], kernel_size,
+                                               int(prop_step), _ptr(ws), ws_bytes, _stream(x.device))
+        _lib.check(rc, f'{name}_bwd_f32')
+        return gx, gg, None, None
+
+
+def affinity_propagate(input, gate_weight, kernel_size=3, prop_step=1):
+    """fluid.layers.affinity_propagate(input, gate_weight, kernel_size), the op the Paddle module calls once per step
+    (cspn_paddle/demo.py:41-43, 51-52), run prop_step times with the gates exactly as given:
+        d_{t+1}(p) = sum_k gate_k(p) * d_t(p + off_k),   d_0 = input,
+    zero padding, no centre term, no normalisation (the caller normalises: cspn_paddle/README.md:54).  A 4-D input
+    (B, C, H, W) is 2D with kernel_size 3, 5 or 7; a 5-D input (B, C, D, H, W) is 3D with kernel_size 3 or 5.  gate_weight is
+    (B, K**d-1, ...), shared by the C channels, or (B, (K**d-1)*C, ...) with C > 1, one gate per channel.  Taps in the raster
+    order of the K x K (x K) operators (DESIGN.md section 4.11).  Differentiable in both arguments; fp32 CUDA tensors only;
+    prop_step == 0 returns input itself."""
+    _check_gates(input, gate_weight, kernel_size, prop_step)
+    if prop_step == 0:
+        return input
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        op = torch.ops.cspn_b200.affinity_propagate2d if input.dim() == 4 else torch.ops.cspn_b200.affinity_propagate3d
+        return op(input, gate_weight, kernel_size, prop_step)
+    if torch.is_grad_enabled() and (input.requires_grad or gate_weight.requires_grad):
+        return _AffinityPropagateFn.apply(input, gate_weight, kernel_size, prop_step)
+    return _affinity_propagate_fwd(input, gate_weight, kernel_size, prop_step)

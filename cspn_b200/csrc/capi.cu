@@ -394,6 +394,97 @@ int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const float* grad
     return rc;
 }
 
+// ---- caller-supplied gates (fluid.layers.affinity_propagate): 2D K in {3, 5, 7}, 3D K in {3, 5} ----------------------
+static int check_gates(const float* gates, const float* feat, const void* out, int B, int C, int D, int H, int W, int K,
+                       int iters, bool is3d) {
+    if (!gates || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d D=%d H=%d W=%d", B, C, D, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (is3d ? (K != 3 && K != 5) : !kernel_size_ok(K)) { set_error("%s kernel size must be %s, got %d", is3d ? "3D" : "2D", is3d ? "3 or 5" : "3, 5 or 7", K); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (iters < 0) { set_error("prop_step must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+size_t cspn2d_gates_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
+    return widek_gates_workspace_bytes(B, C, H, W, iters);
+}
+
+int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out, int B, int C, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, out, B, C, 1, H, W, K, iters, false);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
+    int launches = 0;
+    rc = widek_gates_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn2d_gates_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
+    return widek_gates_bwd_workspace_bytes(B, C, H, W, iters);
+}
+
+int cspn2d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out, float* grad_gates, float* grad_feat,
+                         int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                         cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, grad_out, B, C, 1, H, W, K, iters, false);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{gates, feat, nullptr, nullptr, B, C, H, W, K * K - 1, iters, 0};
+    int launches = 0;
+    rc = widek_gates_backward(p, K, grad_out, grad_gates, grad_feat, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
+    return widek3d_gates_workspace_bytes(B, C, D, H, W, iters);
+}
+
+int cspn3d_gates_fwd_f32(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, out, B, C, D, H, W, K, iters, true);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = widek3d_gates_forward(gates, feat, out, B, C, D, H, W, K, iters, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn3d_gates_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
+    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
+    return widek3d_gates_bwd_workspace_bytes(C, D, H, W, iters);
+}
+
+int cspn3d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out, float* grad_gates, float* grad_feat,
+                         int B, int C, int D, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                         cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, grad_out, B, C, D, H, W, K, iters, true);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = widek3d_gates_backward(gates, feat, grad_out, grad_gates, grad_feat, B, C, D, H, W, K, iters, workspace, workspace_bytes,
+                                (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

@@ -90,6 +90,12 @@ int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad
 int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                           size_t ws_bytes, cudaStream_t stream, int* launches);
+// caller-supplied gates, K in {3, 5, 7}: p.guidance [B][K*K-1][H][W] used as given (p.sparse null, p.gch == K*K-1)
+size_t widek_gates_workspace_bytes(int B, int C, int H, int W, int iters);
+size_t widek_gates_bwd_workspace_bytes(int B, int C, int H, int W, int iters);
+int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,
+                         size_t ws_bytes, cudaStream_t stream, int* launches);
 
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);
@@ -109,5 +115,13 @@ size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters)
 int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
                      int D, int H, int W, int K, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream,
                      int* launches);
+// caller-supplied gates [B][K^3-1][D][H][W], K in {3, 5} (cspn3d_wide.cu)
+size_t widek3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int iters);
+size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters);
+int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
+                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,
+                           int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
+                           int* launches);
 
 }  // namespace cspn

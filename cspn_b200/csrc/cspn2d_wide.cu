@@ -26,6 +26,12 @@
 // step kernels' PADDLE flag drops the kappa d0 term and the d0 load; the adjoint step is shared as it is; the gather's
 // PADDLE flag applies the own-location chain rule (grad_g_j at p, grad_feat = lambda_0).  K = 3 runs here too: the
 // cluster kernel keeps the folded 3x3 form only.
+//
+// Caller-supplied gates (fluid.layers.affinity_propagate itself, DESIGN.md section 4.11), K in {3, 5, 7}:
+//   d_{t+1}(p) = sum_k g_k(p) d_t(p + off_k)   with the gates used as given (no |.|, no normalisation, no centre term).
+// The RAW flag of the step and adjoint kernels reads the caller's gates [image][NT][H][W] (NT planes per image instead of
+// the workspace's NP); there is no prep launch.  The gather's RAW mode writes Gw_k to the gate gradient at p and does
+// not read the gates; the last adjoint step writes lambda_0 straight into the input gradient.
 #include <cstdlib>
 #include <cstring>
 
@@ -111,10 +117,10 @@ prepk_paddle_kernel(const float* __restrict__ guidance, float* __restrict__ wk, 
 // ---- step, 4 pixels of a row per thread (W % 4 == 0, 16-byte aligned cur / d0 / dst / wk) -------------------------
 // Tile 64 x 16 pixels per CTA of 16 x 16 threads.  The shared tile holds rows y0-R .. y0+15+R and columns x0-4 ..
 // x0+67 as float4 (the halo is rounded up to 4 columns so every row of a thread's window is three aligned LDS.128).
-// PADDLE: no kappa d0 term (d0 is not read).
+// PADDLE: no kappa d0 term (d0 is not read).  RAW (with PADDLE): wk is the caller's gates, NT planes per image.
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R, bool PADDLE = false>
+template <int R, bool PADDLE = false, bool RAW = false>
 __global__ void __launch_bounds__(256)
 stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
                  float* __restrict__ dst, int C, int H, int W) {
@@ -136,7 +142,7 @@ stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, con
     const int x = x0 + 4 * tx, y = y0 + ty;
     if (x >= W || y >= H) return;
     const size_t p = (size_t)y * W + x;
-    const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
+    const float* w = wk + (size_t)(bc / C) * (RAW ? T::NT : T::NP) * HW + p;
     float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, acc3 = 0.f;
     if (!PADDLE) {
         const float4 kap = __ldg(reinterpret_cast<const float4*>(w + T::NT * HW));
@@ -177,7 +183,7 @@ __device__ __forceinline__ void load_tile_scalar(float (*tile)[kSclTW + 2 * R], 
     }
 }
 
-template <int R, bool PADDLE = false>
+template <int R, bool PADDLE = false, bool RAW = false>
 __global__ void __launch_bounds__(256)
 stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
                     float* __restrict__ dst, int C, int H, int W) {
@@ -190,15 +196,16 @@ stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, 
     const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
     if (x >= W || y >= H) return;
     const size_t p = (size_t)y * W + x;
-    const float* w = wk + (size_t)(bc / C) * T::NP * HW + p;
+    const float* w = wk + (size_t)(bc / C) * (RAW ? T::NT : T::NP) * HW + p;
     float acc = PADDLE ? 0.f : __ldg(w + T::NT * HW) * __ldg(d0 + (size_t)bc * HW + p);
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
     dst[(size_t)bc * HW + p] = acc;
 }
 
-// lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only
-template <int R>
+// lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only.
+// RAW: wk is the caller's gates, NT planes per image.
+template <int R, bool RAW = false>
 __global__ void __launch_bounds__(256)
 adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out, int C, int H,
             int W) {
@@ -210,7 +217,7 @@ adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, floa
     __syncthreads();
     const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
     if (x >= W || y >= H) return;
-    const float* w = wk + (size_t)(bc / C) * T::NP * HW;
+    const float* w = wk + (size_t)(bc / C) * (RAW ? T::NT : T::NP) * HW;
     float acc = 0.f;
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) {
@@ -226,7 +233,8 @@ adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, floa
 // grid z = image of the group; every pointer is offset to the group's first image.
 // PADDLE (sparse null, gch = NT): the own-location chain rule of cspn3d_wide.cu's fin3k_kernel mode 2 -- no centre term,
 // grad_g_j lands at p, grad_blur = lambda_0.
-template <int R, bool PADDLE = false>
+// RAW (with PADDLE, grad_blur null): the gates are the caller's, so grad_g_k(p) = Gw_k(p); guidance and wk are not read.
+template <int R, bool PADDLE = false, bool RAW = false>
 __global__ void __launch_bounds__(256)
 gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
                const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
@@ -267,6 +275,11 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
         if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
     }
     if (!in || !grad_guidance) return;
+    if (RAW) {
+#pragma unroll
+        for (int k = 0; k < T::NT; ++k) grad_guidance[((size_t)b * T::NT + k) * HW + p] = gw[k];
+        return;
+    }
     const float* g = guidance + (size_t)b * gch * HW;
     if (PADDLE) {
         float S = 0.f;
@@ -337,38 +350,43 @@ void launch_prep(const float* guidance, const float* sparse, float* wk, int nimg
     else prepk_kernel<R><<<grid, block, 0, s>>>(guidance, sparse, wk, H, W, gch, norm_abs);
 }
 
-template <int R, bool PADDLE>
+template <int R, bool PADDLE, bool RAW = false>
 void launch_step(bool vec, const float* wk, const float* d0, const float* cur, float* dst, int nbc, int C, int H, int W,
                  cudaStream_t s) {
     if (vec)
-        stepk_vec_kernel<R, PADDLE><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
+        stepk_vec_kernel<R, PADDLE, RAW><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
             wk, d0, cur, dst, C, H, W);
     else
-        stepk_scalar_kernel<R, PADDLE><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
+        stepk_scalar_kernel<R, PADDLE, RAW><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
             wk, d0, cur, dst, C, H, W);
 }
 
-template <int R, bool PADDLE>
+// RAW: the caller's gates (p.guidance, NT planes per image) are the weight planes; the workspace holds only the
+// ping-pong buffer
+template <int R, bool PADDLE, bool RAW = false>
 int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) {
-    constexpr int NP = Taps<R>::NP;
+    constexpr int NPL = RAW ? Taps<R>::NT : Taps<R>::NP;   // weight planes per image
     const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
-    float* wk_all = static_cast<float*>(ws);
-    float* tmp_all = wk_all + (size_t)p.B * NP * HW;
-    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(p.out) && aligned16(ws);
+    float* wk_ws = static_cast<float*>(ws);
+    const float* wk_all = RAW ? p.guidance : wk_ws;
+    float* tmp_all = RAW ? wk_ws : wk_ws + (size_t)p.B * NPL * HW;
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(p.out) && aligned16(ws) && (!RAW || aligned16(p.guidance));
     const int G = group_size(p.B);
     for (int b0 = 0; b0 < p.B; b0 += G) {
         const int nimg = p.B - b0 < G ? p.B - b0 : G;
-        float* wk = wk_all + (size_t)b0 * NP * HW;
+        const float* wk = wk_all + (size_t)b0 * NPL * HW;
         const float* blur = p.blur + (size_t)b0 * plane;
         float* out = p.out + (size_t)b0 * plane;
         float* tmp = tmp_all + (size_t)b0 * plane;
-        launch_prep<R, PADDLE>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr, wk, nimg,
-                               p.H, p.W, p.gch, p.norm_abs, stream);
-        ++*launches;
+        if constexpr (!RAW) {
+            launch_prep<R, PADDLE>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr,
+                                   wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+            ++*launches;
+        }
         const float* cur = blur;
         float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < p.iters; ++it) {
-            launch_step<R, PADDLE>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
+            launch_step<R, PADDLE, RAW>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
             ++*launches;
             cur = dst;
             dst = (dst == out) ? tmp : out;
@@ -378,40 +396,54 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) 
     return CSPN_OK;
 }
 
-template <int R, bool PADDLE>
+// RAW: the caller's gates are the weight planes; the workspace holds d_1..d_{N-1} and lambda_1..lambda_{N-1} only.  The
+// last adjoint step writes lambda_0 straight into grad_blur (skipped when that is null), and without grad_guidance the
+// forward steps and the gather, which only feed the gate gradient, are skipped.
+template <int R, bool PADDLE, bool RAW = false>
 int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                cudaStream_t stream, int* launches) {
-    constexpr int NP = Taps<R>::NP;
+    constexpr int NPL = RAW ? Taps<R>::NT : Taps<R>::NP;   // weight planes per image
     const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
     const long long n = (long long)p.B * plane;
-    float* wk_all = static_cast<float*>(ws);
-    float* steps = wk_all + (size_t)p.B * NP * HW;   // steps[t] = d_{t+1}, t < N-1
-    float* lam = steps + (size_t)p.iters * n;        // lam[t]   = lambda_t
-    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(ws);
+    float* wk_ws = static_cast<float*>(ws);
+    const float* wk_all = RAW ? p.guidance : wk_ws;
+    float* steps = RAW ? wk_ws : wk_ws + (size_t)p.B * NPL * HW;        // steps[t] = d_{t+1}, t < N-1
+    // lam[t] = lambda_t; RAW keeps 1 <= t < N only, right after the steps
+    float* lam = RAW ? steps + (size_t)(p.iters >= 2 ? p.iters - 2 : 0) * n : steps + (size_t)p.iters * n;
+    const bool gates_grad = !RAW || grad_guidance;   // the steps and the gather feed the guidance gradient
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(ws) && (!RAW || aligned16(p.guidance));
     const int G = group_size(p.B);
     for (int b0 = 0; b0 < p.B; b0 += G) {
         const int nimg = p.B - b0 < G ? p.B - b0 : G;
         const size_t off = (size_t)b0 * plane;
-        float* wk = wk_all + (size_t)b0 * NP * HW;
+        const float* wk = wk_all + (size_t)b0 * NPL * HW;
         const float* blur = p.blur + off;
         const float* guidance = p.guidance + (size_t)b0 * p.gch * HW;
         const float* sparse = p.sparse ? p.sparse + (size_t)b0 * HW : nullptr;
-        launch_prep<R, PADDLE>(guidance, sparse, wk, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
-        ++*launches;
-        for (int t = 0; t + 1 < p.iters; ++t) {        // d_{t+1} = step(d_t)
-            launch_step<R, PADDLE>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
+        if constexpr (!RAW) {
+            launch_prep<R, PADDLE>(guidance, sparse, wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+            ++*launches;
+        }
+        for (int t = 0; gates_grad && t + 1 < p.iters; ++t) {   // d_{t+1} = step(d_t)
+            launch_step<R, PADDLE, RAW>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
                            nimg * p.C, p.C, p.H, p.W, stream);
             ++*launches;
         }
         const dim3 grid((p.W + kSclTW - 1) / kSclTW, (p.H + kSclTH - 1) / kSclTH, nimg * p.C);
         for (int t = p.iters - 1; t >= 0; --t) {        // lambda_t from lambda_{t+1}
             const float* lin = (t == p.iters - 1 ? grad_out : lam + (size_t)(t + 1) * n) + off;
-            adjk_kernel<R><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lam + (size_t)t * n + off, p.C, p.H, p.W);
+            float* lout = lam + (size_t)t * n + off;
+            if (RAW && t == 0) {                        // lambda_0 is grad_blur
+                if (!grad_blur) continue;
+                lout = grad_blur + off;
+            }
+            adjk_kernel<R, RAW><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lout, p.C, p.H, p.W);
             ++*launches;
         }
-        gatherk_kernel<R, PADDLE><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
+        if (!gates_grad) continue;
+        gatherk_kernel<R, PADDLE, RAW><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
             guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off,
-            grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr, grad_blur ? grad_blur + off : nullptr, n,
+            grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr, grad_blur && !RAW ? grad_blur + off : nullptr, n,
             p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
         ++*launches;
     }
@@ -501,6 +533,57 @@ int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, floa
     if (K == 3) return backward_k<1, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
     return K == 5 ? backward_k<2, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
                   : backward_k<3, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+}
+
+// Caller-supplied gates: p.guidance [B][K*K-1][H][W] used as given, p.sparse null, p.gch == K*K-1 (the C ABI sets both)
+size_t widek_gates_workspace_bytes(int B, int C, int H, int W, int iters) {
+    return iters >= 2 ? sizeof(float) * (size_t)B * C * H * W : 0;
+}
+
+size_t widek_gates_bwd_workspace_bytes(int B, int C, int H, int W, int iters) {
+    return iters >= 2 ? sizeof(float) * (2 * (size_t)iters - 2) * B * C * H * W : 0;
+}
+
+static bool gates_grid_ok(const Problem2D& p, int K, const char* what) {
+    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D gates %s: B*C=%lld exceeds gridDim.z", K, K, what, (long long)p.B * p.C); return false; }
+    if ((p.H + kSclTH - 1) / kSclTH > 65535) { set_error("%dx%d 2D gates %s: H=%d exceeds gridDim.y", K, K, what, p.H); return false; }
+    return true;
+}
+
+int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+    if (p.iters == 0) {
+        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_gates_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%d 2D gates path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if (!gates_grid_ok(p, K, "path")) return CSPN_ERR_UNSUPPORTED;
+    if (K == 3) return forward_k<1, true, true>(p, ws, stream, launches);
+    return K == 5 ? forward_k<2, true, true>(p, ws, stream, launches) : forward_k<3, true, true>(p, ws, stream, launches);
+}
+
+int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,
+                         size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
+    if (p.iters == 0) {   // the identity: no dependence on the gates
+        if (grad_gates) CSPN_CUDA_TRY(cudaMemsetAsync(grad_gates, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
+        if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek_gates_bwd_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%d 2D gates backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if (!gates_grid_ok(p, K, "backward")) return CSPN_ERR_UNSUPPORTED;
+    if (!grad_gates && !grad_feat) return CSPN_OK;
+    // every gate gradient is written by the gather (g_k(p) feeds pixel p alone; a tap that reads the padding gets 0)
+    if (K == 3) return backward_k<1, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches);
+    return K == 5 ? backward_k<2, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches)
+                  : backward_k<3, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches);
 }
 
 }  // namespace cspn

@@ -20,6 +20,13 @@
 // (lambda_{t+1} tile + halo in shared memory), K gather launches -- one per z-slab of the window, 25 register accumulators
 // Gw_k(p) = sum_c sum_t lambda_{t+1}(p) d_t(p + off_k) each, written over the then dead weight planes -- and one finalize
 // with the chain rule of cspn3d.cu's bwd3d_finalize_kernel over 124 taps.
+//
+// Caller-supplied gates (fluid.layers.affinity_propagate itself, DESIGN.md section 4.11), K in {3, 5}:
+//   d_{t+1}(p) = sum_k g_k(p) d_t(p + off_k)   with the gates used as given (no |.|, no division, no centre term).
+// The step kernels' RAW mode reads the caller's gates [vol][NT][V] as the weight planes: no prep, no cold-sum branch.  The
+// backward runs the staged form above on the gates themselves: the adjoint reads the volume's gates, the last adjoint writes
+// lambda_0 straight into grad_feat, and the K gather launches write Gw_k straight into grad_gates (no prep, no finalize).
+// K = 3 runs here on R = 1 instantiations; cspn3d.cu keeps the 3x3x3 operator.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -97,11 +104,12 @@ prep3k_kernel(const float* __restrict__ g, float* __restrict__ wk, int D, int H,
 // ---- step, 4 voxels of a row per thread (W % 4 == 0, 16-byte aligned pointers) ----------------------------------
 // CTA tile 64 x 16 voxels of one z-plane, 16 x 16 threads.  The shared tile holds planes z-R .. z+R, rows y0-R .. y0+15+R
 // and columns x0-4 .. x0+67 as float4 (the halo rounded up to 4 columns: a thread's window row is three aligned LDS.128).
-// PADDLE: w = raw guidance [vol][NT][V], out = sum_k |g_k| d_t(p+off_k) / sum_k |g_k|.  Otherwise w = weight planes
-// [vol][NP][V], out = kappa d0 + sum_k w_k d_t(p+off_k), or without the kappa term when d0 is null ('paddle' planes).
+// PADDLE: w = raw guidance [vol][NT][V], out = sum_k |g_k| d_t(p+off_k) / sum_k |g_k|.  RAW: w = the caller's gates
+// [vol][NT][V], out = sum_k g_k d_t(p+off_k).  Otherwise w = weight planes [vol][NP][V], out = kappa d0 + sum_k w_k
+// d_t(p+off_k), or without the kappa term when d0 is null ('paddle' planes).
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R, bool PADDLE>
+template <int R, bool PADDLE, bool RAW = false>
 __global__ void __launch_bounds__(256)
 step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, const float* __restrict__ cur,
                   float* __restrict__ dst, int C, int D, int H, int W) {
@@ -124,9 +132,9 @@ step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, con
     const int x = x0 + 4 * tx, y = y0 + ty;
     if (x >= W || y >= H) return;
     const size_t p = (size_t)z * HW + (size_t)y * W + x;
-    const float* wp = w + (size_t)(bc / C) * (PADDLE ? T::NT : T::NP) * V + p;
+    const float* wp = w + (size_t)(bc / C) * (PADDLE || RAW ? T::NT : T::NP) * V + p;
     float acc[4] = {0.f, 0.f, 0.f, 0.f}, S[4] = {0.f, 0.f, 0.f, 0.f};
-    if (!PADDLE && d0) {
+    if (!PADDLE && !RAW && d0) {
         const float4 kap = ld_stream4(wp + T::NT * V);
         const float4 dd = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)bc * V + p));
         acc[0] = kap.x * dd.x; acc[1] = kap.y * dd.y; acc[2] = kap.z * dd.z; acc[3] = kap.w * dd.w;
@@ -191,7 +199,7 @@ __device__ __forceinline__ void load_tile3_scalar(float (*tile)[kSclTH + 2 * R][
     }
 }
 
-template <int R, bool PADDLE>
+template <int R, bool PADDLE, bool RAW = false>
 __global__ void __launch_bounds__(256)
 step3k_scalar_kernel(const float* __restrict__ w, const float* __restrict__ d0, const float* __restrict__ cur,
                      float* __restrict__ dst, int C, int D, int H, int W) {
@@ -205,8 +213,8 @@ step3k_scalar_kernel(const float* __restrict__ w, const float* __restrict__ d0, 
     const int tx = threadIdx.x, ty = threadIdx.y, x = x0 + tx, y = y0 + ty;
     if (x >= W || y >= H) return;
     const size_t p = ((size_t)z * H + y) * W + x;
-    const float* wp = w + (size_t)(bc / C) * (PADDLE ? T::NT : T::NP) * V + p;
-    float acc = (!PADDLE && d0) ? __ldg(wp + T::NT * V) * __ldg(d0 + (size_t)bc * V + p) : 0.f, S = 0.f;
+    const float* wp = w + (size_t)(bc / C) * (PADDLE || RAW ? T::NT : T::NP) * V + p;
+    float acc = (!PADDLE && !RAW && d0) ? __ldg(wp + T::NT * V) * __ldg(d0 + (size_t)bc * V + p) : 0.f, S = 0.f;
 #pragma unroll 1
     for (int f = 0; f < T::K; ++f) {
 #pragma unroll
@@ -368,17 +376,20 @@ fin3k_kernel(const float* __restrict__ g, const float* __restrict__ feat, const 
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int R>
+// RAW: w is the caller's gates (the step with PADDLE false and RAW true); otherwise `paddle` picks the PADDLE mode
+template <int R, bool RAW = false>
 void launch_step(bool vec, bool paddle, const float* w, const float* d0, const float* cur, float* dst, int nbc, int C, int D,
                  int H, int W, cudaStream_t s) {
     const unsigned gz = (unsigned)(D * nbc);
     if (vec) {
         const dim3 grid((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, gz), block(16, 16);
-        if (paddle) step3k_vec_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
+        if constexpr (RAW) step3k_vec_kernel<R, false, true><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W);
+        else if (paddle) step3k_vec_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
         else step3k_vec_kernel<R, false><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
     } else {
         const dim3 grid((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, gz), block(kSclTW, kSclTH);
-        if (paddle) step3k_scalar_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
+        if constexpr (RAW) step3k_scalar_kernel<R, false, true><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W);
+        else if (paddle) step3k_scalar_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
         else step3k_scalar_kernel<R, false><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
     }
 }
@@ -456,6 +467,80 @@ int backward_3k(const float* guidance, const float* feat, const float* grad_out,
     return CSPN_OK;
 }
 
+// ---- caller-supplied gates --------------------------------------------------------------------------------------
+// Volumes per launch group: those of the paths above with no weight planes; one step needs no ping-pong buffer, so then
+// only gridDim.z bounds the group.
+int gates_group(int B, int C, int D, int H, int W, int iters) {
+    if (iters > 1) return group3d(B, C, D, H, W, iters, 0);
+    const long long gz = 65535 / ((long long)D * C);
+    return (int)(gz < 1 ? 1 : (gz < B ? gz : B));
+}
+
+template <int R>
+int forward_gates_3k(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int iters, void* ws,
+                     cudaStream_t stream, int* launches) {
+    using T = Taps3<R>;
+    const size_t V = (size_t)D * H * W, n = (size_t)C * V;
+    const int G = gates_group(B, C, D, H, W, iters);
+    float* tmp = static_cast<float*>(ws);   // [G][C][V] when iters > 1
+    const bool vec = W % 4 == 0 && aligned16(gates) && aligned16(feat) && aligned16(out) && aligned16(ws);
+    for (int b0 = 0; b0 < B; b0 += G) {
+        const int nvol = B - b0 < G ? B - b0 : G;
+        const float* g = gates + (size_t)b0 * T::NT * V;
+        float* o = out + (size_t)b0 * n;
+        const float* cur = feat + (size_t)b0 * n;
+        float* dst = (iters & 1) ? o : tmp;   // ping-pong so that the last step writes out
+        for (int it = 0; it < iters; ++it) {
+            launch_step<R, true>(vec, false, g, nullptr, cur, dst, nvol * C, C, D, H, W, stream);
+            ++*launches;
+            cur = dst;
+            dst = (dst == o) ? tmp : o;
+        }
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
+// One volume at a time: N-1 forward steps keep d_1..d_{N-1}, N adjoint steps on the gates keep lambda_1..lambda_{N-1} and
+// write lambda_0 = grad_feat, and the K gather launches write Gw_k = grad_gates.  Workspace (2N-2)*C*V floats.  Without
+// grad_g the forward steps and the gathers, which only feed it, are skipped; without grad_feat the last adjoint is.
+template <int R>
+int backward_gates_3k(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
+                      int D, int H, int W, int iters, void* ws, cudaStream_t stream, int* launches) {
+    using T = Taps3<R>;
+    const size_t V = (size_t)D * H * W, n = (size_t)C * V;
+    float* steps = static_cast<float*>(ws);                         // steps[t] = d_{t+1}, t < N-1
+    float* lam = steps + (size_t)(iters >= 2 ? iters - 2 : 0) * n;   // lam + t*n = lambda_t for 1 <= t < N (after steps)
+    const bool vec = W % 4 == 0 && aligned16(gates) && aligned16(feat) && aligned16(ws);
+    const dim3 block(kSclTW, kSclTH), grid((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, D);
+    for (int b = 0; b < B; ++b) {
+        const float* g = gates + (size_t)b * T::NT * V;
+        const float* d0 = feat + (size_t)b * n;
+        const float* go = grad_out + (size_t)b * n;
+        for (int t = 0; grad_g && t + 1 < iters; ++t) {   // d_{t+1} = step(d_t)
+            launch_step<R, true>(vec, false, g, nullptr, t == 0 ? d0 : steps + (size_t)(t - 1) * n, steps + (size_t)t * n, C, C,
+                                 D, H, W, stream);
+            ++*launches;
+        }
+        for (int t = iters - 1; t >= 0; --t) {          // lambda_t from lambda_{t+1}; lambda_0 is grad_feat
+            float* lout = t == 0 ? (grad_feat ? grad_feat + (size_t)b * n : nullptr) : lam + (size_t)t * n;
+            if (!lout) continue;
+            adj3k_kernel<R><<<dim3(grid.x, grid.y, D * C), block, 0, stream>>>(
+                g, t == iters - 1 ? go : lam + (size_t)(t + 1) * n, lout, D, H, W);
+            ++*launches;
+        }
+        if (grad_g) {
+            for (int f = 0; f < T::K; ++f) {            // Gw_k = grad_g_k, one z-slab of taps per launch
+                gather3k_kernel<R><<<grid, block, 0, stream>>>(d0, steps, lam, go, grad_g + (size_t)b * T::NT * V, (long long)n, iters,
+                                                               C, D, H, W, f);
+                ++*launches;
+            }
+        }
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
 bool grid_ok(int C, int D, int H, const char* what, int K) {
     if ((long long)D * C > 65535) {
         set_error("%dx%dx%d 3D %s: D*C=%lld exceeds gridDim.z", K, K, K, what, (long long)D * C);
@@ -514,6 +599,54 @@ int widek3d_backward(const float* guidance, const float* feat, const float* grad
     }
     if (!grid_ok(C, D, H, "backward", K)) return CSPN_ERR_UNSUPPORTED;
     return backward_3k<2>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, mode, ws, stream, launches);
+}
+
+// Caller-supplied gates [B][K^3-1][D][H][W], used as given, K in {3, 5}
+size_t widek3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
+    if (iters <= 1) return 0;
+    return sizeof(float) * (size_t)gates_group(B, C, D, H, W, iters) * C * D * H * W;
+}
+
+size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters) {
+    if (iters <= 1) return 0;
+    return sizeof(float) * (2 * (size_t)iters - 2) * C * D * H * W;
+}
+
+int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
+                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+    if (iters == 0) {
+        CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * D * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek3d_gates_workspace_bytes(B, C, D, H, W, iters);
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%dx%d 3D gates path needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if (!grid_ok(C, D, H, "gates path", K)) return CSPN_ERR_UNSUPPORTED;
+    return K == 3 ? forward_gates_3k<1>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches)
+                  : forward_gates_3k<2>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches);
+}
+
+int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,
+                           int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
+                           int* launches) {
+    const size_t V = (size_t)D * H * W;
+    if (iters == 0) {   // the identity: no dependence on the gates
+        if (grad_g) CSPN_CUDA_TRY(cudaMemsetAsync(grad_g, 0, (size_t)B * (K * K * K - 1) * V * sizeof(float), stream));
+        if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, (size_t)B * C * V * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        return CSPN_OK;
+    }
+    const size_t need = widek3d_gates_bwd_workspace_bytes(C, D, H, W, iters);
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%dx%d 3D gates backward needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if (!grid_ok(C, D, H, "gates backward", K)) return CSPN_ERR_UNSUPPORTED;
+    if (!grad_g && !grad_feat) return CSPN_OK;
+    // every gate gradient is written by the gathers (g_k(p) feeds voxel p alone; a tap that reads the padding gets 0)
+    return K == 3 ? backward_gates_3k<1>(gates, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches)
+                  : backward_gates_3k<2>(gates, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches);
 }
 
 }  // namespace cspn

@@ -25,6 +25,12 @@
 //       (K x K x K kernel, K in {3, 5}; K = 3 is propagate3d)
 //   propagate3d_k_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, int norm_type,
 //                          bool need_guidance, bool need_feat) -> (Tensor, Tensor)
+//   affinity_propagate2d(Tensor input, Tensor gate_weight, int kernel_size, int prop_step) -> Tensor
+//       (fluid.layers.affinity_propagate with the caller's gates, K in {3, 5, 7}; gate_weight (B, K*K-1, H, W) shared, or
+//       (B, (K*K-1)*C, H, W) per channel)
+//   affinity_propagate2d_backward(Tensor input, Tensor gate_weight, Tensor grad_out, int kernel_size, int prop_step,
+//                                 bool need_input, bool need_gate) -> (Tensor, Tensor)
+//   affinity_propagate3d / affinity_propagate3d_backward: the same for (B, C, D, H, W), K in {3, 5}
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -325,6 +331,94 @@ std::tuple<at::Tensor, at::Tensor> propagate3d_k_backward_cuda(const at::Tensor&
     return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
 }
 
+// caller-supplied gates (fluid.layers.affinity_propagate), nd = 2 (K in {3, 5, 7}) or 3 (K in {3, 5}).  Returns the
+// (images, channels) the C ABI is called with: per-channel gates are B*C images of one channel.
+std::pair<int, int> check_gates(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step, int nd) {
+    TORCH_CHECK_VALUE(input.dim() == nd + 2 && gate.dim() == nd + 2, "input and gate_weight must be ",
+                      nd == 2 ? "(B,C,H,W)" : "(B,C,D,H,W)");
+    TORCH_CHECK_VALUE(nd == 2 ? (K == 3 || K == 5 || K == 7) : (K == 3 || K == 5), "kernel_size of a ", nd,
+                      "D affinity_propagate must be ", nd == 2 ? "3, 5 or 7" : "3 or 5", ", got ", K);
+    TORCH_CHECK_VALUE(prop_step >= 0, "prop_step must be >= 0, got ", prop_step);
+    TORCH_CHECK(input.scalar_type() == at::kFloat && gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    const int64_t nt = (nd == 2 ? K * K : K * K * K) - 1, B = input.size(0), C = input.size(1);
+    bool shape_ok = gate.size(0) == B;
+    for (int i = 2; i < nd + 2; ++i) shape_ok = shape_ok && gate.size(i) == input.size(i);
+    const bool per_channel = C > 1 && gate.size(1) == nt * C;
+    TORCH_CHECK_VALUE(shape_ok && (gate.size(1) == nt || per_channel), "a kernel of size ", K, " needs gate_weight (B,", nt,
+                      ",...) or, with C > 1 input channels, (B,", nt, "*C,...); got ", gate.sizes(), " for input ", input.sizes());
+    TORCH_CHECK(gate.device() == input.device(), "input and gate_weight are on different devices");
+    return per_channel ? std::make_pair((int)(B * C), 1) : std::make_pair((int)B, (int)C);
+}
+
+at::Tensor affinity_propagate_cuda(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step, int nd) {
+    const auto [B, C] = check_gates(input, gate, K, prop_step, nd);
+    if (prop_step == 0) return input.clone();
+    const c10::cuda::CUDAGuard guard(input.device());
+    const at::Tensor g = gate.contiguous(), x = input.contiguous();
+    at::Tensor out = at::empty_like(x);
+    const auto stream = (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream();
+    const int H = (int)x.size(nd), W = (int)x.size(nd + 1), D = nd == 3 ? (int)x.size(2) : 1;
+    const size_t ws_bytes = nd == 2 ? cspn2d_gates_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
+                                    : cspn3d_gates_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, x.options().dtype(at::kByte));
+    void* w = ws_bytes ? ws.data_ptr() : nullptr;
+    if (nd == 2)
+        check_rc(cspn2d_gates_fwd_f32(fptr(g), fptr(x), out.data_ptr<float>(), B, C, H, W, (int)K, (int)prop_step, w, ws_bytes, stream),
+                 "cspn2d_gates_fwd_f32");
+    else
+        check_rc(cspn3d_gates_fwd_f32(fptr(g), fptr(x), out.data_ptr<float>(), B, C, D, H, W, (int)K, (int)prop_step, w, ws_bytes,
+                                      stream),
+                 "cspn3d_gates_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> affinity_propagate_backward_cuda(const at::Tensor& input, const at::Tensor& gate,
+                                                                    const at::Tensor& grad_out, int64_t K, int64_t prop_step,
+                                                                    bool need_x, bool need_g, int nd) {
+    const auto [B, C] = check_gates(input, gate, K, prop_step, nd);
+    TORCH_CHECK(grad_out.sizes() == input.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == input.device(),
+                "grad_out must match input");
+    const c10::cuda::CUDAGuard guard(input.device());
+    const at::Tensor g = gate.contiguous(), x = input.contiguous(), go = grad_out.contiguous();
+    at::Tensor gx = need_x ? at::empty_like(x) : at::Tensor();
+    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
+    const auto stream = (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream();
+    const int H = (int)x.size(nd), W = (int)x.size(nd + 1), D = nd == 3 ? (int)x.size(2) : 1;
+    const size_t ws_bytes = nd == 2 ? cspn2d_gates_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
+                                    : cspn3d_gates_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step);
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, x.options().dtype(at::kByte));
+    void* w = ws_bytes ? ws.data_ptr() : nullptr;
+    float* pgg = need_g ? gg.data_ptr<float>() : nullptr;
+    float* pgx = need_x ? gx.data_ptr<float>() : nullptr;
+    if (nd == 2)
+        check_rc(cspn2d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), pgg, pgx, B, C, H, W, (int)K, (int)prop_step, w, ws_bytes, stream),
+                 "cspn2d_gates_bwd_f32");
+    else
+        check_rc(cspn3d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), pgg, pgx, B, C, D, H, W, (int)K, (int)prop_step, w, ws_bytes,
+                                      stream),
+                 "cspn3d_gates_bwd_f32");
+    return {need_x ? gx : at::zeros({0}, x.options()), need_g ? gg : at::zeros({0}, g.options())};
+}
+
+at::Tensor affinity_propagate2d_cuda(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step) {
+    return affinity_propagate_cuda(input, gate, K, prop_step, 2);
+}
+at::Tensor affinity_propagate3d_cuda(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step) {
+    return affinity_propagate_cuda(input, gate, K, prop_step, 3);
+}
+std::tuple<at::Tensor, at::Tensor> affinity_propagate2d_backward_cuda(const at::Tensor& input, const at::Tensor& gate,
+                                                                      const at::Tensor& grad_out, int64_t K, int64_t prop_step,
+                                                                      bool need_x, bool need_g) {
+    return affinity_propagate_backward_cuda(input, gate, grad_out, K, prop_step, need_x, need_g, 2);
+}
+std::tuple<at::Tensor, at::Tensor> affinity_propagate3d_backward_cuda(const at::Tensor& input, const at::Tensor& gate,
+                                                                      const at::Tensor& grad_out, int64_t K, int64_t prop_step,
+                                                                      bool need_x, bool need_g) {
+    return affinity_propagate_backward_cuda(input, gate, grad_out, K, prop_step, need_x, need_g, 3);
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -344,6 +438,12 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate3d_k(Tensor guidance, Tensor feat, int kernel_size, int prop_time, int norm_type) -> Tensor");
     m.def("propagate3d_k_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, int norm_type, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
+    m.def("affinity_propagate2d(Tensor input, Tensor gate_weight, int kernel_size, int prop_step) -> Tensor");
+    m.def("affinity_propagate2d_backward(Tensor input, Tensor gate_weight, Tensor grad_out, int kernel_size, int prop_step, "
+          "bool need_input, bool need_gate) -> (Tensor, Tensor)");
+    m.def("affinity_propagate3d(Tensor input, Tensor gate_weight, int kernel_size, int prop_step) -> Tensor");
+    m.def("affinity_propagate3d_backward(Tensor input, Tensor gate_weight, Tensor grad_out, int kernel_size, int prop_step, "
+          "bool need_input, bool need_gate) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -357,4 +457,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate3d_backward", &propagate3d_backward_cuda);
     m.impl("propagate3d_k", &propagate3d_k_cuda);
     m.impl("propagate3d_k_backward", &propagate3d_k_backward_cuda);
+    m.impl("affinity_propagate2d", &affinity_propagate2d_cuda);
+    m.impl("affinity_propagate2d_backward", &affinity_propagate2d_backward_cuda);
+    m.impl("affinity_propagate3d", &affinity_propagate3d_cuda);
+    m.impl("affinity_propagate3d_backward", &affinity_propagate3d_backward_cuda);
 }

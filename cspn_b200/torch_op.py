@@ -22,7 +22,9 @@ _loaded = False
 
 
 def available():
-    return os.path.isfile(TORCH_LIB_PATH) and os.path.isfile(_lib.LIB_PATH)
+    # once loaded, the shim stays available: no file-system lookups on the per-call path of affinity_propagate (a stat on
+    # a network file system can take longer than a small propagation)
+    return _loaded or (os.path.isfile(TORCH_LIB_PATH) and os.path.isfile(_lib.LIB_PATH))
 
 
 def load():
@@ -181,6 +183,45 @@ def _register():
         return (gg if need_g else None), (gf if need_f else None), None, None, None
 
     lib.register_autograd('cspn_b200::propagate3d_k', backward3d_k, setup_context=setup3d_k)
+
+    for nd in (2, 3):
+        _register_gates(lib, nd)
+
+
+def _register_gates(lib, nd):
+    """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""
+    sizes = (3, 5, 7) if nd == 2 else (3, 5)
+
+    @lib.register_fake(f'cspn_b200::affinity_propagate{nd}d')
+    def _(input, gate_weight, kernel_size, prop_step):
+        torch._check(input.dim() == nd + 2 and gate_weight.dim() == nd + 2,
+                     lambda: f'input and gate_weight must have {nd + 2} dimensions')
+        torch._check(kernel_size in sizes, lambda: f'kernel_size of a {nd}D affinity_propagate must be one of {sizes}')
+        nt = kernel_size ** nd - 1
+        torch._check(gate_weight.shape[1] == nt or (input.shape[1] > 1 and gate_weight.shape[1] == nt * input.shape[1]),
+                     lambda: f'a kernel of size {kernel_size} needs {nt} or {nt}*C gate channels')
+        return torch.empty_like(input, memory_format=torch.contiguous_format)
+
+    @lib.register_fake(f'cspn_b200::affinity_propagate{nd}d_backward')
+    def _(input, gate_weight, grad_out, kernel_size, prop_step, need_input, need_gate):
+        gx = torch.empty_like(input, memory_format=torch.contiguous_format) if need_input else input.new_empty(0)
+        gg = torch.empty_like(gate_weight, memory_format=torch.contiguous_format) if need_gate else gate_weight.new_empty(0)
+        return gx, gg
+
+    def setup(ctx, inputs, output):
+        input, gate_weight, kernel_size, prop_step = inputs
+        ctx.save_for_backward(input, gate_weight)
+        ctx.cfg = (kernel_size, prop_step)
+
+    def backward(ctx, grad_out):
+        input, gate_weight = ctx.saved_tensors
+        kernel_size, prop_step = ctx.cfg
+        need_x, need_g = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        op = getattr(torch.ops.cspn_b200, f'affinity_propagate{nd}d_backward')
+        gx, gg = op(input, gate_weight, grad_out.contiguous(), kernel_size, prop_step, need_x, need_g)
+        return (gx if need_x else None), (gg if need_g else None), None, None
+
+    lib.register_autograd(f'cspn_b200::affinity_propagate{nd}d', backward, setup_context=setup)
 
 
 def propagate2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum', algo=_lib.ALGO_AUTO):

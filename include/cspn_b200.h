@@ -206,6 +206,49 @@ CSPN_API int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const fl
                      int B, int C, int D, int H, int W, int K, int iters, int norm_type,
                      void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- caller-supplied gates: fluid.layers.affinity_propagate(input, gate_weight, kernel_size) itself -----------------
+ * The Paddle op the reference calls once per step (cspn_paddle/demo.py:41-43, 51-52), with its gates already normalised by
+ * the caller (cspn_paddle/README.md:54), run `iters` times:
+ *   d_{t+1}(p) = sum_k g_k(p) d_t(p + off_k),  d_0 = feat,
+ * with the gates used exactly as given (no |.|, no normalisation, no centre term, no sparse replacement), zero padding and
+ * IEEE arithmetic (inf * 0 = NaN where a tap reads the padding).  Taps as in the K x K (2D) and K x K x K (3D) calls above.
+ * gates [B][K^d-1][(D)][H][W], one gate shared by the C channels of feat / out / grad_feat [B][C][(D)][H][W]; per-channel
+ * gates (demo.py:28-45, [B][(K^d-1)*C]...) are the same memory as B*C volumes with C = 1.  grad_gates has the shape of
+ * gates; either gradient may be NULL, and the backward then skips the work that only feeds it (without grad_gates it
+ * runs the adjoint steps alone).  2D: K in {3, 5, 7}; 3D: K in {3, 5}.
+ * Workspace (0 for iters == 0; none depends on the device):
+ *   2D forward   B*C*H*W floats for iters >= 2, else 0;
+ *   2D backward  (2*iters-2)*B*C*H*W floats (lambda_0 is written straight into grad_feat);
+ *   3D forward   G*C*D*H*W floats for iters >= 2, else 0, with G the volumes per launch group (all B unless that exceeds
+ *                4 GiB or gridDim.z);
+ *   3D backward  (2*iters-2)*C*D*H*W floats (one volume at a time; lambda_0 is written straight into grad_feat).
+ * CSPN_ERR_INVALID_ARGUMENT for a bad K, iters < 0, a non-positive shape or a null gates / feat / out (grad_out in the
+ * backward); CSPN_ERR_UNSUPPORTED for a shape the launch grid cannot take (B*C > 65535 in 2D, D*C > 65535 in 3D, or
+ * H > 524280). */
+CSPN_API size_t cspn2d_gates_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out,
+                         int B, int C, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_gates_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out,
+                         float* grad_gates, float* grad_feat, int B, int C, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+
+CSPN_API int cspn3d_gates_fwd_f32(const float* gates, const float* feat, float* out,
+                         int B, int C, int D, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn3d_gates_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+
+CSPN_API int cspn3d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out,
+                         float* grad_gates, float* grad_feat, int B, int C, int D, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
