@@ -82,14 +82,15 @@ def cspn3d_ref(guidance, feat, prop_time, K, norm_type):
 
 
 # ---- dyadic inputs ----------------------------------------------------------------------------------------------------
-def hot_taps(gen, n, valid):
-    """(n, taps, *S) bool: at each site m in {1, 2, 4} distinct taps among the `valid` ones ((taps, *S) bool), m capped at
-    the largest power of two the valid taps allow.  Random keys, -inf on invalid taps, the top m win."""
+def hot_taps(gen, n, valid, ms=(1, 2, 4)):
+    """(n, taps, *S) bool: at each site m in `ms` (powers of two up to 4) distinct taps among the `valid` ones
+    ((taps, *S) bool), m capped at the largest power of two the valid taps allow.  Random keys, -inf on invalid taps, the
+    top m win."""
     taps, shape = valid.shape[0], valid.shape[1:]
     nvalid = valid.sum(0)
     assert nvalid.min() >= 1, 'a site without a valid tap'
     cap = torch.where(nvalid >= 4, 4, torch.where(nvalid >= 2, 2, 1))
-    m = torch.minimum(torch.tensor([1, 2, 4])[torch.randint(0, 3, (n, *shape), generator=gen)], cap)
+    m = torch.minimum(torch.tensor(ms)[torch.randint(0, len(ms), (n, *shape), generator=gen)], cap)
     keys = torch.rand(n, taps, *shape, generator=gen).masked_fill(~valid, -float('inf'))
     top = keys.topk(4, dim=1).indices
     chosen = torch.arange(4).view(1, 4, *[1] * len(shape)) < m.unsqueeze(1)
@@ -114,11 +115,11 @@ def guidance_from_sites(val, K, gathered):
     return torch.stack([shift(val[:, k], tuple(-o for o in off), r) for k, off in enumerate(offsets(K, nd))], 1)
 
 
-def dyadic_guidance(gen, n, shape, K, gathered):
+def dyadic_guidance(gen, n, shape, K, gathered, ms=(1, 2, 4)):
     nd = len(shape)
     offs = offsets(K, nd)
     valid = inside(shape, offs) if gathered else torch.ones(len(offs), *shape, dtype=torch.bool)
-    val = hot_taps(gen, n, valid).float() * signs(gen, (n, len(offs), *shape))
+    val = hot_taps(gen, n, valid, ms).float() * signs(gen, (n, len(offs), *shape))
     return guidance_from_sites(val, K, gathered)
 
 
@@ -185,12 +186,13 @@ def one_tap_guidance(seed, shape, K, gathered):
 
 
 # ---- exactness --------------------------------------------------------------------------------------------------------
-def check_exact(t, N, what):
-    """The values of an exact case: finite multiples of 4^-(N+1), and below 2^24 in those units."""
-    x = t.detach().double() * 4.0 ** (N + 1)
+def check_exact(t, N, what, unit=None):
+    """The values of an exact case: finite multiples of `unit` (default 4^-(N+1)), and below 2^24 in those units."""
+    unit = 4.0 ** -(N + 1) if unit is None else unit
+    x = t.detach().double() / unit
     assert torch.isfinite(x).all(), what
-    assert torch.equal(x, x.round()), f'{what}: not a multiple of 4^-{N + 1}'
-    assert float(x.abs().max()) < 2.0 ** 24, f'{what}: {float(x.abs().max())} units of 4^-{N + 1}'
+    assert torch.equal(x, x.round()), f'{what}: not a multiple of {unit:g}'
+    assert float(x.abs().max()) < 2.0 ** 24, f'{what}: {float(x.abs().max())} units of {unit:g}'
 
 
 def autograd(ref, guidance, x, grad_out, dtype):

@@ -1,7 +1,7 @@
-"""The forced-plan matrix of the 2D cluster kernel, shared by tests/test_forced_plans_gpu.py (which runs it) and
-tests/test_plan_cpu.py (which checks, without a GPU, that the planner honours every combination and that together they
-reach every configuration in every mode), plus what the 2D GPU tests share: the special-value goldens and the backward
-called through the C ABI.
+"""The forced-plan matrix of the 2D cluster kernel, shared by tests/test_forced_plans_gpu.py and
+tests/test_cluster_exact_gpu.py (which run it) and tests/test_plan_cpu.py (which checks, without a GPU, that the planner
+honours every combination and that together they reach every configuration in every mode), plus what the 2D GPU tests
+share: the special-value goldens and the forward and backward called through the C ABI under a forced plan.
 
 Which kernels a call runs normally depends on the card: the planner picks configuration, cluster size, row bands and
 passes from cudaOccupancyMaxActiveClusters and the SM count.  CSPN_B200_FORCE_CFG / _FORCE_CS / _FORCE_PASSES and
@@ -13,8 +13,10 @@ row that is not a multiple of PR.  So all plans of one problem whose band origin
 must give the same bits, whatever their cluster size, strips, pass split, chaining or GENERAL kernel: see `bit_group`.
 """
 import math
+import warnings
 from collections import namedtuple
 
+import pytest
 import torch
 
 from cspn_b200 import _lib
@@ -137,6 +139,67 @@ def bit_group(plan, info):
     band of every pass starts on a multiple of PR, else None (such a plan is only held against the oracle)."""
     PR = CONFIGS[plan.cfg][0]
     return PR if all(b[0] % PR == 0 for p in info['passes'] for b in p['bands']) else None
+
+
+def forward(g, d, s, n, norm):
+    """The C ABI on this thread (cspn_last_* are thread-local).  `out` and a workspace of exactly the queried size sit in
+    sentinel-filled guarded buffers (tests/memory_contract.py): every plan must store all of `out` and nothing outside it
+    or past the workspace.  Returns the workspace's interior."""
+    L = _lib.lib()
+    gc, dc = g.cuda().contiguous(), d.cuda().contiguous()
+    sc = None if s is None else s.cuda().contiguous()
+    B, C, H, W = dc.shape
+    ws_bytes = L.cspn2d_workspace_bytes(B, C, H, W, n, _lib.ALGO_CLUSTER)
+    ws = mc.workspace(ws_bytes)
+    out = mc.guarded(dc.shape)
+    rc = L.cspn2d_fwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), out.ptr(), B, C, H, W,
+                          gc.shape[1], n, _lib.NORM2D[norm], _lib.ALGO_CLUSTER, ws.ptr(), ws_bytes,
+                          torch.cuda.current_stream().cuda_stream)
+    _lib.check(rc, 'cspn2d_fwd_f32')
+    torch.cuda.synchronize()
+    mc.assert_written(out, 'out')
+    assert ws.guards_intact(), 'a store landed past the workspace'
+    return out.t.cpu(), L.cspn_last_algo(), L.cspn_last_launches(), ws.t
+
+
+def chain_flags(info, B, C, H, W, ws):
+    """The flag words of the last chained pass, one per (strip boundary, image-channel, CTA): the workspace layout of
+    cluster2d_forward / chain_ws in cspn2d_cluster.cu (a continuation buffer when there are several passes, then the
+    history blocks, then the flags).  Each is 1 once the chained kernel has finished that block."""
+    BC, passes = B * C, info['passes']
+    base = B * C * H * W * 4 if sum(p['count'] for p in passes) > 1 else 0
+    ceil256 = lambda x: (x + 255) // 256 * 256
+    hist = max(ceil256((len(p['strips']) - 1) * BC * p['cs'] * p['iters'] * p['NW'] * 8 * 4) for p in passes)
+    last = passes[-1]
+    blocks = (len(last['strips']) - 1) * BC * last['cs']
+    return ws[base + hist:base + hist + 4 * blocks].view(torch.int32).cpu()
+
+
+def refused(plan, shape):
+    """The device cannot host this forced combination (cudaOccupancyMaxActiveClusters gives 0).  tests/test_plan_cpu.py
+    shows the geometry of every combination is valid, so only the occupancy query can refuse it."""
+    assert plan.cs > 1, f'a one-CTA cluster of configuration {plan.cfg} cannot be refused: {plan}'
+    warnings.warn(f'the device refused forced plan {plan} for {shape}')
+
+
+def run_forced(plan, g, d, s, n, norm):
+    """Forward under `plan` (already forced): (None, None) when the device refuses it, else the output and plan_info,
+    checked to come from the forced plan: the cluster algorithm, one launch per pass, a chained plan's flags all set."""
+    B, C, H, W = d.shape
+    info = plan_info(plan, H, W, n)
+    if not info['supported']:
+        with pytest.raises(_lib.CspnError, match='unsupported'):
+            forward(g, d, s, n, norm)
+        refused(plan, (B, C, H, W, n))
+        return None, None
+    n_pass = check_honoured(plan, info)
+    if plan.chain and not chains(plan):       # no chained kernel in this configuration: the unchained plan runs
+        assert 'chained' not in _lib.describe_plan(B, C, H, W, n, _lib.ALGO_CLUSTER)
+    out, algo, launches, ws = forward(g, d, s, n, norm)
+    assert _lib.ALGO_NAMES[algo] == 'cluster' and launches == n_pass, (plan, algo, launches, n_pass)
+    if chains(plan):
+        assert (chain_flags(info, B, C, H, W, ws) == 1).all(), f'{plan}: the chained kernel did not run'
+    return out, info
 
 
 def backward(g, d, s, go, n, norm):

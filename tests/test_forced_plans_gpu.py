@@ -6,18 +6,14 @@ Each forced plan is checked to be the one that ran: plan_info shows the forced c
 count, the call reports the cluster algorithm and one launch per pass (2 per pass + 1 for the backward), and a chained
 call leaves its strips' "history complete" flags set in the workspace.  A combination the device cannot host must be
 refused as unsupported; those refusals are reported as warnings."""
-import warnings
-
 import numpy as np
 import pytest
 import torch
 
-from cspn_b200 import _lib
 from cspn_b200.synth import make_inputs
 from conftest import load_golden
-import memory_contract as mc
-from forced_plans import (NAN_PATCH_PLANS, NORMS, PROBLEMS, SPECIAL, backward, bit_group, chains, check_honoured, force,
-                          plan_info, special_plans)
+from forced_plans import (NAN_PATCH_PLANS, NORMS, PROBLEMS, SPECIAL, backward, bit_group, check_honoured, force, plan_info,
+                          refused, run_forced, special_plans)
 from oracle import c_oracle, cspn_numpy as onp, cspn_torch_port as tp
 
 pytestmark = pytest.mark.gpu
@@ -26,67 +22,6 @@ pytestmark = pytest.mark.gpu
 def inputs(pb, seed):
     """About one pixel in 20 sparse, so that masked pixels sit in every tile and halo."""
     return make_inputs(seed, pb.B, pb.C, pb.H, pb.W, pb.gch, pb.sparse, pb.H * pb.W // 20)
-
-
-def _forward(g, d, s, n, norm):
-    """The C ABI on this thread (cspn_last_* are thread-local).  `out` and a workspace of exactly the queried size sit in
-    sentinel-filled guarded buffers (tests/memory_contract.py): every plan must store all of `out` and nothing outside it
-    or past the workspace.  Returns the workspace's interior."""
-    L = _lib.lib()
-    gc, dc = g.cuda().contiguous(), d.cuda().contiguous()
-    sc = None if s is None else s.cuda().contiguous()
-    B, C, H, W = dc.shape
-    ws_bytes = L.cspn2d_workspace_bytes(B, C, H, W, n, _lib.ALGO_CLUSTER)
-    ws = mc.workspace(ws_bytes)
-    out = mc.guarded(dc.shape)
-    rc = L.cspn2d_fwd_f32(gc.data_ptr(), dc.data_ptr(), None if sc is None else sc.data_ptr(), out.ptr(), B, C, H, W,
-                          gc.shape[1], n, _lib.NORM2D[norm], _lib.ALGO_CLUSTER, ws.ptr(), ws_bytes,
-                          torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, 'cspn2d_fwd_f32')
-    torch.cuda.synchronize()
-    mc.assert_written(out, 'out')
-    assert ws.guards_intact(), 'a store landed past the workspace'
-    return out.t.cpu(), L.cspn_last_algo(), L.cspn_last_launches(), ws.t
-
-
-def chain_flags(info, B, C, H, W, ws):
-    """The flag words of the last chained pass, one per (strip boundary, image-channel, CTA): the workspace layout of
-    cluster2d_forward / chain_ws in cspn2d_cluster.cu (a continuation buffer when there are several passes, then the
-    history blocks, then the flags).  Each is 1 once the chained kernel has finished that block."""
-    BC, passes = B * C, info['passes']
-    base = B * C * H * W * 4 if sum(p['count'] for p in passes) > 1 else 0
-    ceil256 = lambda x: (x + 255) // 256 * 256
-    hist = max(ceil256((len(p['strips']) - 1) * BC * p['cs'] * p['iters'] * p['NW'] * 8 * 4) for p in passes)
-    last = passes[-1]
-    blocks = (len(last['strips']) - 1) * BC * last['cs']
-    return ws[base + hist:base + hist + 4 * blocks].view(torch.int32).cpu()
-
-
-def refused(plan, shape):
-    """The device cannot host this forced combination (cudaOccupancyMaxActiveClusters gives 0).  tests/test_plan_cpu.py
-    shows the geometry of every combination is valid, so only the occupancy query can refuse it."""
-    assert plan.cs > 1, f'a one-CTA cluster of configuration {plan.cfg} cannot be refused: {plan}'
-    warnings.warn(f'the device refused forced plan {plan} for {shape}')
-
-
-def run_forced(plan, g, d, s, n, norm):
-    """Forward under `plan` (already forced): None when the device refuses it, else the output, checked to come from
-    the forced plan."""
-    B, C, H, W = d.shape
-    info = plan_info(plan, H, W, n)
-    if not info['supported']:
-        with pytest.raises(_lib.CspnError, match='unsupported'):
-            _forward(g, d, s, n, norm)
-        refused(plan, (B, C, H, W, n))
-        return None, None
-    n_pass = check_honoured(plan, info)
-    if plan.chain and not chains(plan):       # no chained kernel in this configuration: the unchained plan runs
-        assert 'chained' not in _lib.describe_plan(B, C, H, W, n, _lib.ALGO_CLUSTER)
-    out, algo, launches, ws = _forward(g, d, s, n, norm)
-    assert _lib.ALGO_NAMES[algo] == 'cluster' and launches == n_pass, (plan, algo, launches, n_pass)
-    if chains(plan):
-        assert (chain_flags(info, B, C, H, W, ws) == 1).all(), f'{plan}: the chained kernel did not run'
-    return out, info
 
 
 def same_bits(a, b):

@@ -71,9 +71,10 @@ def test_headline_shape_is_a_single_pass_single_band_plan():
     assert p['count'] == 1 and len(p['bands']) == 1 and p['cs'] * p['RB'] >= 352 and len(p['strips']) == 15
 
 
-def replay_chained(info, guidance, blur, sparse, norm):
+def replay_chained(info, guidance, blur, sparse, norm, lag=0):
     """Chained plan on the numpy oracle: strips left to right; a strip's column -1 is, at every step, what the strip to its
-    left computed there (its history), so only the right edge goes stale."""
+    left computed there (its history), so only the right edge goes stale.  `lag` > 0 hands the history over that many
+    steps late (zeros before), a deliberately wrong plan for tests/test_cluster_exact_cpu.py."""
     f64 = np.float64
     gate_wb, gate_sum = onp.affinity_normalization_2d(guidance.astype(f64), norm)
     raw = blur.astype(f64)
@@ -94,7 +95,7 @@ def replay_chained(info, guidance, blur, sparse, norm):
                 with np.errstate(invalid='ignore'):
                     for t in range(p['iters']):
                         new_hist.append(d[..., rec:rec + 1].copy())
-                        left = hist[t] if hist is not None else np.zeros_like(d[..., :1])
+                        left = hist[t - lag] if hist is not None and t >= lag else np.zeros_like(d[..., :1])
                         ext = np.concatenate([left, d], axis=-1)             # column -1 in front: exact, not zero
                         acc = np.zeros_like(d)
                         for k, (dy, dx) in enumerate(onp.OFFSETS_2D):
