@@ -25,14 +25,17 @@ SIGNATURES = {
     'cspn2d_bwd_f32': (_i, [_vp] * 6 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn2d_k_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_k_fwd_f32': (_i, [_vp] * 4 + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn2d_k_fwd_gather_f32': (_i, [_vp] * 5 + [_i, _vp] + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn2d_k_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_k_bwd_f32': (_i, [_vp] * 6 + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn2d_paddle_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_paddle_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_paddle_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_paddle_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_paddle_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_gates_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_gates_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_gates_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_gates_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_gates_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn3d_gates_workspace_bytes': (_sz, [_i] * 7),

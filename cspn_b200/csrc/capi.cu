@@ -51,6 +51,24 @@ int check2d(const float* guidance, const float* blur, float* out, int B, int C, 
     return CSPN_OK;
 }
 
+// The destinations of a fused gather (cspn2d_*fwd_gather_f32) and its step count: the checks every gather entry shares
+int check_gather(float* const* peer_out, int n_peer, const float* multicast_out, int iters) {
+    if (n_peer < 0 || n_peer > 7 || (n_peer > 0 && !peer_out)) { set_error("n_peer must be 0..7 with a pointer array"); return CSPN_ERR_INVALID_ARGUMENT; }
+    for (int i = 0; i < n_peer; ++i)
+        if (!peer_out[i] || (reinterpret_cast<uintptr_t>(peer_out[i]) & 15)) { set_error("peer_out[%d] is null or not 16-byte aligned", i); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (reinterpret_cast<uintptr_t>(multicast_out) & 15) { set_error("multicast_out is not 16-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (iters == 0) { set_error("the fused gather needs prop_time >= 1"); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+Fan make_fan(float* const* peer_out, int n_peer, float* multicast_out) {
+    Fan f{};
+    for (int i = 0; i < n_peer; ++i) f.peer[i] = peer_out[i];
+    f.n_peer = n_peer;
+    f.mc = multicast_out;
+    return f;
+}
+
 // Picks the algorithm actually run for `algo` on this problem.  AUTO prefers the cluster kernel.
 int resolve_algo(const Problem2D& p, int algo, char* why, int why_len, const void* ws = nullptr) {
     if (algo == CSPN_ALGO_GENERIC) return CSPN_ALGO_GENERIC;
@@ -133,11 +151,8 @@ int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, const float*
     g_last_launches = 0;
     int rc = check2d(guidance, blur, out, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_CLUSTER);
     if (rc != CSPN_OK) return rc;
-    if (n_peer < 0 || n_peer > 7 || (n_peer > 0 && !peer_out)) { set_error("n_peer must be 0..7 with a pointer array"); return CSPN_ERR_INVALID_ARGUMENT; }
-    for (int i = 0; i < n_peer; ++i)
-        if (!peer_out[i] || (reinterpret_cast<uintptr_t>(peer_out[i]) & 15)) { set_error("peer_out[%d] is null or not 16-byte aligned", i); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (reinterpret_cast<uintptr_t>(multicast_out) & 15) { set_error("multicast_out is not 16-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters == 0) { set_error("the fused gather needs prop_time >= 1"); return CSPN_ERR_UNSUPPORTED; }
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
     DeviceGuard guard(device_of(blur));
     if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
     Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
@@ -215,6 +230,28 @@ int cspn2d_k_fwd_f32(const float* guidance, const float* blur, const float* spar
     return rc;
 }
 
+int cspn2d_k_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out, float* const* peer_out,
+                            int n_peer, float* multicast_out, int B, int C, int H, int W, int guidance_channels, int K,
+                            int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_k(guidance, blur, out, B, C, H, W, guidance_channels, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return cspn2d_fwd_gather_f32(guidance, blur, sparse, out, peer_out, n_peer, multicast_out, B, C, H, W,
+                                     guidance_channels, iters, norm_type, workspace, workspace_bytes, stream);
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(blur));
+    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = widek_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
+    g_last_launches = launches;
+    return rc;
+}
+
 size_t cspn2d_k_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
     if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters < 0 || !kernel_size_ok(K)) return 0;
     if (K == 3) return cspn2d_bwd_workspace_bytes(B, C, H, W, iters);
@@ -266,6 +303,25 @@ int cspn2d_paddle_fwd_f32(const float* guidance, const float* feat, float* out, 
     Problem2D p{guidance, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
     int launches = 0;
     rc = widek_paddle_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+int cspn2d_paddle_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
+                                 float* multicast_out, int B, int C, int H, int W, int K, int iters, void* workspace,
+                                 size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check2d_paddle(guidance, feat, out, B, C, H, W, K, iters);
+    if (rc != CSPN_OK) return rc;
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{guidance, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = widek_paddle_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
     g_last_launches = launches;
     return rc;
 }
@@ -420,6 +476,25 @@ int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out, int 
     Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
     int launches = 0;
     rc = widek_gates_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+int cspn2d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out, float* const* peer_out, int n_peer,
+                                float* multicast_out, int B, int C, int H, int W, int K, int iters, void* workspace,
+                                size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, out, B, C, 1, H, W, K, iters, false);
+    if (rc != CSPN_OK) return rc;
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = widek_gates_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
     g_last_launches = launches;
     return rc;
 }

@@ -80,20 +80,32 @@ size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters);
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
           size_t ws_bytes, cudaStream_t stream, int* launches);
 
-// K x K kernels, K in {5, 7} (cspn2d_wide.cu)
+// Fused gather of the K x K, 'paddle' and gates forwards (cspn2d_{k,paddle,gates}_fwd_gather_f32): the last step also
+// stores its result to these destinations, each addressed like p.out -- up to 7 peer-mapped bases (NVLink stores) and one
+// NVLS multicast base or null; all 16-byte aligned.  Passed by value to the step kernel (the Scatter of cspn2d_cluster.cu).
+struct Fan {
+    float* peer[7];
+    int n_peer;
+    float* mc;
+};
+
+// K x K kernels, K in {5, 7} (cspn2d_wide.cu); fan non-null: the fused gather
 size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters);
-int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                  const Fan* fan = nullptr);
 size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                    size_t ws_bytes, cudaStream_t stream, int* launches);
 // 'paddle' own-location norm, K in {3, 5, 7}, on the same kernels and workspaces (p.sparse null, p.gch == K*K-1)
-int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                         const Fan* fan = nullptr);
 int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
                           size_t ws_bytes, cudaStream_t stream, int* launches);
 // caller-supplied gates, K in {3, 5, 7}: p.guidance [B][K*K-1][H][W] used as given (p.sparse null, p.gch == K*K-1)
 size_t widek_gates_workspace_bytes(int B, int C, int H, int W, int iters);
 size_t widek_gates_bwd_workspace_bytes(int B, int C, int H, int W, int iters);
-int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                        const Fan* fan = nullptr);
 int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,
                          size_t ws_bytes, cudaStream_t stream, int* launches);
 

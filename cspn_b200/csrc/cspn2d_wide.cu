@@ -32,6 +32,11 @@
 // The RAW flag of the step and adjoint kernels reads the caller's gates [image][NT][H][W] (NT planes per image instead of
 // the workspace's NP); there is no prep launch.  The gather's RAW mode writes Gw_k to the gate gradient at p and does
 // not read the gates; the last adjoint step writes lambda_0 straight into the input gradient.
+//
+// Fused gather (cspn2d_{k,paddle,gates}_fwd_gather_f32, DESIGN.md section 4.6): the FAN flag of the two step kernels
+// stores each result also to the same element of every peer GPU's gather buffer (NVLink stores) and / or to one NVLS
+// multicast address (multimem.st).  Only the last step of a launch group, the one that writes `out`, runs it; the
+// intermediate iterates never leave the GPU.
 #include <cstdlib>
 #include <cstring>
 
@@ -118,12 +123,13 @@ prepk_paddle_kernel(const float* __restrict__ guidance, float* __restrict__ wk, 
 // Tile 64 x 16 pixels per CTA of 16 x 16 threads.  The shared tile holds rows y0-R .. y0+15+R and columns x0-4 ..
 // x0+67 as float4 (the halo is rounded up to 4 columns so every row of a thread's window is three aligned LDS.128).
 // PADDLE: no kappa d0 term (d0 is not read).  RAW (with PADDLE): wk is the caller's gates, NT planes per image.
+// FAN: the result also goes to fan's destinations (the last step of a fused gather); fan is not read otherwise.
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R, bool PADDLE = false, bool RAW = false>
+template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
 __global__ void __launch_bounds__(256)
 stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-                 float* __restrict__ dst, int C, int H, int W) {
+                 float* __restrict__ dst, int C, int H, int W, const Fan fan) {
     using T = Taps<R>;
     constexpr int SH = kVecTH + 2 * R, SQ = kVecTW / 4 + 2;
     __shared__ float4 tile[SH][SQ];
@@ -166,7 +172,17 @@ stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, con
             acc3 = fmaf(wv.w, row[7 + dx], acc3);
         }
     }
-    *reinterpret_cast<float4*>(dst + (size_t)bc * HW + p) = make_float4(acc0, acc1, acc2, acc3);
+    const size_t o = (size_t)bc * HW + p;
+    const float4 v = make_float4(acc0, acc1, acc2, acc3);
+    *reinterpret_cast<float4*>(dst + o) = v;
+    if constexpr (FAN) {
+#pragma unroll
+        for (int e = 0; e < 7; ++e)          // peer GPUs' gather buffers (NVLink stores); n_peer is uniform
+            if (e < fan.n_peer) __stcs(reinterpret_cast<float4*>(fan.peer[e] + o), v);
+        if (fan.mc)                          // NVLS: one store, replicated by the switch
+            asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(fan.mc + o), "f"(v.x), "f"(v.y),
+                         "f"(v.z), "f"(v.w) : "memory");
+    }
 }
 
 // ---- step / adjoint, one pixel per thread (any W, any alignment).  Tile 32 x 8 pixels + R halo --------------------
@@ -183,10 +199,10 @@ __device__ __forceinline__ void load_tile_scalar(float (*tile)[kSclTW + 2 * R], 
     }
 }
 
-template <int R, bool PADDLE = false, bool RAW = false>
+template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
 __global__ void __launch_bounds__(256)
 stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-                    float* __restrict__ dst, int C, int H, int W) {
+                    float* __restrict__ dst, int C, int H, int W, const Fan fan) {
     using T = Taps<R>;
     __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
     const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, bc = blockIdx.z;
@@ -200,7 +216,14 @@ stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, 
     float acc = PADDLE ? 0.f : __ldg(w + T::NT * HW) * __ldg(d0 + (size_t)bc * HW + p);
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
-    dst[(size_t)bc * HW + p] = acc;
+    const size_t o = (size_t)bc * HW + p;
+    dst[o] = acc;
+    if constexpr (FAN) {
+#pragma unroll
+        for (int e = 0; e < 7; ++e)
+            if (e < fan.n_peer) __stcs(fan.peer[e] + o, acc);
+        if (fan.mc) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(fan.mc + o), "f"(acc) : "memory");
+    }
 }
 
 // lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only.
@@ -350,21 +373,26 @@ void launch_prep(const float* guidance, const float* sparse, float* wk, int nimg
     else prepk_kernel<R><<<grid, block, 0, s>>>(guidance, sparse, wk, H, W, gch, norm_abs);
 }
 
+// fan non-null: the FAN instantiation, which also stores the result to fan's destinations
 template <int R, bool PADDLE, bool RAW = false>
 void launch_step(bool vec, const float* wk, const float* d0, const float* cur, float* dst, int nbc, int C, int H, int W,
-                 cudaStream_t s) {
-    if (vec)
-        stepk_vec_kernel<R, PADDLE, RAW><<<dim3((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), dim3(16, 16), 0, s>>>(
-            wk, d0, cur, dst, C, H, W);
-    else
-        stepk_scalar_kernel<R, PADDLE, RAW><<<dim3((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), dim3(kSclTW, kSclTH), 0, s>>>(
-            wk, d0, cur, dst, C, H, W);
+                 cudaStream_t s, const Fan* fan = nullptr) {
+    const dim3 vgrid((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, nbc), vblock(16, 16);
+    const dim3 sgrid((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, nbc), sblock(kSclTW, kSclTH);
+    if (fan) {
+        if (vec) stepk_vec_kernel<R, PADDLE, RAW, true><<<vgrid, vblock, 0, s>>>(wk, d0, cur, dst, C, H, W, *fan);
+        else stepk_scalar_kernel<R, PADDLE, RAW, true><<<sgrid, sblock, 0, s>>>(wk, d0, cur, dst, C, H, W, *fan);
+        return;
+    }
+    if (vec) stepk_vec_kernel<R, PADDLE, RAW><<<vgrid, vblock, 0, s>>>(wk, d0, cur, dst, C, H, W, Fan{});
+    else stepk_scalar_kernel<R, PADDLE, RAW><<<sgrid, sblock, 0, s>>>(wk, d0, cur, dst, C, H, W, Fan{});
 }
 
 // RAW: the caller's gates (p.guidance, NT planes per image) are the weight planes; the workspace holds only the
-// ping-pong buffer
+// ping-pong buffer.  fan (fused gather): destinations addressed like p.out, which the last step of every launch group
+// also writes, each offset to the group as `out` is.
 template <int R, bool PADDLE, bool RAW = false>
-int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) {
+int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches, const Fan* fan = nullptr) {
     constexpr int NPL = RAW ? Taps<R>::NT : Taps<R>::NP;   // weight planes per image
     const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
     float* wk_ws = static_cast<float*>(ws);
@@ -383,10 +411,17 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches) 
                                    wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
             ++*launches;
         }
+        Fan gfan{};
+        if (fan) {
+            gfan.n_peer = fan->n_peer;
+            for (int e = 0; e < fan->n_peer; ++e) gfan.peer[e] = fan->peer[e] + (size_t)b0 * plane;
+            gfan.mc = fan->mc ? fan->mc + (size_t)b0 * plane : nullptr;
+        }
         const float* cur = blur;
         float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < p.iters; ++it) {
-            launch_step<R, PADDLE, RAW>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
+            launch_step<R, PADDLE, RAW>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream,
+                                        fan && it == p.iters - 1 ? &gfan : nullptr);
             ++*launches;
             cur = dst;
             dst = (dst == out) ? tmp : out;
@@ -465,7 +500,7 @@ size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
     return sizeof(float) * ((size_t)B * K * K * HW + 2 * (size_t)iters * B * C * HW);
 }
 
-int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
     const size_t n = (size_t)p.B * p.C * p.H * p.W;
     if (p.iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -477,7 +512,7 @@ int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStre
         return CSPN_ERR_WORKSPACE;
     }
     if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
-    return K == 5 ? forward_k<2, false>(p, ws, stream, launches) : forward_k<3, false>(p, ws, stream, launches);
+    return K == 5 ? forward_k<2, false>(p, ws, stream, launches, fan) : forward_k<3, false>(p, ws, stream, launches, fan);
 }
 
 int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
@@ -500,7 +535,8 @@ int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad
 }
 
 // 'paddle': p.sparse is null and p.gch == K*K-1 (the C ABI sets both); same workspaces as the K x K path
-int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                         const Fan* fan) {
     if (p.iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
@@ -511,8 +547,8 @@ int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, c
         return CSPN_ERR_WORKSPACE;
     }
     if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D 'paddle' path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
-    if (K == 3) return forward_k<1, true>(p, ws, stream, launches);
-    return K == 5 ? forward_k<2, true>(p, ws, stream, launches) : forward_k<3, true>(p, ws, stream, launches);
+    if (K == 3) return forward_k<1, true>(p, ws, stream, launches, fan);
+    return K == 5 ? forward_k<2, true>(p, ws, stream, launches, fan) : forward_k<3, true>(p, ws, stream, launches, fan);
 }
 
 int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
@@ -550,7 +586,8 @@ static bool gates_grid_ok(const Problem2D& p, int K, const char* what) {
     return true;
 }
 
-int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                        const Fan* fan) {
     if (p.iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
@@ -561,8 +598,9 @@ int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cu
         return CSPN_ERR_WORKSPACE;
     }
     if (!gates_grid_ok(p, K, "path")) return CSPN_ERR_UNSUPPORTED;
-    if (K == 3) return forward_k<1, true, true>(p, ws, stream, launches);
-    return K == 5 ? forward_k<2, true, true>(p, ws, stream, launches) : forward_k<3, true, true>(p, ws, stream, launches);
+    if (K == 3) return forward_k<1, true, true>(p, ws, stream, launches, fan);
+    return K == 5 ? forward_k<2, true, true>(p, ws, stream, launches, fan)
+                  : forward_k<3, true, true>(p, ws, stream, launches, fan);
 }
 
 int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,

@@ -140,6 +140,25 @@ CSPN_API int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const fl
                      int guidance_channels, int K, int iters, int norm_type,
                      void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- fused gather of the K x K, 'paddle' and gates forwards (2D) ----------------------------------------------------
+ * cspn2d_k_fwd_gather_f32, cspn2d_paddle_fwd_gather_f32 and cspn2d_gates_fwd_gather_f32 take the arguments of their plain
+ * forward plus peer_out / n_peer / multicast_out after `out`, as cspn2d_fwd_gather_f32 does, and give `out` its bits.  The
+ * last step of the forward also stores its result to each peer_out[i] (the same [B][C][H][W] block inside another GPU's
+ * gather buffer, a peer pointer mapped over NVLink) and / or to multicast_out (an NVLS multicast address, one
+ * multimem.st); intermediate steps stay local.  n_peer 0..7 with a non-null array when non-zero, every peer_out[i]
+ * non-null, every peer_out[i] and multicast_out (may be NULL) 16-byte aligned, else CSPN_ERR_INVALID_ARGUMENT;
+ * iters == 0 is CSPN_ERR_UNSUPPORTED.
+ * Workspace as for the plain forward (its *_workspace_bytes), and cspn_last_launches() counts the same launches.
+ * K = 3 in cspn2d_k_fwd_gather_f32 delegates to cspn2d_fwd_gather_f32 and so needs the cluster kernel
+ * (CSPN_ERR_UNSUPPORTED for a shape it cannot take, e.g. W % 4 != 0); the 'paddle' and gates entries take any W for
+ * K in {3, 5, 7}.  Per-channel gates are B*C images with C = 1, as in the plain calls: the output memory, and with it the
+ * peer offsets, is the same.  The caller orders the remote stores before their consumers (a barrier across ranks after
+ * the call). */
+CSPN_API int cspn2d_k_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out,
+                            float* const* peer_out, int n_peer, float* multicast_out,
+                            int B, int C, int H, int W, int guidance_channels, int K, int iters, int norm_type,
+                            void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
@@ -154,6 +173,12 @@ CSPN_API size_t cspn2d_paddle_workspace_bytes(int B, int C, int H, int W, int K,
 CSPN_API int cspn2d_paddle_fwd_f32(const float* guidance, const float* feat, float* out,
                           int B, int C, int H, int W, int K, int iters,
                           void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+/* cspn2d_paddle_fwd_f32 fused with the final gather of a data-parallel run: see cspn2d_k_fwd_gather_f32 */
+CSPN_API int cspn2d_paddle_fwd_gather_f32(const float* guidance, const float* feat, float* out,
+                                 float* const* peer_out, int n_peer, float* multicast_out,
+                                 int B, int C, int H, int W, int K, int iters,
+                                 void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
 CSPN_API size_t cspn2d_paddle_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 
@@ -230,6 +255,12 @@ CSPN_API size_t cspn2d_gates_workspace_bytes(int B, int C, int H, int W, int K, 
 CSPN_API int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out,
                          int B, int C, int H, int W, int K, int iters,
                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+/* cspn2d_gates_fwd_f32 fused with the final gather of a data-parallel run: see cspn2d_k_fwd_gather_f32 (2D only) */
+CSPN_API int cspn2d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out,
+                                float* const* peer_out, int n_peer, float* multicast_out,
+                                int B, int C, int H, int W, int K, int iters,
+                                void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
 CSPN_API size_t cspn2d_gates_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 

@@ -1,9 +1,13 @@
 """Multi-GPU check of the fused / chunked final gather (run under torchrun on 2..8 GPUs of one box):
 
-    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/gather_check.py
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 \
+        tools/gather_check.py [B H W N] [--families]
 
-Every rank propagates its own images; all three gather routes must leave the same full batch on every rank, equal to what
-each rank computes alone.  Prints one line per route with its time per step (CUDA events, max over ranks)."""
+Every rank propagates its own images; every gather route must leave the same full batch on every rank, bit for bit equal
+to each rank's own plain forward after a serial NCCL all-gather.  Prints one line per route with its time per call (CUDA
+events, max over ranks).  The 3x3 operator (propagate2d) always runs; --families adds the K x K operator with K = 5 and
+7 (propagate_k), the Paddle module's own-location gates (propagate_paddle, K = 5) and caller-supplied gates
+(affinity_propagate, K = 5)."""
 import os
 import sys
 
@@ -16,17 +20,20 @@ from cspn_b200.gather import ChunkedGather, FusedGather
 from cspn_b200.sharding import gather_outputs
 from cspn_b200.synth import make_inputs
 
-B, H, W, N = [int(a) for a in sys.argv[1:5]] if len(sys.argv) > 4 else (32, 352, 1216, 24)
+FAMILIES = '--families' in sys.argv
+ARGS = [a for a in sys.argv[1:] if a != '--families']
+B, H, W, N = [int(a) for a in ARGS[:4]] if len(ARGS) > 3 else (32, 352, 1216, 24)
 rank, world, local = int(os.environ['RANK']), int(os.environ['WORLD_SIZE']), int(os.environ['LOCAL_RANK'])
 torch.cuda.set_device(local)
 dev = torch.device('cuda', local)
 dist.init_process_group('nccl', device_id=dev)
-g, d, s = [t.to(dev) for t in make_inputs(rank, min(B, 8), 1, H, W)]
-if B > 8:
-    g, d, s = [t.repeat((B + 7) // 8, 1, 1, 1)[:B].contiguous() for t in (g, d, s)]
-mine = cspn_b200.propagate2d(g, d, s, N, '8sum')
-ref = gather_outputs(mine, world * B)                       # kernel, then NCCL all_gather_into_tensor
-assert torch.equal(ref[rank * B:(rank + 1) * B], mine)
+
+
+def inputs(seed, gch):
+    g, d, s = [t.to(dev) for t in make_inputs(seed, min(B, 8), 1, H, W, gch)]
+    if B > 8:
+        g, d, s = [t.repeat((B + 7) // 8, 1, 1, 1)[:B].contiguous() for t in (g, d, s)]
+    return g, d, s
 
 
 def timed(fn, reps=10, warm=3):
@@ -49,30 +56,53 @@ def report(name, ms, ok, extra=''):
     oks = torch.tensor([1 if ok else 0], device=dev)
     dist.all_reduce(oks, op=dist.ReduceOp.MIN)
     if rank == 0:
-        print(f'{name}: {ms:.4f} ms/step on {world} GPUs, identical on every rank: {bool(oks.item())} {extra}', flush=True)
+        print(f'{name}: {ms:.4f} ms/call on {world} GPUs, identical on every rank: {bool(oks.item())} {extra}', flush=True)
     return bool(oks.item())
 
 
-full = torch.empty(world * B, 1, H, W, device=dev)
-all_ok = report('kernel only', timed(lambda: cspn_b200.propagate2d(g, d, s, N, '8sum')), True)
-all_ok &= report('serial NCCL (kernel, then all_gather_into_tensor)',
-                 timed(lambda: dist.all_gather_into_tensor(full, cspn_b200.propagate2d(g, d, s, N, '8sum'))), torch.equal(full, ref))
-if B % 4 == 0:
-    cg = ChunkedGather(B, 1, H, W, dev, n_chunks=4)
-    ms = timed(lambda: cg.propagate(g, d, s, N, '8sum'))
-    all_ok &= report('chunked NCCL (4 chunks, kernel i+1 overlaps gather i)', ms, torch.equal(cg.as_rank_major(), ref))
-for mc in (True, False):
-    try:
-        fg = FusedGather(B, 1, H, W, dev, multicast=mc)
-        ms = timed(lambda: fg.propagate(g, d, s, N, '8sum'))
-        res = fg.propagate(g, d, s, N, '8sum')
-        torch.cuda.synchronize()
-        all_ok &= report(f'fused epilogue ({fg.mode})', ms, torch.equal(res, ref))
-        if fg.mode == 'peer_stores':
-            break
-    except Exception as e:                                     # noqa: BLE001 -- report and go on with the other routes
-        if rank == 0:
-            print(f'fused epilogue (multicast={mc}) unavailable: {type(e).__name__}: {str(e)[:300]}', flush=True)
+def check_routes(op, plain, fused, chunked=None):
+    """plain() -> this rank's (B, 1, H, W) result; fused(FusedGather) and chunked(ChunkedGather) -> the gathered batch."""
+    mine = plain()
+    ref = gather_outputs(mine, world * B)                   # kernel, then NCCL all_gather_into_tensor
+    ok = torch.equal(ref[rank * B:(rank + 1) * B], mine)
+    full = torch.empty(world * B, 1, H, W, device=dev)
+    ok &= report(f'{op}: kernel only', timed(plain), True)
+    ok &= report(f'{op}: serial NCCL (kernel, then all_gather_into_tensor)',
+                 timed(lambda: dist.all_gather_into_tensor(full, plain())), torch.equal(full, ref))
+    if chunked is not None and B % 4 == 0:
+        cg = ChunkedGather(B, 1, H, W, dev, n_chunks=4)
+        ms = timed(lambda: chunked(cg))
+        ok &= report(f'{op}: chunked NCCL (4 chunks, kernel i+1 overlaps gather i)', ms, torch.equal(cg.as_rank_major(), ref))
+    for mc in (True, False):
+        try:
+            fg = FusedGather(B, 1, H, W, dev, multicast=mc)
+            ms = timed(lambda: fused(fg))
+            res = fused(fg)
+            torch.cuda.synchronize()
+            ok &= report(f'{op}: fused ({fg.mode})', ms, torch.equal(res, ref))
+            if fg.mode == 'peer_stores':
+                break
+        except Exception as e:                                 # noqa: BLE001 -- report and go on with the other routes
+            if rank == 0:
+                print(f'{op}: fused (multicast={mc}) unavailable: {type(e).__name__}: {str(e)[:300]}', flush=True)
+    return ok
+
+
+g, d, s = inputs(rank, 8)
+all_ok = check_routes('propagate2d 3x3', lambda: cspn_b200.propagate2d(g, d, s, N, '8sum'),
+                      lambda fg: fg.propagate(g, d, s, N, '8sum'), lambda cg: cg.propagate(g, d, s, N, '8sum'))
+if FAMILIES:
+    for K in (5, 7):
+        gk, dk, sk = inputs(rank + 100 * K, K * K - 1)
+        all_ok &= check_routes(f'propagate2d_k {K}x{K}', lambda gk=gk, dk=dk, sk=sk, K=K: cspn_b200.propagate2d_k(gk, dk, sk, K, N),
+                               lambda fg, gk=gk, dk=dk, sk=sk, K=K: fg.propagate_k(gk, dk, sk, K, N),
+                               lambda cg, gk=gk, dk=dk, sk=sk, K=K: cg.propagate_k(gk, dk, sk, K, N))
+    gp, fp, _ = inputs(rank + 1000, 24)
+    all_ok &= check_routes('propagate2d_paddle 5x5', lambda: cspn_b200.propagate2d_paddle(gp, fp, 5, N),
+                           lambda fg: fg.propagate_paddle(gp, fp, 5, N))
+    gates = gp.abs() / gp.abs().sum(1, keepdim=True)            # demo.py's normalisation, done by the caller
+    all_ok &= check_routes('affinity_propagate 5x5', lambda: cspn_b200.affinity_propagate(fp, gates, 5, N),
+                           lambda fg: fg.affinity_propagate(fp, gates, 5, N))
 dist.barrier()
 dist.destroy_process_group()
 sys.exit(0 if all_ok else 1)
