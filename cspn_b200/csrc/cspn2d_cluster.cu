@@ -26,7 +26,8 @@
 //   * per iteration, x-neighbours come from warp shuffles, y-neighbours inside a thread from its own registers,
 //     across warps from a double-buffered shared-memory row exchange, and across CTAs of the cluster from the same
 //     exchange buffers written remotely through DSMEM with st.async, whose complete_tx lands on the consumer's
-//     mbarrier: pure dataflow, one mbarrier wait per iteration and no cluster-wide barrier inside the loop.
+//     mbarrier: pure dataflow, one mbarrier wait per iteration and no cluster-wide barrier inside the loop.  Each warp
+//     has its own exchange mbarrier, armed only by the producers of the two rows it reads (see publish).
 // No tensor cores: a 9-point stencil with per-pixel weights is FMA-issue + HBM bound, not a contraction.
 #include <cstdlib>
 #include <mutex>
@@ -84,13 +85,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// lane-predicated forms: no divergent branch (BSSY/BSYNC) around the single arriving lane
-__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %1, 0;\n@p mbarrier.arrive.shared::cta.b64 _, [%0];\n}\n" ::"r"(bar), "r"((int)pred) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx_if(uint32_t bar, uint32_t bytes, bool pred) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %2, 0;\n@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n}\n" ::"r"(bar), "r"(bytes), "r"((int)pred) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t done;
     do {
@@ -104,6 +98,39 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
             : "r"(bar), "r"(parity)
             : "memory");
     } while (!done);
+}
+// The exchange barriers: forms that address `bar` + OFF bytes (OFF = the parity's offset, an immediate in the address
+// rather than one more register per parity)
+template <uint32_t OFF>
+__device__ __forceinline__ void mbar_wait_at(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    do {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1+%3], %2;\n"
+            "selp.u32 %0, 1, 0, p;\n"
+            "}\n"
+            : "=r"(done)
+            : "r"(bar), "r"(parity), "n"(OFF)
+            : "memory");
+    } while (!done);
+}
+// Arrival of a publishing lane (see Xch::arr_bar): none if `bar` is 0; on `own` (the lane's own warp's barrier) it also
+// arms the TX bytes the neighbour CTA delivers there; elsewhere a plain arrival (expect_tx of 0 bytes).  Predicated, so
+// no divergent branch (BSSY/BSYNC) around the arriving lanes, and both roles come from the one address register.
+template <uint32_t OFF, uint32_t TX>
+__device__ __forceinline__ void mbar_arrive_xch(uint32_t bar, uint32_t own) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p, q;\n"
+        ".reg .b32 tx;\n"
+        "setp.ne.b32 p, %0, 0;\n"
+        "setp.eq.b32 q, %0, %1;\n"
+        "selp.b32 tx, %3, 0, q;\n"
+        "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0+%2], tx;\n"
+        "}\n" ::"r"(bar), "r"(own), "n"(OFF), "n"(TX)
+        : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -182,7 +209,7 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 //                             shift of cspn.py:105-129 cannot ride on the box origin; the row shift dy_k does)
 //   then xch[2][2*NW+2][TW]   row-exchange buffers (parity, slot, column)
 //   then cbuf[RB][TW]         folded constant term c' of the current task
-//   then 3 mbarriers          tma, full[0], full[1]
+//   then 1 + 2*NW mbarriers   tma, then the row-exchange barriers xbar[parity][warp]
 //
 // Arithmetic is scalar FFMA: sm_90 has no packed FP32 FMA, and the stencil has no contraction for the tensor cores.
 template <int PR, int PC, int NW>
@@ -202,7 +229,11 @@ struct Cfg {
     // the folded constant term c' (one float per pixel) lives in shared memory: it is read once per pixel and
     // iteration (one LDS.128 per patch row), which frees PR*PC registers per thread
     static constexpr size_t kCBytes = (size_t)RB * TW * sizeof(float);
-    static constexpr size_t kSmemBytes = kStageBytes + kXchBytes + kCBytes + 64;
+    // one exchange mbarrier per warp and parity (the parity-1 set follows the parity-0 set), after the TMA barrier;
+    // rounded up to 16 bytes: the chained-strip history behind it is read as float4
+    static constexpr uint32_t kXBarParity = 8 * NW;
+    static constexpr size_t kBarBytes = (8 + 2 * kXBarParity + 15) / 16 * 16;
+    static constexpr size_t kSmemBytes = kStageBytes + kXchBytes + kCBytes + kBarBytes;
     // chained strips: the recorded column of the left neighbour strip (in) and of this strip (out), [step][warp][8 rows]
     static constexpr int kChainMaxIters = cspn::kChainMaxIters;
     static constexpr int kHistRow = NW * 8;
@@ -213,6 +244,7 @@ struct Cfg {
     static_assert(TWP <= 256, "TMA box <= 256 columns");
     static_assert(RB <= 256 && RB % 4 == 0, "TMA box rows; plane size must stay a multiple of 128 B");
     static_assert(PR >= 2, "a patch needs distinct top and bottom rows");
+    static_assert(NW >= 2, "the CTA's top and bottom rows belong to different warps (one remote neighbour per warp)");
     static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared memory of an sm_90 CTA");
 };
 
@@ -263,16 +295,20 @@ struct Xch {
     int step;                 // running step index of the traced task
 #endif
     float* base;          // xch + lane*PC (parity 0, slot 0)
-    uint32_t bar_full0;   // local mbarriers: full[0], full[1] = full[0] + 8
-    uint32_t rx_bytes;    // halo bytes this CTA receives per exchange
-    // shared::cluster addresses in the neighbour CTAs (parity 0; parity 1 is a constant offset away)
-    uint32_t up_data, up_bar;   // CTA above: its last slot ("halo from below") at my lane's columns, its full[0]
-    uint32_t dn_data, dn_bar;   // CTA below: its slot 0 ("halo from above"), its full[0]
+    uint32_t bar_own;     // this warp's exchange mbarrier xbar[0][wy] (xbar[1][wy] is Cfg::kXBarParity bytes further)
+    // a publish ends with one arrival by lane 0 and one by lane 1, each on the barrier of a warp that reads what was just
+    // published: lane 0 on xbar[.][wy-1] (reads my top row), lane 1 on xbar[.][wy+1] (my bottom row).  At the CTA's top
+    // (bottom) edge the reader is a warp of the CTA above (below), whose barrier the remote bytes complete instead: there
+    // lane 0 (1) arms the bytes this warp will receive from that CTA on its own barrier, or stays idle at the image border.
+    uint32_t arr_bar;     // parity-0 barrier this lane arrives on (bar_own: with the remote bytes), 0: none (lanes 2..31)
     bool has_up, has_dn;
     // warp roles as predicates for the branch-free publish: remote_up = this warp owns the CTA's top row and a CTA
-    // above exists; remote_dn likewise
+    // above exists; remote_dn likewise (never both: NW >= 2)
     bool remote_up, remote_dn;
-    uint32_t my_tx;       // tx bytes this warp's lane-0 arrival arms: rx_bytes in the CTA's first warp, 0 elsewhere
+    // shared::cluster addresses in the neighbour CTA this warp sends to (parity 0; parity 1 is a constant offset away):
+    // remote_up: the CTA above's last slot ("halo from below") at my lane's columns and its last warp's barrier;
+    // remote_dn: the CTA below's slot 0 ("halo from above") and its first warp's barrier
+    uint32_t rm_data, rm_bar;
     bool first_lane, last_lane;
     const float* cbuf;    // this thread's first pixel of c' (row r is r*TW floats further)
     // chained strips (CHAIN kernels; set per task)
@@ -281,23 +317,32 @@ struct Xch {
 };
 
 // Publish the boundary rows of the new d into exchange buffer PAR (local shared memory, and the neighbour CTAs'
-// halo slots through DSMEM), then signal full[PAR].  Branch-free: roles are predicates.
+// halo slots through DSMEM), then signal the barriers of the warps that read them.  Branch-free: roles are predicates.
+//
+// The barriers follow the data, not the CTA: warp wy reads two rows per step (the bottom row of warp wy-1 and the top
+// row of warp wy+1, or a halo row from the neighbour CTA at the CTA's edges), so its barrier xbar[PAR][wy] completes
+// when exactly those two rows are there: one arrival per local neighbour warp; at a CTA edge with a neighbour CTA, the
+// st.async bytes from that CTA plus this warp's own arrival that arms them; at the image border nothing (the slot stays
+// zero).  A warp therefore waits for its two neighbours only, not for the slowest of the cluster's CTAs.
+// Double buffering stays safe: a producer overwrites parity P (at step s+2) only after its own wait at step s+1, which
+// needs the publish of step s+1 of every consumer of its rows (the dependency is symmetric: whom I read, reads me), and
+// each consumer publishes step s+1 only after it has read parity P at step s.  The same chain keeps every barrier at
+// one phase per step: no arrival for step s+2 can reach xbar[P][wy] before warp wy has waited there for step s.
 template <int PR, int PC, int NW, int PAR>
 __device__ __forceinline__ void publish(const Xch& x, int wy, const float (&top)[PC], const float (&bot)[PC]) {
     using K = Cfg<PR, PC, NW>;
     float* p = x.base + (size_t)PAR * K::kSlots * K::TWX;
     store_row_smem(p + (1 + 2 * wy) * K::TWX, top);
     store_row_smem(p + (2 + 2 * wy) * K::TWX, bot);
-    const uint32_t bar = x.bar_full0 + 8 * PAR;
     // my top row is the "halo from below" (last slot) of the CTA above; my bottom row the "halo from above" below
     // (remote_up / remote_dn are warp-uniform by construction -- wy comes from a shuffle -- so these are uniform
     // branches, not divergence regions)
-    if (x.remote_up) store_row_remote(x.up_data + PAR * (uint32_t)K::kXchParityBytes, top, x.up_bar + 8 * PAR);
-    if (x.remote_dn) store_row_remote(x.dn_data + PAR * (uint32_t)K::kXchParityBytes, bot, x.dn_bar + 8 * PAR);
+    const uint32_t rm_data = x.rm_data + PAR * (uint32_t)K::kXchParityBytes, rm_bar = x.rm_bar + PAR * K::kXBarParity;
+    if (x.remote_up) store_row_remote(rm_data, top, rm_bar);
+    if (x.remote_dn) store_row_remote(rm_data, bot, rm_bar);
     __syncwarp();
-    // one arrival per warp (lane 0); the first warp's also arms the bytes the neighbour CTAs will deliver (expect_tx of 0
-    // bytes is a plain arrival): one predicated instruction and one predicate instead of two of each
-    mbar_arrive_expect_tx_if(bar, x.my_tx, x.first_lane);
+    // lanes 0 and 1: one predicated instruction, each lane with its own barrier address
+    mbar_arrive_xch<PAR * K::kXBarParity, K::TW * sizeof(float)>(x.arr_bar, x.bar_own);
 }
 
 // ---- one propagation step ---------------------------------------------------------------------------------------
@@ -364,7 +409,7 @@ __device__ __forceinline__ void iterate3(const Xch& x, int wy, uint32_t phase, c
     // ---- B: the neighbours' rows, then publish at once ---------------------------------------------------------------
 #ifndef CSPN_ABLATE_NO_SYNC
     CSPN_STAMP(x, 5 + 3 * x.step);
-    mbar_wait(x.bar_full0 + 8 * PAR, phase);
+    mbar_wait_at<PAR * K::kXBarParity>(x.bar_own, phase);
     CSPN_STAMP(x, 6 + 3 * x.step);
 #endif
     {
@@ -536,7 +581,7 @@ __device__ __forceinline__ void iterate_adj(const Xch& x, int wy, uint32_t phase
     }
 #pragma unroll
     for (int r = 0; r < PR; ++r) fold_edges<PC>(lout[r], xl[r], xr[r], x.first_lane, x.last_lane);
-    mbar_wait(x.bar_full0 + 8 * PAR, phase);
+    mbar_wait_at<PAR * K::kXBarParity>(x.bar_own, phase);
     {
         const float* p = x.base + (size_t)PAR * K::kSlots * K::TWX;
         float a[PC], b[PC];
@@ -560,7 +605,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
     float* xch = reinterpret_cast<float*>(smem_raw + K::kStageBytes);
     float* cbuf = reinterpret_cast<float*>(smem_raw + K::kStageBytes + K::kXchBytes);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + K::kStageBytes + K::kXchBytes + K::kCBytes);
-    const uint32_t bar_tma = smem_u32(bars), bar_full0 = smem_u32(bars + 1);
+    const uint32_t bar_tma = smem_u32(bars), bar_x0 = smem_u32(bars + 1);   // bar_x0: xbar[0][0]
     [[maybe_unused]] float* hist_in = reinterpret_cast<float*>(smem_raw + K::kSmemBytes);   // CHAIN: [step][warp][8], then history-out
     static_assert(!CHAIN || (MODE == kForward && K::kChainFits), "chained strips: forward kernels of the 8-warp configurations");
 
@@ -578,17 +623,21 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
     xc.step = 0;
 #endif
     xc.base = xch + 4 + lane * PC;     // 4 zero floats lead every exchange row
-    xc.bar_full0 = bar_full0;
+    xc.bar_own = bar_x0 + 8 * wy;
     xc.has_up = crank > 0;
     xc.has_dn = crank + 1 < csize;
-    xc.up_data = xc.has_up ? map_to_cta(smem_u32(xc.base + (K::kSlots - 1) * TWX), crank - 1) : 0u;
-    xc.up_bar = xc.has_up ? map_to_cta(bar_full0, crank - 1) : 0u;
-    xc.dn_data = xc.has_dn ? map_to_cta(smem_u32(xc.base), crank + 1) : 0u;
-    xc.dn_bar = xc.has_dn ? map_to_cta(bar_full0, crank + 1) : 0u;
-    xc.rx_bytes = (uint32_t)((xc.has_up ? 1 : 0) + (xc.has_dn ? 1 : 0)) * TW * sizeof(float);
     xc.remote_up = xc.has_up && wy == 0;
     xc.remote_dn = xc.has_dn && wy == NW - 1;
-    xc.my_tx = wy == 0 ? xc.rx_bytes : 0u;
+    xc.rm_data = xc.remote_up ? map_to_cta(smem_u32(xc.base + (K::kSlots - 1) * TWX), crank - 1)
+               : xc.remote_dn ? map_to_cta(smem_u32(xc.base), crank + 1) : 0u;
+    xc.rm_bar = xc.remote_up ? map_to_cta(bar_x0 + 8 * (NW - 1), crank - 1) : xc.remote_dn ? map_to_cta(bar_x0, crank + 1) : 0u;
+    {
+        // lane 0 serves the reader above my rows, lane 1 the reader below (see Xch)
+        const bool up = lane == 0;
+        const bool edge = up ? wy == 0 : wy == NW - 1;           // the reader is in the neighbour CTA (if any)
+        const bool remote = up ? xc.has_up : xc.has_dn;
+        xc.arr_bar = lane >= 2 || (edge && !remote) ? 0u : edge ? xc.bar_own : xc.bar_own + (up ? -8 : 8);
+    }
     xc.first_lane = lane == 0;
     xc.last_lane = lane == 31;
     xc.cbuf = cbuf + (size_t)(wy * PR) * TW + lane * PC;
@@ -630,8 +679,13 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
 
     if (tid == 0) {
         mbar_init(bar_tma, 1);
-        mbar_init(bar_full0, NW);
-        mbar_init(bar_full0 + 8, NW);
+        // arrivals per phase of warp v's barriers: one per local neighbour warp, plus v's own arrival that arms the bytes
+        // of the neighbour CTA at the CTA's edges
+        for (int v = 0; v < NW; ++v) {
+            const uint32_t n = (v > 0) + (v < NW - 1) + (v == 0 && xc.has_up) + (v == NW - 1 && xc.has_dn);
+            mbar_init(bar_x0 + 8 * v, n);
+            mbar_init(bar_x0 + K::kXBarParity + 8 * v, n);
+        }
         fence_barrier_init();
         fence_proxy_async();
         if (task < n_tasks) issue_stage(task);
