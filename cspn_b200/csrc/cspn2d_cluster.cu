@@ -99,6 +99,22 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
             : "memory");
     } while (!done);
 }
+// For waits expected to last thousands of cycles (the producer warps): with the suspend-time hint (in ns) the warp
+// sleeps in the try_wait until the phase completes or the hint expires, rather than polling
+__device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    do {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"
+            "selp.u32 %0, 1, 0, p;\n"
+            "}\n"
+            : "=r"(done)
+            : "r"(bar), "r"(parity), "r"(1000000u)
+            : "memory");
+    } while (!done);
+}
 // The exchange barriers: forms that address `bar` + OFF bytes (OFF = the parity's offset, an immediate in the address
 // rather than one more register per parity)
 template <uint32_t OFF>
@@ -208,13 +224,26 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 //                             column tile_x0-4 (TMA needs a 16-byte aligned innermost origin, so the +-1 column
 //                             shift of cspn.py:105-129 cannot ride on the box origin; the row shift dy_k does)
 //   then xch[2][2*NW+2][TW]   row-exchange buffers (parity, slot, column)
-//   then cbuf[RB][TW]         folded constant term c' of the current task
-//   then 1 + 2*NW mbarriers   tma, then the row-exchange barriers xbar[parity][warp]
+//   then cbuf[RB][TW]         folded constant term c' of the current task (kSplit: two, current and next task)
+//   then d0[RB][TW]           kSplit: the next task's start value d_0
+//   then 1 + 2*NW mbarriers   tma, then the row-exchange barriers xbar[parity][warp] (kSplit: then `ready`, `free`, `hist`)
+//   then (CHAIN) history      [in][out] pairs: one, kSplit: two (current and next task)
 //
 // Arithmetic is scalar FFMA: sm_90 has no packed FP32 FMA, and the stencil has no contraction for the tensor cores.
+//
+// kSplit configurations add a producer warpgroup (4 warps) to the NW consumer warps: while the consumers iterate task i,
+// the producers stage task i+1's guidance, normalise it in place (w'_k of pixel (r, x) overwrites stage[k][r][4+x]), and
+// write its c' into the second cbuf and its d_0 into the d0 tile.  At the task boundary the consumers then only load
+// their w' and d_0 from shared memory, instead of waiting for TMA and global loads and normalising.  12 warps leave 168
+// registers per thread (65 536 / 384, rounded down to 8), which the step loop of PR <= 3 fits without spills once the
+// prologue has left it; PR = 4 and 5 need 225-255 and keep the inline prologue.  (Rebalancing with setmaxnreg, 96 for
+// the producers and 208 for the consumers, made the producers spill and bought the consumers nothing.)
 template <int PR, int PC, int NW>
 struct Cfg {
-    static constexpr int kThreads = 32 * NW;
+    static constexpr int kThreads = 32 * NW;   // consumer (propagating) threads
+    static constexpr bool kSplit = NW == 8 && PR <= 3;
+    static constexpr int kProducerThreads = kSplit ? 128 : 0;
+    static constexpr int kBlockThreads = kThreads + kProducerThreads;
     static constexpr int RB = NW * PR;   // rows per CTA band
     static constexpr int TW = 32 * PC;   // tile (strip) width
     static constexpr int TWP = TW + 8;   // staged row pitch: 4 apron columns on each side
@@ -229,16 +258,20 @@ struct Cfg {
     // the folded constant term c' (one float per pixel) lives in shared memory: it is read once per pixel and
     // iteration (one LDS.128 per patch row), which frees PR*PC registers per thread
     static constexpr size_t kCBytes = (size_t)RB * TW * sizeof(float);
+    static constexpr int kBufs = kSplit ? 2 : 1;   // cbuf and history sets: the producers fill the next task's
+    static constexpr size_t kD0Bytes = kSplit ? kCBytes : 0;
     // one exchange mbarrier per warp and parity (the parity-1 set follows the parity-0 set), after the TMA barrier;
-    // rounded up to 16 bytes: the chained-strip history behind it is read as float4
+    // kSplit: then `ready` (the producers have prepared the next task), `free` (the consumers have read the stage) and
+    // `hist` (chained strips: the consumers have copied the task's history out).
+    // Rounded up to 16 bytes: the chained-strip history behind it is read as float4
     static constexpr uint32_t kXBarParity = 8 * NW;
-    static constexpr size_t kBarBytes = (8 + 2 * kXBarParity + 15) / 16 * 16;
-    static constexpr size_t kSmemBytes = kStageBytes + kXchBytes + kCBytes + kBarBytes;
+    static constexpr size_t kBarBytes = (8 + 2 * kXBarParity + (kSplit ? 24 : 0) + 15) / 16 * 16;
+    static constexpr size_t kSmemBytes = kStageBytes + kXchBytes + kBufs * kCBytes + kD0Bytes + kBarBytes;
     // chained strips: the recorded column of the left neighbour strip (in) and of this strip (out), [step][warp][8 rows]
     static constexpr int kChainMaxIters = cspn::kChainMaxIters;
     static constexpr int kHistRow = NW * 8;
     static constexpr size_t kHistBytes = (size_t)kChainMaxIters * kHistRow * sizeof(float);
-    static constexpr size_t kSmemBytesChain = kSmemBytes + 2 * kHistBytes;
+    static constexpr size_t kSmemBytesChain = kSmemBytes + kBufs * 2 * kHistBytes;
     static constexpr bool kChainFits = kSmemBytesChain <= 232448 && PR <= 8;
     static_assert(PC == 4, "vectorised global/shared accesses below assume 4 columns per thread");
     static_assert(TWP <= 256, "TMA box <= 256 columns");
@@ -278,10 +311,12 @@ __device__ __forceinline__ void store_row_remote(uint32_t addr, const float (&v)
 }
 
 // -DCSPN_TRACE: clock stamps of cluster 0's tasks 1..kTraceTasks (steady state), lane 0 of every warp:
-// trace[((slot*16 + cta)*8 + warp)*kTraceEvents + event].  Events: 0 task start, 1 guidance landed, 2 prologue done,
+// trace[((slot*16 + cta)*kTraceWarps + warp)*kTraceEvents + event].  Events: 0 task start, 1 guidance landed, 2 prologue done,
 // 3 staging buffer released, 4 exchange buffers free, 5+3t / 6+3t / 7+3t = step t before wait / after wait / after
 // publish, kTraceEvents-2 loop done, kTraceEvents-1 stored.
-constexpr int kTraceTasks = 4, kTraceEvents = 5 + 3 * 64 + 2;
+// Producer warps (kSplit kernels; rows 8..11 of a CTA) stamp the task they prepare: 0 waiting for the stage, 1 stage free,
+// 2 task ready.  With a producer, consumer events 1 / 2 / 3 are: task ready, w' and d_0 loaded, cluster wait done.
+constexpr int kTraceTasks = 4, kTraceEvents = 5 + 3 * 64 + 2, kTraceWarps = 12;
 #ifdef CSPN_TRACE
 #define CSPN_STAMP(xc, ev) do { if ((xc).tr) (xc).tr[(ev)] = clock64(); } while (0)
 #else
@@ -592,10 +627,100 @@ __device__ __forceinline__ void iterate_adj(const Xch& x, int wy, uint32_t phase
     }
 }
 
+// ---- prologue: affinity normalisation + mask folding of one patch row (cspn.py:85-144, 63-64) ------------------------
+// a_k(y,x) = g_k(y+dy_k, x+dx_k): dy_k came with the TMA box, dx_k is applied here: the thread reads its own PC columns of
+// plane k (`row0`: its first column in plane 0; plane k lies k * `plane` floats further) and takes the missing neighbour
+// column from the next / previous lane (tile edge lanes read the apron column of the staged row instead).  No lane reads
+// another lane's columns from memory, so w' may overwrite the row in place afterwards.
+template <int PC, bool ABS>
+__device__ __forceinline__ void gather_row(const float* row0, size_t plane, int lane, float (&a)[8][PC], float (&S)[PC]) {
+#pragma unroll
+    for (int j = 0; j < PC; ++j) S[j] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const float* row = row0 + k * plane;
+        float v[PC];
+        load_row_smem(row, v);
+        if (off2_dx(k) == 1) {
+            float nb = __shfl_down_sync(0xffffffffu, v[0], 1);
+            if (lane == 31) nb = row[PC];
+#pragma unroll
+            for (int j = 0; j < PC - 1; ++j) a[k][j] = v[j + 1];
+            a[k][PC - 1] = nb;
+        } else if (off2_dx(k) == -1) {
+            float nb = __shfl_up_sync(0xffffffffu, v[PC - 1], 1);
+            if (lane == 0) nb = row[-1];
+#pragma unroll
+            for (int j = PC - 1; j > 0; --j) a[k][j] = v[j - 1];
+            a[k][0] = nb;
+        } else {
+#pragma unroll
+            for (int j = 0; j < PC; ++j) a[k][j] = v[j];
+        }
+#pragma unroll
+        for (int j = 0; j < PC; ++j) {
+            if (ABS) a[k][j] = fabsf(a[k][j]);        // cspn.py:88-89
+            S[j] += fabsf(a[k][j]);                    // cspn.py:135-136
+        }
+    }
+}
+// Folded weights w'_k and constant term c' of one patch row from its gathered affinities a, S = sum_k |a_k|, the mask
+// m = sign(sparse) and d_0.  `in`: the row lies inside the image (else w' = 0 and c' = 0: the pixel stays 0 forever).
+template <int PC>
+__device__ __forceinline__ void fold_row(const float (&a)[8][PC], const float (&S)[PC], const float (&mrow)[PC], const float (&d)[PC],
+                                         bool in, float (&w)[PC][8], float (&cj)[PC]) {
+    bool exact_div = false;
+#pragma unroll
+    for (int j = 0; j < PC; ++j) {
+        const float inv = rcp_approx(S[j]);
+        const float om = 1.f - mrow[j];
+        const float scale = in ? om * inv : 0.f;
+        float sw = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) { w[j][k] = a[k][j] * scale; sw += w[j][k]; }
+        // (1-m)(1 - gate_sum) + m == 1 - sum_k w'_k, formed from the quotients as cspn.py:139 does
+        cj[j] = in ? (1.f - sw) * d[j] : 0.f;
+        // a * (1/S) is a / S to 2 ulp and has the same 0/0, x/inf and inf/inf results, EXCEPT when 1/S overflows
+        // (S subnormal): there the reference's quotient (cspn.py:138) is an ordinary number
+        exact_div |= in && (inv > 8.0e37f);
+    }
+    if (exact_div) {                                   // cold: IEEE division, the reference's own expression
+#pragma unroll
+        for (int j = 0; j < PC; ++j) {
+            const float om = 1.f - mrow[j];
+            float gsum = 0.f;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const float q = __fdiv_rn(a[k][j], S[j]);
+                gsum += q;                             // gate_sum, cspn.py:139
+                w[j][k] = om * q;
+            }
+            cj[j] = (om * (1.f - gsum) + mrow[j]) * d[j];
+        }
+    }
+}
+
+__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    return done != 0;
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+
 // GENERAL = false compiles out row bands and the continuation input of multi-pass plans: the common single-pass,
 // single-band launch (every BASELINE 2D config) pays nothing for them.
 template <int PR, int PC, int NW, bool ABS, bool GENERAL, int MODE = kForward, bool CHAIN = false>
-__global__ void __launch_bounds__(32 * NW, 1)
+__global__ void __launch_bounds__(Cfg<PR, PC, NW>::kBlockThreads, 1)
 cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __grid_constant__ CUtensorMap tm_blur,
                       const __grid_constant__ CUtensorMap tm_sparse, const __grid_constant__ ClusterParams prm) {
     using K = Cfg<PR, PC, NW>;
@@ -604,9 +729,13 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
     float* stage = reinterpret_cast<float*>(smem_raw);
     float* xch = reinterpret_cast<float*>(smem_raw + K::kStageBytes);
     float* cbuf = reinterpret_cast<float*>(smem_raw + K::kStageBytes + K::kXchBytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + K::kStageBytes + K::kXchBytes + K::kCBytes);
+    [[maybe_unused]] float* d0buf = reinterpret_cast<float*>(smem_raw + K::kStageBytes + K::kXchBytes + K::kBufs * K::kCBytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + K::kStageBytes + K::kXchBytes + K::kBufs * K::kCBytes + K::kD0Bytes);
     const uint32_t bar_tma = smem_u32(bars), bar_x0 = smem_u32(bars + 1);   // bar_x0: xbar[0][0]
+    [[maybe_unused]] const uint32_t bar_ready = bar_x0 + 2 * K::kXBarParity, bar_free = bar_ready + 8,
+                                     bar_hist = bar_free + 8;   // kSplit
     [[maybe_unused]] float* hist_in = reinterpret_cast<float*>(smem_raw + K::kSmemBytes);   // CHAIN: [step][warp][8], then history-out
+    constexpr size_t kHistPair = 2 * K::kHistBytes / sizeof(float);   // floats from one [in][out] history pair to the next
     static_assert(!CHAIN || (MODE == kForward && K::kChainFits), "chained strips: forward kernels of the 8-warp configurations");
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -686,28 +815,181 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
             mbar_init(bar_x0 + 8 * v, n);
             mbar_init(bar_x0 + K::kXBarParity + 8 * v, n);
         }
+        if constexpr (K::kSplit) {
+            mbar_init(bar_ready, K::kProducerThreads);
+            mbar_init(bar_free, K::kThreads);
+            mbar_init(bar_hist, K::kThreads);
+        }
         fence_barrier_init();
         fence_proxy_async();
-        if (task < n_tasks) issue_stage(task);
+        if (!K::kSplit && task < n_tasks) issue_stage(task);
     }
     // every CTA's barriers must be initialised before a neighbour's st.async can target them
     cluster_arrive();
     // halo slots without a neighbour stay zero for the whole kernel (rows outside the image), and so do the 4 pad
     // floats on either side of every row (columns outside the tile).  Nobody else ever writes these locations.
-    if (!xc.has_up)
-        for (int i = tid; i < TWX; i += K::kThreads) { xch[i] = 0.f; xch[(size_t)K::kSlots * TWX + i] = 0.f; }
-    if (!xc.has_dn)
-        for (int i = tid; i < TWX; i += K::kThreads) {
-            xch[(size_t)(K::kSlots - 1) * TWX + i] = 0.f;
-            xch[(size_t)(2 * K::kSlots - 1) * TWX + i] = 0.f;
+    if (tid < K::kThreads) {
+        if (!xc.has_up)
+            for (int i = tid; i < TWX; i += K::kThreads) { xch[i] = 0.f; xch[(size_t)K::kSlots * TWX + i] = 0.f; }
+        if (!xc.has_dn)
+            for (int i = tid; i < TWX; i += K::kThreads) {
+                xch[(size_t)(K::kSlots - 1) * TWX + i] = 0.f;
+                xch[(size_t)(2 * K::kSlots - 1) * TWX + i] = 0.f;
+            }
+        for (int i = tid; i < 2 * K::kSlots * 8; i += K::kThreads) {
+            const int row = i >> 3, c = i & 7;
+            xch[(size_t)row * TWX + (c < 4 ? c : TW + c)] = 0.f;
         }
-    for (int i = tid; i < 2 * K::kSlots * 8; i += K::kThreads) {
-        const int row = i >> 3, c = i & 7;
-        xch[(size_t)row * TWX + (c < 4 ? c : TW + c)] = 0.f;
     }
     cluster_wait();
 
     uint32_t ph_tma = 0, ph0 = 0, ph1 = 0;  // phase parities of the three mbarriers (they run on across tasks)
+    if constexpr (K::kSplit) {
+        if (wy >= NW) {
+            // ---- producer warpgroup: prepares task t+Q in the stage, cbuf[nb], d0buf and history pair nb while the
+            // consumers iterate task t.  It takes part in every cluster-barrier phase the consumers take part in (the
+            // barrier counts every thread of the CTA), so it leaves only after the last one.
+            const int ptid = tid - K::kThreads, pw = wy - NW;
+            // chained strips: the consumers copy a finished task's history out and arrive on `hist`; producer thread 0 then
+            // publishes the strip's flag.  It does so while it spins on a neighbour strip's flag too, so publishing a flag
+            // never waits for the preparation of a later task (which may itself wait for a flag).
+            [[maybe_unused]] size_t pend_blk = ~size_t(0);   // flag to publish, ~0: none
+            [[maybe_unused]] uint32_t ph_hist = 0;
+            [[maybe_unused]] auto publish_flag = [&](bool block) {
+                if (ptid != 0 || pend_blk == ~size_t(0)) return;
+                if (block) mbar_wait_sleep(bar_hist, ph_hist);
+                else if (!mbar_test(bar_hist, ph_hist)) return;
+                ph_hist ^= 1;
+                // release is cumulative over the consumers' stores that the barrier made visible to this thread
+                asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(prm.flags + pend_blk), "r"(1u) : "memory");
+                pend_blk = ~size_t(0);
+            };
+            auto prepare = [&](int t, int nb) {
+                int strip = t % prm.n_strips, qi = t / prm.n_strips;
+                if constexpr (CHAIN) chain_decode(t, strip, qi);
+                const int band = GENERAL ? qi % prm.n_bands : 0;
+                const int bc = GENERAL ? qi / prm.n_bands : qi;
+                const int y_cta = (GENERAL ? prm.band_y0[band] : 0) + cta_dy;
+                const int x_thr = prm.tile_x0[strip] + lane * PC;
+                const bool col_in = (x_thr >= 0) && (x_thr < W);
+                if (ptid == 0) {
+                    fence_proxy_async();   // generic-proxy reads and in-place writes of `stage` before the async-proxy writes
+                    issue_stage(t);
+                }
+                float* cb = cbuf + (size_t)nb * RB * TW;
+                // blur_depth rows go straight into this thread's slots of d0buf, sparse_depth rows (only their sign is used)
+                // into its slots of the c' buffer: both are read back by this thread only, before c' overwrites them
+                const float* blur = prm.blur + (size_t)bc * HW;
+                const float* sparse = prm.sparse ? prm.sparse + (size_t)(bc / prm.C) * HW : nullptr;
+#pragma unroll
+                for (int h = 0; h < NW / 4; ++h) {
+#pragma unroll
+                    for (int r = 0; r < PR; ++r) {
+                        const int rr = (pw + 4 * h) * PR + r, y = y_cta + rr;
+                        float* dc = d0buf + (size_t)rr * TW + lane * PC;
+                        float* sc = cb + (size_t)rr * TW + lane * PC;
+                        if (col_in && y < H) {
+                            cp_async16(smem_u32(dc), blur + (size_t)y * W + x_thr);
+                            if (sparse) cp_async16(smem_u32(sc), sparse + (size_t)y * W + x_thr);
+                            else *reinterpret_cast<float4*>(sc) = make_float4(0.f, 0.f, 0.f, 0.f);
+                        } else {
+                            *reinterpret_cast<float4*>(dc) = make_float4(0.f, 0.f, 0.f, 0.f);   // outside the image: d = 0
+                            *reinterpret_cast<float4*>(sc) = make_float4(0.f, 0.f, 0.f, 0.f);
+                        }
+                    }
+                }
+                if constexpr (CHAIN) {
+                    float4* hin = reinterpret_cast<float4*>(hist_in + nb * kHistPair);
+                    const int n16 = prm.iters * K::kHistRow / 4;
+                    if (strip == 0) {      // image border on the left: column -1 is the reference's zero padding
+                        for (int i = ptid; i < n16; i += K::kProducerThreads) hin[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    } else {
+                        // the left neighbour strip's history block of this CTA's rows must be complete (normally it has been for
+                        // a long time).  That strip is an earlier task, so this wait cannot close a cycle.
+                        const size_t blk = ((size_t)(strip - 1) * (prm.n_tasks / prm.n_strips) + qi) * csize + crank;
+                        for (;;) {
+                            unsigned ready;
+                            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(ready) : "l"(prm.flags + blk) : "memory");
+                            if (ready != 0u) break;
+                            publish_flag(false);
+                        }
+                        const float4* src = reinterpret_cast<const float4*>(prm.hist + blk * (size_t)(prm.iters * K::kHistRow));
+                        for (int i = ptid; i < n16; i += K::kProducerThreads) hin[i] = __ldcg(src + i);
+                    }
+                }
+                mbar_wait_sleep(bar_tma, ph_tma);
+                ph_tma ^= 1;
+                cp_async_wait_all();
+#pragma unroll 1
+                for (int h = 0; h < NW / 4; ++h) {
+#pragma unroll
+                    for (int r = 0; r < PR; ++r) {
+                        const int rr = (pw + 4 * h) * PR + r, y = y_cta + rr;
+                        const bool in = col_in && y < H;
+                        float* row0 = stage + (size_t)rr * TWP + 4 + lane * PC;
+                        float* dc = d0buf + (size_t)rr * TW + lane * PC;
+                        float* sc = cb + (size_t)rr * TW + lane * PC;
+                        float S[PC], a[8][PC], d[PC], w[PC][8], cj[PC];
+                        gather_row<PC, ABS>(row0, (size_t)RB * TWP, lane, a, S);
+                        load_row_smem(dc, d);
+                        const float4 sv = *reinterpret_cast<const float4*>(sc);
+                        const float mrow[PC] = {signf(sv.x), signf(sv.y), signf(sv.z), signf(sv.w)};
+                        fold_row<PC>(a, S, mrow, d, in, w, cj);
+#pragma unroll
+                        for (int k = 0; k < 8; ++k)
+                            *reinterpret_cast<float4*>(row0 + k * (size_t)RB * TWP) = make_float4(w[0][k], w[1][k], w[2][k], w[3][k]);
+                        if constexpr (MODE != kAdjoint) store_row_smem(sc, cj);   // the adjoint has no constant term
+                        // a pass after the first continues from the previous pass's result; c' above still used d_0
+                        if (GENERAL && prm.init != nullptr && in)
+                            *reinterpret_cast<float4*>(dc) =
+                                __ldg(reinterpret_cast<const float4*>(prm.init + (size_t)bc * HW + (size_t)y * W + x_thr));
+                    }
+                }
+                mbar_arrive(bar_ready);
+            };
+            // one cluster-barrier phase per task, as the consumers (every grid has at least one task per cluster); the
+            // last wait is followed by the exit, as the consumers' is
+            uint32_t ph_free = 0;
+            int nb = 0;
+            prepare(task, nb);
+            for (;;) {
+                cluster_arrive_relaxed();           // this phase guards the exchange buffers, which the producers never touch
+                if constexpr (CHAIN) {
+                    int strip, qi;
+                    chain_decode(task, strip, qi);
+                    if (strip + 1 < prm.n_strips) pend_blk = ((size_t)strip * (prm.n_tasks / prm.n_strips) + qi) * csize + crank;
+                }
+                const int next = task + task_stride;
+                if (next >= n_tasks) break;
+                {
+#ifdef CSPN_TRACE
+                    const int slot = (next - (int)cluster_id_x()) / task_stride - 1;
+                    unsigned long long* tr = (prm.trace && cluster_id_x() == 0 && lane == 0 && slot < kTraceTasks)
+                                                 ? prm.trace + ((size_t)(slot * 16 + (int)crank) * kTraceWarps + wy) * kTraceEvents : nullptr;
+                    if (tr) tr[0] = clock64();
+#endif
+                    mbar_wait_sleep(bar_free, ph_free);   // the consumers have loaded this task's w' and d_0
+                    ph_free ^= 1;
+#ifdef CSPN_TRACE
+                    if (tr) tr[1] = clock64();
+#endif
+                    nb ^= 1;
+                    prepare(next, nb);
+#ifdef CSPN_TRACE
+                    if (tr) tr[2] = clock64();
+#endif
+                }
+                if constexpr (CHAIN) publish_flag(true);
+                cluster_wait();
+                task = next;
+            }
+            if constexpr (CHAIN) publish_flag(true);
+            cluster_wait();
+            return;
+        }
+    }
+    [[maybe_unused]] uint32_t ph_ready = 0;
+    [[maybe_unused]] int cur = 0;           // kSplit: cbuf / history pair of the current task
     bool first = true;
     for (; task < n_tasks; task += task_stride) {
         const int nq = prm.n_tasks / prm.n_strips;
@@ -724,12 +1006,43 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
         {
             const int slot = (task - (int)cluster_id_x()) / task_stride - 1;    // the cluster's 2nd, 3rd, ... task
             xc.tr = (prm.trace && cluster_id_x() == 0 && lane == 0 && slot >= 0 && slot < kTraceTasks)
-                        ? prm.trace + ((size_t)(slot * 16 + (int)crank) * 8 + wy) * kTraceEvents : nullptr;
+                        ? prm.trace + ((size_t)(slot * 16 + (int)crank) * kTraceWarps + wy) * kTraceEvents : nullptr;
             xc.step = 0;
         }
         CSPN_STAMP(xc, 0);
 #endif
 
+        // ---- thread state ---------------------------------------------------------------------------
+        float w[PR][PC][8], d[PR][PC];
+        [[maybe_unused]] bool has_out = false;
+        if constexpr (CHAIN) {
+            has_out = strip + 1 < prm.n_strips;
+            xc.store_hist = has_out && lane == prm.chain_lane;
+        }
+        bool early_publish = false;
+        if constexpr (K::kSplit) {
+            // ---- task boundary: the producers have staged, normalised and folded this task ------------------------
+            xc.cbuf = cbuf + ((size_t)cur * RB + wy * PR) * TW + lane * PC;
+            if constexpr (CHAIN) xc.hin = smem_u32(hist_in + cur * kHistPair + wy * 8);
+            mbar_wait(bar_ready, ph_ready);
+            ph_ready ^= 1;
+            CSPN_STAMP(xc, 1);
+#pragma unroll
+            for (int r = 0; r < PR; ++r) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    const float4 v = *reinterpret_cast<const float4*>(stage + ((size_t)k * RB + wy * PR + r) * TWP + 4 + lane * PC);
+                    w[r][0][k] = v.x; w[r][1][k] = v.y; w[r][2][k] = v.z; w[r][3][k] = v.w;
+                }
+                load_row_smem(d0buf + (size_t)(wy * PR + r) * TW + lane * PC, d[r]);
+            }
+            mbar_arrive(bar_free);         // the producers may stage the next task
+            CSPN_STAMP(xc, 2);
+            // the neighbours have finished reading the exchange buffers of the previous task (they arrived right after
+            // their step loop)
+            if (!first) cluster_wait();
+            CSPN_STAMP(xc, 3);
+        } else {
         // chained strip with a left neighbour: ask for that strip's "history complete" flag now, look at the answer after the
         // loads below have been issued (it was set long ago unless the batch is small)
         [[maybe_unused]] unsigned hist_ready = 1u;
@@ -741,8 +1054,6 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
             }
         }
 
-        // ---- thread state ---------------------------------------------------------------------------
-        float w[PR][PC][8], d[PR][PC];
         const float* blur = prm.blur + (size_t)bc * HW;
         const float* sparse = prm.sparse ? prm.sparse + (size_t)b * HW : nullptr;
 
@@ -768,11 +1079,8 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
         // the neighbours have finished reading the exchange buffers of the previous task (they arrived right after their
         // step loop): waited for here, under the loads
         if (!first) cluster_wait();
-        [[maybe_unused]] bool has_out = false;
         if constexpr (CHAIN) {
             const bool has_in = strip > 0;
-            has_out = strip + 1 < prm.n_strips;
-            xc.store_hist = has_out && lane == prm.chain_lane;
             if (!has_in) {      // image border on the left: column -1 is the reference's zero padding
                 const int n16 = prm.iters * K::kHistRow / 4;
                 for (int i = tid; i < n16; i += K::kThreads) reinterpret_cast<float4*>(hist_in)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -790,50 +1098,18 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
         // the first row exchange of a task needs only blur_depth: it is published from inside the prologue (after row 0),
         // so its DSMEM round trip hides under the normalisation of the other rows instead of stalling the first step.
         // (A continuation pass starts from the previous pass's result, read further down: it publishes after the prologue.)
-        const bool early_publish = (MODE != kAdjoint) && !(GENERAL && init != nullptr);
+        early_publish = (MODE != kAdjoint) && !(GENERAL && init != nullptr);
 
         mbar_wait(bar_tma, ph_tma);
         ph_tma ^= 1;
         CSPN_STAMP(xc, 1);
 
         // ---- prologue: affinity normalisation + mask folding (cspn.py:85-144, 63-64) ------------------
-        // a_k(y,x) = g_k(y+dy_k, x+dx_k): dy_k came with the TMA box, dx_k is applied here: the thread reads its own
-        // PC columns of plane k and takes the missing neighbour column from the next / previous lane (tile edge
-        // lanes read the apron column of the staged row instead).
 #pragma unroll
         for (int r = 0; r < PR; ++r) {
             const int y = y_thr + r;
-            float S[PC], A[PC], a[8][PC];
-#pragma unroll
-            for (int j = 0; j < PC; ++j) { S[j] = 0.f; A[j] = 0.f; }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const float* row = stage + ((size_t)k * RB + wy * PR + r) * TWP + 4 + lane * PC;
-                float v[PC];
-                load_row_smem(row, v);
-                if (off2_dx(k) == 1) {
-                    float nb = __shfl_down_sync(0xffffffffu, v[0], 1);
-                    if (lane == 31) nb = row[PC];
-#pragma unroll
-                    for (int j = 0; j < PC - 1; ++j) a[k][j] = v[j + 1];
-                    a[k][PC - 1] = nb;
-                } else if (off2_dx(k) == -1) {
-                    float nb = __shfl_up_sync(0xffffffffu, v[PC - 1], 1);
-                    if (lane == 0) nb = row[-1];
-#pragma unroll
-                    for (int j = PC - 1; j > 0; --j) a[k][j] = v[j - 1];
-                    a[k][0] = nb;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < PC; ++j) a[k][j] = v[j];
-                }
-#pragma unroll
-                for (int j = 0; j < PC; ++j) {
-                    if (ABS) a[k][j] = fabsf(a[k][j]);        // cspn.py:88-89
-                    S[j] += fabsf(a[k][j]);                    // cspn.py:135-136
-                    A[j] += a[k][j];                           // numerator of gate_sum, cspn.py:139
-                }
-            }
+            float S[PC], a[8][PC];
+            gather_row<PC, ABS>(stage + ((size_t)wy * PR + r) * TWP + 4 + lane * PC, (size_t)RB * TWP, lane, a, S);
             // this row's blur_depth (from the c' slot the cp.async filled) and mask
             if (r == 0) cp_async_wait_all();            // this thread's own copies: no barrier needed
             load_row_smem(my_c + r * TW, d[r]);
@@ -844,36 +1120,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                 publish<PR, PC, NW, 0>(xc, wy, d[0], bot);
             }
             float cj[PC];
-            bool exact_div = false;
-#pragma unroll
-            for (int j = 0; j < PC; ++j) {
-                const bool in = col_in && (y < H);
-                const float inv = rcp_approx(S[j]);
-                const float om = 1.f - mrow[j];
-                const float scale = in ? om * inv : 0.f;      // pixels outside the image: w = 0, c = 0, d = 0 forever
-                float sw = 0.f;
-#pragma unroll
-                for (int k = 0; k < 8; ++k) { w[r][j][k] = a[k][j] * scale; sw += w[r][j][k]; }
-                // (1-m)(1 - gate_sum) + m == 1 - sum_k w'_k, formed from the quotients as cspn.py:139 does
-                cj[j] = in ? (1.f - sw) * d[r][j] : 0.f;
-                // a * (1/S) is a / S to 2 ulp and has the same 0/0, x/inf and inf/inf results, EXCEPT when 1/S overflows
-                // (S subnormal): there the reference's quotient (cspn.py:138) is an ordinary number
-                exact_div |= in && (inv > 8.0e37f);
-            }
-            if (exact_div) {                                   // cold: IEEE division, the reference's own expression
-#pragma unroll
-                for (int j = 0; j < PC; ++j) {
-                    const float om = 1.f - mrow[j];
-                    float gsum = 0.f;
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const float q = __fdiv_rn(a[k][j], S[j]);
-                        gsum += q;                             // gate_sum, cspn.py:139
-                        w[r][j][k] = om * q;
-                    }
-                    cj[j] = (om * (1.f - gsum) + mrow[j]) * d[r][j];
-                }
-            }
+            fold_row<PC>(a, S, mrow, d[r], col_in && (y < H), w[r], cj);
             // only this thread ever reads these values back: no barrier needed
             if constexpr (MODE != kAdjoint) {
                 store_row_smem(const_cast<float*>(xc.cbuf) + r * TW, cj);   // the adjoint has no constant term
@@ -904,6 +1151,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                 if (prm.sparse) tma_prefetch_3d(&tm_sparse, prm.tile_x0[strip_n], y_n, bc_n / prm.C);
             }
         }
+        }   // !kSplit
 
         // ---- the N iterations: registers only, one mbarrier wait each ----------------------------------
         first = false;
@@ -1021,18 +1269,30 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
         }
         if constexpr (CHAIN) {
             if (has_out) {      // uniform over the cluster: hand this CTA's rows of the recorded column to the next strip
-                __syncthreads();                                  // every warp's history stores are in shared memory
                 const size_t blk = ((size_t)strip * nq + qi) * csize + crank;
                 float4* dst = reinterpret_cast<float4*>(prm.hist + blk * (size_t)(prm.iters * K::kHistRow));
-                const float4* src = reinterpret_cast<const float4*>(hist_in + K::kHistBytes / sizeof(float));
-                const int n16 = prm.iters * K::kHistRow / 4;
-                for (int i = tid; i < n16; i += K::kThreads) __stcg(dst + i, src[i]);
-                __syncthreads();
-                // release is cumulative over what the barrier made visible to this thread: no separate fence
-                if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(prm.flags + blk), "r"(1u) : "memory");
+                const float4* src = reinterpret_cast<const float4*>(hist_in + cur * kHistPair + K::kHistBytes / sizeof(float));
+                if constexpr (K::kSplit) {
+                    // each warp copies its own 8 floats of every step (written by its own lane) and tells the producers, who
+                    // publish the flag: no barrier across warps and no release latency on the way to the next task
+                    __syncwarp();
+                    for (int i = lane; i < 2 * prm.iters; i += 32) {
+                        const int o = (i >> 1) * (K::kHistRow / 4) + wy * 2 + (i & 1);
+                        __stcg(dst + o, src[o]);
+                    }
+                    mbar_arrive(bar_hist);
+                } else {
+                    __syncthreads();                              // every warp's history stores are in shared memory
+                    const int n16 = prm.iters * K::kHistRow / 4;
+                    for (int i = tid; i < n16; i += K::kThreads) __stcg(dst + i, src[i]);
+                    __syncthreads();
+                    // release is cumulative over what the barrier made visible to this thread: no separate fence
+                    if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(prm.flags + blk), "r"(1u) : "memory");
+                }
             }
         }
         CSPN_STAMP(xc, kTraceEvents - 1);
+        if constexpr (K::kSplit) cur ^= 1;
     }
     // No CTA may exit while a neighbour could still address its shared memory.
     if (!first) cluster_wait();
@@ -1047,6 +1307,7 @@ struct KernelCfg {
     const void* fn_adj[2];     // kAdjoint    [norm_abs]
     const void* fn_chain[2][2];   // kForward with chained strips: [general][norm_abs]; null when the configuration has no such kernel
     size_t smem, smem_chain;
+    int threads;               // per CTA: the consumer warps, plus the producer warpgroup of kSplit configurations
     int RB() const { return PR * NW; }
     int TW() const { return 32 * PC; }
 };
@@ -1061,7 +1322,7 @@ KernelCfg make_cfg() {
                      {(const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kAdjoint>,
                       (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kAdjoint>},
                      {{nullptr, nullptr}, {nullptr, nullptr}},
-                     Cfg<PR, PC, NW>::kSmemBytes, 0};
+                     Cfg<PR, PC, NW>::kSmemBytes, 0, Cfg<PR, PC, NW>::kBlockThreads};
 }
 template <int PR, int PC, int NW>
 KernelCfg make_cfg_chain() {
@@ -1081,7 +1342,7 @@ KernelCfg make_cfg_chain() {
 const std::vector<KernelCfg>& configs() {
     static const std::vector<KernelCfg> v = [] {
         KernelCfg k{5, 4, 8, {{nullptr, nullptr}, {nullptr, nullptr}}, {nullptr, nullptr}, {nullptr, nullptr}, {{nullptr, nullptr}, {nullptr, nullptr}},
-                    Cfg<5, 4, 8>::kSmemBytes, Cfg<5, 4, 8>::kSmemBytesChain};
+                    Cfg<5, 4, 8>::kSmemBytes, Cfg<5, 4, 8>::kSmemBytesChain, Cfg<5, 4, 8>::kBlockThreads};
         k.fn[0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false>;
         k.fn_chain[0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false, kForward, true>;
         return std::vector<KernelCfg>{k};
@@ -1159,7 +1420,7 @@ int max_active_clusters(int ci, int cs, int dev, bool chained = false) {
     }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(cs * 64);
-    cfg.blockDim = dim3(32 * k.NW);
+    cfg.blockDim = dim3(k.threads);
     cfg.dynamicSmemBytes = chained ? k.smem_chain : k.smem;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
@@ -1215,7 +1476,8 @@ bool layout_1d(int L, int T, int halo, int align, int min_useful, int max_n, int
 // Best (configuration, cluster size, strips, bands) for one pass of `iters` steps: minimises SM time per image.
 // Deliberately independent of B and C, so the same image gets the same tiling (hence bit-identical results) whatever
 // batch it is part of.  `dev` < 0: no device query (planning without a GPU): assume the H100 SXM occupancy table
-// measured by tools/probe.cu.
+// measured by tools/probe.cu (one CTA per SM; it holds for the 384-thread producer kernels too, which the device query
+// confirms: 7 co-resident 15-CTA clusters of the 3x4x8 chained kernel on an H100 SXM).
 bool plan_pass(int H, int W, int iters, int dev, int forced, bool chained, PassPlan& best) {
     static const int kProbe256[17] = {0, 132, 66, 39, 30, 22, 17, 15, 15, 9, 7, 7, 7, 7, 7, 7, 7};
     const char* fcs = getenv("CSPN_B200_FORCE_CS");   // developer hook for tuning runs (with CSPN_B200_FORCE_PASSES)
@@ -1435,9 +1697,9 @@ int cluster2d_describe(int B, int C, int H, int W, int iters, char* buf, int len
         snprintf(passes, sizeof(passes), "%d passes (%d x %d + %d x %d steps), ", plan.n_pass, plan.n_long, pp.iters + 1,
                  plan.n_pass - plan.n_long, pp.iters);
     return snprintf(buf, len,
-                    "cluster: %spatch %dx%d px/thread, %d warps -> CTA tile %d rows x %d cols, cluster of %d CTAs (%d rows), "
+                    "cluster: %spatch %dx%d px/thread, %d warps%s -> CTA tile %d rows x %d cols, cluster of %d CTAs (%d rows), "
                     "%d %sstrip(s) x %d band(s)/image, %ld tasks, %d co-resident clusters, lane efficiency %.2f, smem %zu B",
-                    passes, k.PR, k.PC, k.NW, k.RB(), k.TW(), pp.cs, pp.cs * k.RB(), pp.n_strips, chained ? "chained " : "", pp.n_bands,
+                    passes, k.PR, k.PC, k.NW, k.threads > 32 * k.NW ? " + 4 producer warps" : "", k.RB(), k.TW(), pp.cs, pp.cs * k.RB(), pp.n_strips, chained ? "chained " : "", pp.n_bands,
                     (long)B * C * pp.n_strips * pp.n_bands, pp.max_clusters,
                     (double)useful_x * useful_y / ((double)pp.n_strips * k.TW() * pp.n_bands * pp.cs * k.RB()),
                     chained ? k.smem_chain : k.smem);
@@ -1583,7 +1845,7 @@ int launch_pass(const Problem2D& p, const PassPlan& pp, const void* fn, const fl
 
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(n_clusters * pp.cs));
-    cfg.blockDim = dim3(32 * k.NW);
+    cfg.blockDim = dim3(k.threads);
     cfg.dynamicSmemBytes = chained ? k.smem_chain : k.smem;
     cfg.stream = stream;
     cudaLaunchAttribute at[2];

@@ -5,7 +5,8 @@
 
 Cluster 0 stamps clock64() (lane 0 of every warp) at the phase boundaries of its 2nd..5th task and around every mbarrier
 wait / publish of the step loop.  Prints where a task's cycles go and, per step, how long warps sit in the wait, how long
-the wait -> publish chain is and how much work separates a publish from the next wait.
+the wait -> publish chain is and how much work separates a publish from the next wait.  Kernels with a producer
+warpgroup (warps 8..11) also print how long the producers wait for the stage and take to prepare a task.
 """
 import ctypes
 import os
@@ -24,7 +25,7 @@ L = _lib.lib()
 L.cspn_debug_set_trace.argtypes = [ctypes.c_void_p]
 L.cspn_debug_set_trace.restype = None
 NEV = L.cspn_debug_trace_events()
-TASKS, CTAS, WARPS = 4, 16, 8
+TASKS, CTAS, WARPS, CONSUMERS = 4, 16, 12, 8
 buf = torch.zeros(TASKS * CTAS * WARPS * NEV, dtype=torch.int64, device='cuda')
 g, d, s = [t.cuda() for t in make_inputs(0, min(B, 8), 1, H, W)]
 if B > 8:
@@ -38,19 +39,30 @@ cspn_b200.propagate2d(g, d, s, N, '8sum', _lib.ALGO_CLUSTER)
 torch.cuda.synchronize()
 L.cspn_debug_set_trace(None)
 print(cspn_b200.describe_plan(B, 1, H, W, N, _lib.ALGO_CLUSTER))
-t = buf.cpu().numpy().reshape(TASKS, CTAS, WARPS, NEV).astype(np.int64)
+t_all = buf.cpu().numpy().reshape(TASKS, CTAS, WARPS, NEV).astype(np.int64)
+t = t_all[:, :, :CONSUMERS]
 ncta = int((t[0, :, 0, 0] != 0).sum())
+split = bool((t_all[:, :ncta, CONSUMERS:, 0] != 0).any())
 print(f'traced {TASKS} tasks of cluster 0, {ncta} CTAs, {N} steps; cycles are SM clocks (clock64)')
+if split:
+    names = ['wait for producers', 'load w\' and d0', 'cluster wait', 'first publish']
+else:
+    names = ['load+tma wait', 'prologue', 'syncthreads', 'issue next + cluster wait']
 for slot in range(TASKS):
     x = t[slot, :ncta]                      # [cta][warp][ev]
     if not x[..., 0].all():
         continue
     e = lambda i: x[..., i].astype(np.float64)
     tot = e(NEV - 1) - e(0)
-    seg = {'load+tma wait': e(1) - e(0), 'prologue': e(2) - e(1), 'syncthreads': e(3) - e(2), 'issue next + cluster wait': e(4) - e(3),
-           'step loop': e(NEV - 2) - e(4), 'epilogue': e(NEV - 1) - e(NEV - 2)}
+    seg = dict(zip(names, [e(1) - e(0), e(2) - e(1), e(3) - e(2), e(4) - e(3)]))
+    seg.update({'step loop': e(NEV - 2) - e(4), 'epilogue': e(NEV - 1) - e(NEV - 2)})
     print(f'task slot {slot}: total {tot.mean():.0f} cycles (min {tot.min():.0f} max {tot.max():.0f})  ' +
           '  '.join(f'{k} {v.mean():.0f}' for k, v in seg.items()))
+    if split:
+        p = t_all[slot, :ncta, CONSUMERS:].astype(np.float64)    # [cta][producer warp][ev]
+        if p[..., 0].all():
+            print(f'   producers: wait for stage {(p[..., 1] - p[..., 0]).mean():.0f}   prepare {(p[..., 2] - p[..., 1]).mean():.0f}   '
+                  f'ready {(x[..., 1].mean() - p[..., 2].mean()):.0f} cycles before the consumers got there')
     steps = N - 1   # the last step has no publish
     w0 = np.stack([e(5 + 3 * k) for k in range(N)], -1)
     w1 = np.stack([e(6 + 3 * k) for k in range(N)], -1)
