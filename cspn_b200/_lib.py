@@ -40,15 +40,18 @@ SIGNATURES = {
     'cspn2d_gates_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn3d_gates_workspace_bytes': (_sz, [_i] * 7),
     'cspn3d_gates_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _sz, _vp]),
+    'cspn3d_gates_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_gates_bwd_workspace_bytes': (_sz, [_i] * 7),
     'cspn3d_gates_bwd_f32': (_i, [_vp] * 5 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_workspace_bytes': (_sz, [_i] * 6),
     'cspn3d_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _sz, _vp]),
+    'cspn3d_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_fwd_f32_host': (_i, [_vp] * 3 + [_i] * 8),
     'cspn3d_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn3d_bwd_f32': (_i, [_vp] * 5 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn3d_k_workspace_bytes': (_sz, [_i] * 7),
     'cspn3d_k_fwd_f32': (_i, [_vp] * 3 + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn3d_k_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn3d_k_bwd_workspace_bytes': (_sz, [_i] * 7),
     'cspn3d_k_bwd_f32': (_i, [_vp] * 5 + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn_depth_metrics_workspace_bytes': (_sz, []),

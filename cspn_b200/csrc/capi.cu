@@ -51,7 +51,7 @@ int check2d(const float* guidance, const float* blur, float* out, int B, int C, 
     return CSPN_OK;
 }
 
-// The destinations of a fused gather (cspn2d_*fwd_gather_f32) and its step count: the checks every gather entry shares
+// The destinations of a fused gather (cspn{2,3}d_*fwd_gather_f32) and its step count: the checks every gather entry shares
 int check_gather(float* const* peer_out, int n_peer, const float* multicast_out, int iters) {
     if (n_peer < 0 || n_peer > 7 || (n_peer > 0 && !peer_out)) { set_error("n_peer must be 0..7 with a pointer array"); return CSPN_ERR_INVALID_ARGUMENT; }
     for (int i = 0; i < n_peer; ++i)
@@ -353,19 +353,45 @@ size_t cspn3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
     return generic3d_workspace_bytes(B, C, D, H, W, iters);
 }
 
-int cspn3d_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int iters,
-                   int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
+static int check3d(const float* guidance, const float* feat, const float* out, int B, int C, int D, int H, int W, int iters,
+                   int norm_type) {
     if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
     if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape"); return CSPN_ERR_INVALID_ARGUMENT; }
     if (iters < 0) { set_error("prop_step must be >= 0"); return CSPN_ERR_INVALID_ARGUMENT; }
     if (norm_type < CSPN_NORM_26SUM || norm_type > CSPN_NORM_PADDLE) { set_error("unknown 3D norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+int cspn3d_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int iters,
+                   int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check3d(guidance, feat, out, B, C, D, H, W, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
     DeviceGuard guard(device_of(feat));
     if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
     int launches = 0;
-    int rc = generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
-                               (cudaStream_t)stream, &launches);
+    rc = generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
+                           (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+int cspn3d_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
+                          float* multicast_out, int B, int C, int D, int H, int W, int iters, int norm_type, void* workspace,
+                          size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check3d(guidance, feat, out, B, C, D, H, W, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
+                           (cudaStream_t)stream, &launches, &fan);
     g_last_launches = launches;
     return rc;
 }
@@ -421,6 +447,28 @@ int cspn3d_k_fwd_f32(const float* guidance, const float* feat, float* out, int B
     int launches = 0;
     rc = widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, norm_type, workspace, workspace_bytes, (cudaStream_t)stream,
                          &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+int cspn3d_k_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
+                            float* multicast_out, int B, int C, int D, int H, int W, int K, int iters, int norm_type,
+                            void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check3d_k(guidance, feat, out, B, C, D, H, W, K, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return cspn3d_fwd_gather_f32(guidance, feat, out, peer_out, n_peer, multicast_out, B, C, D, H, W, iters, norm_type,
+                                     workspace, workspace_bytes, stream);
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, norm_type, workspace, workspace_bytes, (cudaStream_t)stream,
+                         &launches, &fan);
     g_last_launches = launches;
     return rc;
 }
@@ -535,6 +583,25 @@ int cspn3d_gates_fwd_f32(const float* gates, const float* feat, float* out, int 
     if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
     int launches = 0;
     rc = widek3d_gates_forward(gates, feat, out, B, C, D, H, W, K, iters, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+int cspn3d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out, float* const* peer_out, int n_peer,
+                                float* multicast_out, int B, int C, int D, int H, int W, int K, int iters, void* workspace,
+                                size_t workspace_bytes, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_gates(gates, feat, out, B, C, D, H, W, K, iters, true);
+    if (rc != CSPN_OK) return rc;
+    rc = check_gather(peer_out, n_peer, multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(feat));
+    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
+    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
+    int launches = 0;
+    rc = widek3d_gates_forward(gates, feat, out, B, C, D, H, W, K, iters, workspace, workspace_bytes, (cudaStream_t)stream,
+                               &launches, &fan);
     g_last_launches = launches;
     return rc;
 }

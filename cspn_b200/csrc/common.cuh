@@ -89,6 +89,32 @@ struct Fan {
     float* mc;
 };
 
+// The destinations of fan moved `off` floats on, as `out` is for a launch group that starts `off` floats into it
+inline Fan offset_fan(const Fan& f, size_t off) {
+    Fan g{};
+    g.n_peer = f.n_peer;
+    for (int e = 0; e < f.n_peer; ++e) g.peer[e] = f.peer[e] + off;
+    g.mc = f.mc ? f.mc + off : nullptr;
+    return g;
+}
+
+// The FAN epilogue of the 3D step kernels: v, just stored at element o of dst, also to element o of every destination
+__device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float4 v) {
+#pragma unroll
+    for (int e = 0; e < 7; ++e)          // peer GPUs' gather buffers (NVLink stores); n_peer is uniform
+        if (e < fan.n_peer) __stcs(reinterpret_cast<float4*>(fan.peer[e] + o), v);
+    if (fan.mc)                          // NVLS: one store, replicated by the switch
+        asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(fan.mc + o), "f"(v.x), "f"(v.y),
+                     "f"(v.z), "f"(v.w) : "memory");
+}
+
+__device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float v) {
+#pragma unroll
+    for (int e = 0; e < 7; ++e)
+        if (e < fan.n_peer) __stcs(fan.peer[e] + o, v);
+    if (fan.mc) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(fan.mc + o), "f"(v) : "memory");
+}
+
 // K x K kernels, K in {5, 7} (cspn2d_wide.cu); fan non-null: the fused gather
 size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
@@ -112,17 +138,19 @@ int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);
 size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters);
+// fan non-null: the fused gather (cspn3d_fwd_gather_f32), destinations addressed like out
 int generic3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W,
-                      int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+                      int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                      const Fan* fan = nullptr);
 
 size_t bwd3d_workspace_bytes(int C, int D, int H, int W, int iters);
 int bwd3d(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat, int B, int C,
           int D, int H, int W, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 
-// K x K x K kernels, K = 5 (cspn3d_wide.cu)
+// K x K x K kernels, K = 5 (cspn3d_wide.cu); fan non-null: the fused gather
 size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
 int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan = nullptr);
 size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters);
 int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
                      int D, int H, int W, int K, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream,
@@ -131,7 +159,7 @@ int widek3d_backward(const float* guidance, const float* feat, const float* grad
 size_t widek3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int iters);
 size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters);
 int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan = nullptr);
 int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,
                            int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
                            int* launches);

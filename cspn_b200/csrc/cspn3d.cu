@@ -8,6 +8,10 @@
 // L2/HBM.  Volumes are processed in groups (grid z carries the volume index): one step launch covers the whole
 // group, because a single volume's step is short enough that launch gaps and the grid's ramp / tail are a visible share;
 // the group is capped so that the 27*D*H*W-float workspace per volume stays below kMaxWorkspace3d.
+//
+// Fused gather (cspn3d_fwd_gather_f32, DESIGN.md section 4.6): the FAN flag of the step kernels stores each result also
+// to the same element of every peer GPU's gather buffer (NVLink stores) and / or to one NVLS multicast address
+// (multimem.st).  Only the last step, the one that writes `out`, runs it; the intermediate iterates never leave the GPU.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -54,9 +58,12 @@ prep3d_kernel(const float* __restrict__ g, float* __restrict__ wk, int D, int H,
     wk[26 * V + p] = (mode == 2) ? 0.f : 1.f - s;
 }
 
+// FAN (every step kernel below): the result also goes to fan's destinations (the last step of a fused gather); fan is
+// not read otherwise.
+template <bool FAN = false>
 __global__ void __launch_bounds__(256)
 step3d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-              float* __restrict__ dst, int C, int D, int H, int W) {
+              float* __restrict__ dst, int C, int D, int H, int W, const Fan fan) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int z = blockIdx.z % D, c = blockIdx.z / D;   // c = volume * C + channel
@@ -73,7 +80,9 @@ step3d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const 
                              ? __ldg(cc + (size_t)zz * HW + (size_t)yy * W + xx) : 0.f;
         acc = fmaf(__ldg(wk + k * V + p), dv, acc);
     }
-    dst[(size_t)c * V + p] = acc;
+    const size_t o = (size_t)c * V + p;
+    dst[o] = acc;
+    if constexpr (FAN) fan_store(fan, o, acc);
 }
 
 // Vectorised step for W % 4 == 0: one thread produces 4 consecutive voxels of a row.  The 27 weight planes stream
@@ -86,9 +95,10 @@ step3d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const 
 #else
 #define CSPN3D_BOUNDS __launch_bounds__(128)
 #endif
+template <bool FAN = false>
 __global__ void CSPN3D_BOUNDS
 step3d_vec4_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-                   float* __restrict__ dst, int C, int D, int H, int W) {
+                   float* __restrict__ dst, int C, int D, int H, int W, const Fan fan) {
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int z = blockIdx.z % D, c = blockIdx.z / D;   // c = volume * C + channel
@@ -129,7 +139,10 @@ step3d_vec4_kernel(const float* __restrict__ wk, const float* __restrict__ d0, c
         acc[2] = fmaf(w.z, r[o + 2], acc[2]);
         acc[3] = fmaf(w.w, r[o + 3], acc[3]);
     }
-    *reinterpret_cast<float4*>(dst + (size_t)c * V + p) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    const size_t o = (size_t)c * V + p;
+    const float4 v = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    *reinterpret_cast<float4*>(dst + o) = v;
+    if constexpr (FAN) fan_store(fan, o, v);
 }
 
 // 'paddle' normalisation straight from the RAW guidance (cspn_paddle/demo.py:24,47-52): the gate of tap k is
@@ -153,9 +166,10 @@ __device__ __forceinline__ float4 ld_stream(const float* p) {
 #ifndef CSPN3D_PADDLE_BLOCKS
 #define CSPN3D_PADDLE_BLOCKS 3
 #endif
+template <bool FAN = false>
 __global__ void __launch_bounds__(128, CSPN3D_PADDLE_BLOCKS)
 step3d_paddle_vec4_kernel(const float* __restrict__ g, const float* __restrict__ cur, float* __restrict__ dst, int C, int D, int H,
-                          int W) {
+                          int W, const Fan fan) {
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int z = blockIdx.z % D, c = blockIdx.z / D;   // c = volume * C + channel
@@ -197,8 +211,11 @@ step3d_paddle_vec4_kernel(const float* __restrict__ g, const float* __restrict__
         acc[2] = fmaf(a2, r[o + 2], acc[2]);
         acc[3] = fmaf(a3, r[o + 3], acc[3]);
     }
-    *reinterpret_cast<float4*>(dst + (size_t)c * V + p) =
+    const size_t o = (size_t)c * V + p;
+    const float4 v =
         make_float4(__fdiv_rn(acc[0], S[0]), __fdiv_rn(acc[1], S[1]), __fdiv_rn(acc[2], S[2]), __fdiv_rn(acc[3], S[3]));
+    *reinterpret_cast<float4*>(dst + o) = v;
+    if constexpr (FAN) fan_store(fan, o, v);
 }
 
 // '26sum' / '26sum_abs' (gathered affinities + centre term, the cspn.py-style generalisation) straight from the RAW guidance,
@@ -210,10 +227,10 @@ step3d_paddle_vec4_kernel(const float* __restrict__ g, const float* __restrict__
 #ifndef CSPN3D_GATHER_BLOCKS
 #define CSPN3D_GATHER_BLOCKS 3
 #endif
-template <bool ABS>
+template <bool ABS, bool FAN = false>
 __global__ void __launch_bounds__(128, CSPN3D_GATHER_BLOCKS)
 step3d_gather_vec4_kernel(const float* __restrict__ g, const float* __restrict__ d0, const float* __restrict__ cur,
-                          float* __restrict__ dst, int C, int D, int H, int W) {
+                          float* __restrict__ dst, int C, int D, int H, int W, const Fan fan) {
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int z = blockIdx.z % D, c = blockIdx.z / D;   // c = volume * C + channel
@@ -301,9 +318,33 @@ step3d_gather_vec4_kernel(const float* __restrict__ g, const float* __restrict__
         }
     }
     const float4 dz0 = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)c * V + p));
-    *reinterpret_cast<float4*>(dst + (size_t)c * V + p) =
-        make_float4(fmaf(1.f - s[0], dz0.x, acc[0]), fmaf(1.f - s[1], dz0.y, acc[1]), fmaf(1.f - s[2], dz0.z, acc[2]),
-                    fmaf(1.f - s[3], dz0.w, acc[3]));
+    const size_t o = (size_t)c * V + p;
+    const float4 v = make_float4(fmaf(1.f - s[0], dz0.x, acc[0]), fmaf(1.f - s[1], dz0.y, acc[1]),
+                                 fmaf(1.f - s[2], dz0.z, acc[2]), fmaf(1.f - s[3], dz0.w, acc[3]));
+    *reinterpret_cast<float4*>(dst + o) = v;
+    if constexpr (FAN) fan_store(fan, o, v);
+}
+
+// One step straight from the raw guidance (every volume in one launch); FAN: the last step of a fused gather
+template <bool FAN>
+void launch_raw_step(int mode, const float* g, const float* feat, const float* cur, float* dst, int nvol, int C, int D, int H,
+                     int W, cudaStream_t s, const Fan& fan) {
+    const dim3 grid((W / 4 + 31) / 32, (H + 3) / 4, D * C * nvol), block(32, 4);
+    if (mode == 2) step3d_paddle_vec4_kernel<FAN><<<grid, block, 0, s>>>(g, cur, dst, C, D, H, W, fan);
+    else if (mode == 1) step3d_gather_vec4_kernel<true, FAN><<<grid, block, 0, s>>>(g, feat, cur, dst, C, D, H, W, fan);
+    else step3d_gather_vec4_kernel<false, FAN><<<grid, block, 0, s>>>(g, feat, cur, dst, C, D, H, W, fan);
+}
+
+// One step on the weight planes of a volume group
+template <bool FAN>
+void launch_plane_step(bool vec4, const float* wk, const float* d0, const float* cur, float* dst, int nvol, int C, int D, int H,
+                       int W, cudaStream_t s, const Fan& fan) {
+    if (vec4)
+        step3d_vec4_kernel<FAN><<<dim3((W / 4 + 31) / 32, (H + 3) / 4, D * C * nvol), dim3(32, 4), 0, s>>>(wk, d0, cur, dst, C, D,
+                                                                                                         H, W, fan);
+    else
+        step3d_kernel<FAN><<<dim3((W + 31) / 32, (H + 7) / 8, D * C * nvol), dim3(32, 8), 0, s>>>(wk, d0, cur, dst, C, D, H, W,
+                                                                                                fan);
 }
 
 }  // namespace
@@ -330,8 +371,10 @@ size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
     return sizeof(float) * (size_t)group3d(B, C, D, H, W, iters, 27) * (27 * V + (iters > 1 ? (size_t)C * V : 0));
 }
 
+// fan (fused gather): destinations addressed like out, which the last step also writes; in the weight-plane route each
+// is offset to the volume group as `out` is.
 int generic3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W,
-                      int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+                      int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
     const size_t V = (size_t)D * H * W;
     if (iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * V * sizeof(float), cudaMemcpyDeviceToDevice,
@@ -357,11 +400,9 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
         float* tmp = static_cast<float*>(ws);
         const float* cur = feat;
         float* dst = (iters & 1) ? out : tmp;
-        const dim3 grid((W / 4 + 31) / 32, (H + 3) / 4, D * C * B), block(32, 4);
         for (int it = 0; it < iters; ++it) {
-            if (mode == 2) step3d_paddle_vec4_kernel<<<grid, block, 0, stream>>>(guidance, cur, dst, C, D, H, W);
-            else if (mode == 1) step3d_gather_vec4_kernel<true><<<grid, block, 0, stream>>>(guidance, feat, cur, dst, C, D, H, W);
-            else step3d_gather_vec4_kernel<false><<<grid, block, 0, stream>>>(guidance, feat, cur, dst, C, D, H, W);
+            if (fan && it == iters - 1) launch_raw_step<true>(mode, guidance, feat, cur, dst, B, C, D, H, W, stream, *fan);
+            else launch_raw_step<false>(mode, guidance, feat, cur, dst, B, C, D, H, W, stream, Fan{});
             ++*launches;
             cur = dst;
             dst = (dst == out) ? tmp : out;
@@ -385,10 +426,10 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
         const float* cur = d0;
         float* dst = (iters & 1) ? o : tmp;
         for (int it = 0; it < iters; ++it) {
-            if (vec4)
-                step3d_vec4_kernel<<<dim3((W / 4 + 31) / 32, (H + 3) / 4, D * C * n), dim3(32, 4), 0, stream>>>(wk, d0, cur, dst, C, D, H, W);
+            if (fan && it == iters - 1)
+                launch_plane_step<true>(vec4, wk, d0, cur, dst, n, C, D, H, W, stream, offset_fan(*fan, (size_t)b0 * C * V));
             else
-                step3d_kernel<<<dim3(g2.x, g2.y, D * C * n), block, 0, stream>>>(wk, d0, cur, dst, C, D, H, W);
+                launch_plane_step<false>(vec4, wk, d0, cur, dst, n, C, D, H, W, stream, Fan{});
             ++*launches;
             cur = dst;
             dst = (dst == o) ? tmp : o;
@@ -530,7 +571,7 @@ int bwd3d(const float* guidance, const float* feat, const float* grad_out, float
         ++*launches;
         for (int t = 0; t + 1 < iters; ++t) {
             step3d_kernel<<<dim3(g2.x, g2.y, D * C), block, 0, stream>>>(wk, d0, t == 0 ? d0 : Dt + (size_t)(t - 1) * n,
-                                                                         Dt + (size_t)t * n, C, D, H, W);
+                                                                         Dt + (size_t)t * n, C, D, H, W, Fan{});
             ++*launches;
         }
         const float* lam_in = grad_out + (size_t)b * n;

@@ -27,6 +27,9 @@
 // backward runs the staged form above on the gates themselves: the adjoint reads the volume's gates, the last adjoint writes
 // lambda_0 straight into grad_feat, and the K gather launches write Gw_k straight into grad_gates (no prep, no finalize).
 // K = 3 runs here on R = 1 instantiations; cspn3d.cu keeps the 3x3x3 operator.
+//
+// Fused gather (cspn3d_{k,gates}_fwd_gather_f32, DESIGN.md section 4.6): the FAN flag of the two step kernels, as in
+// cspn3d.cu: only the last step of a launch group stores to the other GPUs' gather buffers.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -106,13 +109,14 @@ prep3k_kernel(const float* __restrict__ g, float* __restrict__ wk, int D, int H,
 // and columns x0-4 .. x0+67 as float4 (the halo rounded up to 4 columns: a thread's window row is three aligned LDS.128).
 // PADDLE: w = raw guidance [vol][NT][V], out = sum_k |g_k| d_t(p+off_k) / sum_k |g_k|.  RAW: w = the caller's gates
 // [vol][NT][V], out = sum_k g_k d_t(p+off_k).  Otherwise w = weight planes [vol][NP][V], out = kappa d0 + sum_k w_k
-// d_t(p+off_k), or without the kappa term when d0 is null ('paddle' planes).
+// d_t(p+off_k), or without the kappa term when d0 is null ('paddle' planes).  FAN: the result also goes to fan's
+// destinations (the last step of a fused gather); fan is not read otherwise.
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R, bool PADDLE, bool RAW = false>
+template <int R, bool PADDLE, bool RAW = false, bool FAN = false>
 __global__ void __launch_bounds__(256)
 step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, const float* __restrict__ cur,
-                  float* __restrict__ dst, int C, int D, int H, int W) {
+                  float* __restrict__ dst, int C, int D, int H, int W, const Fan fan) {
     using T = Taps3<R>;
     constexpr int SZ = 2 * R + 1, SH = kVecTH + 2 * R, SQ = kVecTW / 4 + 2;
     __shared__ float4 tile[SZ][SH][SQ];
@@ -182,7 +186,10 @@ step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, con
             }
         }
     }
-    *reinterpret_cast<float4*>(dst + (size_t)bc * V + p) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    const size_t o = (size_t)bc * V + p;
+    const float4 v = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    *reinterpret_cast<float4*>(dst + o) = v;
+    if constexpr (FAN) fan_store(fan, o, v);
 }
 
 // ---- step / adjoint, one voxel per thread (any W, any alignment).  Tile 32 x 8 voxels of one z-plane + R halo ----
@@ -199,10 +206,10 @@ __device__ __forceinline__ void load_tile3_scalar(float (*tile)[kSclTH + 2 * R][
     }
 }
 
-template <int R, bool PADDLE, bool RAW = false>
+template <int R, bool PADDLE, bool RAW = false, bool FAN = false>
 __global__ void __launch_bounds__(256)
 step3k_scalar_kernel(const float* __restrict__ w, const float* __restrict__ d0, const float* __restrict__ cur,
-                     float* __restrict__ dst, int C, int D, int H, int W) {
+                     float* __restrict__ dst, int C, int D, int H, int W, const Fan fan) {
     using T = Taps3<R>;
     __shared__ float tile[2 * R + 1][kSclTH + 2 * R][kSclTW + 2 * R];
     const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH;
@@ -237,7 +244,9 @@ step3k_scalar_kernel(const float* __restrict__ w, const float* __restrict__ d0, 
             acc = __fdiv_rn(acc, S);
         }
     }
-    dst[(size_t)bc * V + p] = acc;
+    const size_t o = (size_t)bc * V + p;
+    dst[o] = acc;
+    if constexpr (FAN) fan_store(fan, o, acc);
 }
 
 // lambda_t(q) = sum_k w_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil over source voxels inside the volume.
@@ -377,26 +386,36 @@ fin3k_kernel(const float* __restrict__ g, const float* __restrict__ feat, const 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // RAW: w is the caller's gates (the step with PADDLE false and RAW true); otherwise `paddle` picks the PADDLE mode
-template <int R, bool RAW = false>
-void launch_step(bool vec, bool paddle, const float* w, const float* d0, const float* cur, float* dst, int nbc, int C, int D,
-                 int H, int W, cudaStream_t s) {
+template <int R, bool RAW, bool FAN>
+void launch_step_as(bool vec, bool paddle, const float* w, const float* d0, const float* cur, float* dst, int nbc, int C, int D,
+                    int H, int W, cudaStream_t s, const Fan& fan) {
     const unsigned gz = (unsigned)(D * nbc);
     if (vec) {
         const dim3 grid((W + kVecTW - 1) / kVecTW, (H + kVecTH - 1) / kVecTH, gz), block(16, 16);
-        if constexpr (RAW) step3k_vec_kernel<R, false, true><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W);
-        else if (paddle) step3k_vec_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
-        else step3k_vec_kernel<R, false><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
+        if constexpr (RAW) step3k_vec_kernel<R, false, true, FAN><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W, fan);
+        else if (paddle) step3k_vec_kernel<R, true, false, FAN><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W, fan);
+        else step3k_vec_kernel<R, false, false, FAN><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W, fan);
     } else {
         const dim3 grid((W + kSclTW - 1) / kSclTW, (H + kSclTH - 1) / kSclTH, gz), block(kSclTW, kSclTH);
-        if constexpr (RAW) step3k_scalar_kernel<R, false, true><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W);
-        else if (paddle) step3k_scalar_kernel<R, true><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
-        else step3k_scalar_kernel<R, false><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W);
+        if constexpr (RAW) step3k_scalar_kernel<R, false, true, FAN><<<grid, block, 0, s>>>(w, nullptr, cur, dst, C, D, H, W, fan);
+        else if (paddle) step3k_scalar_kernel<R, true, false, FAN><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W, fan);
+        else step3k_scalar_kernel<R, false, false, FAN><<<grid, block, 0, s>>>(w, d0, cur, dst, C, D, H, W, fan);
     }
 }
 
+// fan non-null: the FAN instantiation, which also stores the result to fan's destinations
+template <int R, bool RAW = false>
+void launch_step(bool vec, bool paddle, const float* w, const float* d0, const float* cur, float* dst, int nbc, int C, int D,
+                 int H, int W, cudaStream_t s, const Fan* fan = nullptr) {
+    if (fan) launch_step_as<R, RAW, true>(vec, paddle, w, d0, cur, dst, nbc, C, D, H, W, s, *fan);
+    else launch_step_as<R, RAW, false>(vec, paddle, w, d0, cur, dst, nbc, C, D, H, W, s, Fan{});
+}
+
+// fan (fused gather): destinations addressed like out, which the last step of every launch group also writes, each offset
+// to the group as `out` is
 template <int R>
 int forward_3k(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int iters, int mode,
-               void* ws, cudaStream_t stream, int* launches) {
+               void* ws, cudaStream_t stream, int* launches, const Fan* fan) {
     using T = Taps3<R>;
     const size_t V = (size_t)D * H * W, n = (size_t)C * V;
     const int G = group3d(B, C, D, H, W, iters, T::NP);
@@ -413,10 +432,12 @@ int forward_3k(const float* guidance, const float* feat, float* out, int B, int 
             prep3k_kernel<R><<<dim3((W + 31) / 32, (H + 7) / 8, D * nvol), dim3(32, 8), 0, stream>>>(g, wk, D, H, W, mode);
             ++*launches;
         }
+        const Fan gfan = fan ? offset_fan(*fan, (size_t)b0 * n) : Fan{};
         const float* cur = d0;
         float* dst = (iters & 1) ? o : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < iters; ++it) {
-            launch_step<R>(vec, paddle, paddle ? g : wk, paddle ? nullptr : d0, cur, dst, nvol * C, C, D, H, W, stream);
+            launch_step<R>(vec, paddle, paddle ? g : wk, paddle ? nullptr : d0, cur, dst, nvol * C, C, D, H, W, stream,
+                           fan && it == iters - 1 ? &gfan : nullptr);
             ++*launches;
             cur = dst;
             dst = (dst == o) ? tmp : o;
@@ -476,9 +497,10 @@ int gates_group(int B, int C, int D, int H, int W, int iters) {
     return (int)(gz < 1 ? 1 : (gz < B ? gz : B));
 }
 
+// fan: as in forward_3k
 template <int R>
 int forward_gates_3k(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int iters, void* ws,
-                     cudaStream_t stream, int* launches) {
+                     cudaStream_t stream, int* launches, const Fan* fan) {
     using T = Taps3<R>;
     const size_t V = (size_t)D * H * W, n = (size_t)C * V;
     const int G = gates_group(B, C, D, H, W, iters);
@@ -488,10 +510,12 @@ int forward_gates_3k(const float* gates, const float* feat, float* out, int B, i
         const int nvol = B - b0 < G ? B - b0 : G;
         const float* g = gates + (size_t)b0 * T::NT * V;
         float* o = out + (size_t)b0 * n;
+        const Fan gfan = fan ? offset_fan(*fan, (size_t)b0 * n) : Fan{};
         const float* cur = feat + (size_t)b0 * n;
         float* dst = (iters & 1) ? o : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < iters; ++it) {
-            launch_step<R, true>(vec, false, g, nullptr, cur, dst, nvol * C, C, D, H, W, stream);
+            launch_step<R, true>(vec, false, g, nullptr, cur, dst, nvol * C, C, D, H, W, stream,
+                                 fan && it == iters - 1 ? &gfan : nullptr);
             ++*launches;
             cur = dst;
             dst = (dst == o) ? tmp : o;
@@ -568,7 +592,7 @@ size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters)
 }
 
 int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
     if (iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * D * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
@@ -579,7 +603,7 @@ int widek3d_forward(const float* guidance, const float* feat, float* out, int B,
         return CSPN_ERR_WORKSPACE;
     }
     if (!grid_ok(C, D, H, "path", K)) return CSPN_ERR_UNSUPPORTED;
-    return forward_3k<2>(guidance, feat, out, B, C, D, H, W, iters, mode, ws, stream, launches);
+    return forward_3k<2>(guidance, feat, out, B, C, D, H, W, iters, mode, ws, stream, launches, fan);
 }
 
 int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
@@ -613,7 +637,7 @@ size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters) 
 }
 
 int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
     if (iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * D * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
@@ -624,8 +648,8 @@ int widek3d_gates_forward(const float* gates, const float* feat, float* out, int
         return CSPN_ERR_WORKSPACE;
     }
     if (!grid_ok(C, D, H, "gates path", K)) return CSPN_ERR_UNSUPPORTED;
-    return K == 3 ? forward_gates_3k<1>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches)
-                  : forward_gates_3k<2>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches);
+    return K == 3 ? forward_gates_3k<1>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches, fan)
+                  : forward_gates_3k<2>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches, fan);
 }
 
 int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,

@@ -2,7 +2,8 @@
 
 The reference's multi-GPU story is nn.DataParallel (eval.py:117): replicas compute their slice of the batch, then the
 outputs are gathered.  Images are independent, so there is no collective on the data path; the only exchange is that
-gather.  Three ways to do it, all ending with the full (world * B_local, C, H, W) output on every rank:
+gather.  Three ways to do it, all ending with the full (world * B_local, C, H, W) output, or (world * B_local, C, D, H, W)
+in 3D, on every rank:
 
   FusedGather (this file)   the kernel stores every finished result into the gather buffers of ALL GPUs: peer pointers
                             of a CUDA symmetric-memory allocation (plain NVLink stores) or, where the fabric offers it,
@@ -12,36 +13,40 @@ gather.  Three ways to do it, all ending with the full (world * B_local, C, H, W
                             hides behind the arithmetic.  `propagate_k` (K x K), `propagate_paddle` (the Paddle module's
                             own-location gates) and `affinity_propagate` (caller-supplied gates, 2D) run
                             `cspn2d_{k,paddle,gates}_fwd_gather_f32`: the last step kernel of the stepped forward stores
-                            to every destination; the intermediate steps stay local.
+                            to every destination; the intermediate steps stay local.  Built with D=..., the buffer holds
+                            volumes, and `propagate3d` (3x3x3), `propagate3d_k` (K x K x K) and `affinity_propagate3d`
+                            (caller-supplied gates, 3D) do the same through `cspn3d_{,k_,gates_}fwd_gather_f32`.
   ChunkedGather             no symmetric memory needed: the local batch is cut into chunks, the kernel of chunk i+1
-                            runs while NCCL all-gathers chunk i (`propagate`, 3x3, and `propagate_k`, K x K).
+                            runs while NCCL all-gathers chunk i (`propagate`, 3x3, and `propagate_k`, K x K; 2D only).
   sharding.gather_outputs   kernel, then one NCCL all_gather_into_tensor (what round 1 measured: the baseline).
 """
 import ctypes
+import math
 
 import torch
 import torch.distributed as dist
 
 from . import _lib
-from .cspn import (_check_gates, _check_inputs_2d_k, _check_inputs_2d_paddle, _ptr, norm_code_2d_k, propagate2d,
-                   propagate2d_k)
+from .cspn import (_check_gates, _check_inputs_2d_k, _check_inputs_2d_paddle, _check_shapes_3d_k, _per_channel_gate_views,
+                   _ptr, norm_code_2d_k, norm_code_3d_k, propagate2d, propagate2d_k)
 
 
 class FusedGather:
     """Owns the symmetric gather buffer of one problem shape.  Each method mirrors the module function of its name and
-    returns a view of that buffer holding all ranks' results, rank-major: out[r * B_local + i] is image i of rank r.
-    The input to propagate (blur_depth, feat or input) must have the (B_local, C, H, W) the buffer was built for."""
+    returns a view of that buffer holding all ranks' results, rank-major: out[r * B_local + i] is image (or volume) i of
+    rank r.  The input to propagate (blur_depth, feat or input) must have the (B_local, C, H, W) the buffer was built for,
+    or with D given, the (B_local, C, D, H, W) of the 3D methods."""
 
-    def __init__(self, B_local, C, H, W, device, group=None, multicast=True):
+    def __init__(self, B_local, C, H, W, device, group=None, multicast=True, *, D=None):
         import torch.distributed._symmetric_memory as symm_mem
         self.group = group if group is not None else dist.group.WORLD
         self.world = dist.get_world_size(self.group)
         self.rank = dist.get_rank(self.group)
         if self.world > 8:
             raise _lib.CspnError('FusedGather addresses at most 8 GPUs of one NVLink domain')
-        self.shape = (B_local, C, H, W)
-        self.block = B_local * C * H * W                  # floats per rank
-        self.buf = symm_mem.empty((self.world * B_local, C, H, W), dtype=torch.float32, device=device)
+        self.shape = (B_local, C, H, W) if D is None else (B_local, C, D, H, W)
+        self.block = math.prod(self.shape)                # floats per rank
+        self.buf = symm_mem.empty((self.world * B_local, *self.shape[1:]), dtype=torch.float32, device=device)
         self.hdl = symm_mem.rendezvous(self.buf, self.group)
         mine = self.rank * self.block * 4                 # byte offset of this rank's block inside every buffer
         ptrs = [int(p) for p in self.hdl.buffer_ptrs]
@@ -109,7 +114,7 @@ class FusedGather:
     def affinity_propagate(self, input, gate_weight, kernel_size=3, prop_step=1):
         """affinity_propagate in 2D; per-channel gates (B, (K*K-1)*C, H, W) included."""
         if input.dim() == 5:
-            raise ValueError('FusedGather.affinity_propagate is 2D only: the 3D gates forward has no fused gather')
+            raise ValueError('FusedGather.affinity_propagate is 2D only: 3D input goes to affinity_propagate3d')
         _, Bi, Ci = _check_gates(input, gate_weight, kernel_size, prop_step)
         self._check_shape(input)
         H, W = input.shape[2:]
@@ -117,6 +122,43 @@ class FusedGather:
         ws_bytes = _lib.lib().cspn2d_gates_workspace_bytes(Bi, Ci, H, W, kernel_size, int(prop_step))
         return self._gather('cspn2d_gates_fwd_gather_f32', x.device, [_ptr(g), _ptr(x)],
                             [Bi, Ci, H, W, kernel_size, int(prop_step)], ws_bytes)
+
+    def _volumes_3d_k(self, guidance, feat, prop_kernel):
+        """The checked inputs of a K x K x K call as the C ABI takes them: per-channel guidance (B, (K**3-1)*C, D, H, W)
+        becomes B*C single-channel volumes, as in Affinity_Propagate3DK."""
+        views = _per_channel_gate_views(guidance, feat, prop_kernel ** 3 - 1)
+        g, f = views if views is not None else (guidance.contiguous(), feat.contiguous())
+        _check_shapes_3d_k(g, f, prop_kernel)
+        self._check_shape(feat)
+        return g, f
+
+    def propagate3d(self, guidance, feat, prop_time=12, norm_type='26sum_abs'):
+        """propagate3d (3x3x3); per-channel guidance (B, 26*C, D, H, W) included, as Affinity_Propagate3D takes it."""
+        code = norm_code_3d_k(3, norm_type)
+        g, f = self._volumes_3d_k(guidance, feat, 3)
+        ws_bytes = _lib.lib().cspn3d_workspace_bytes(*f.shape, int(prop_time))
+        return self._gather('cspn3d_fwd_gather_f32', f.device, [_ptr(g), _ptr(f)], [*f.shape, int(prop_time), code],
+                            ws_bytes)
+
+    def propagate3d_k(self, guidance, feat, prop_kernel=5, prop_time=12, norm_type=None):
+        """propagate3d_k; per-channel guidance (B, (K**3-1)*C, D, H, W) included.  K = 3 is `propagate3d`."""
+        code = norm_code_3d_k(prop_kernel, norm_type)
+        g, f = self._volumes_3d_k(guidance, feat, prop_kernel)
+        ws_bytes = _lib.lib().cspn3d_k_workspace_bytes(*f.shape, prop_kernel, int(prop_time))
+        return self._gather('cspn3d_k_fwd_gather_f32', f.device, [_ptr(g), _ptr(f)],
+                            [*f.shape, prop_kernel, int(prop_time), code], ws_bytes)
+
+    def affinity_propagate3d(self, input, gate_weight, kernel_size=3, prop_step=1):
+        """affinity_propagate in 3D; per-channel gates (B, (K**3-1)*C, D, H, W) included."""
+        if input.dim() != 5:
+            raise ValueError('FusedGather.affinity_propagate3d is 3D only: 2D input goes to affinity_propagate')
+        _, Bi, Ci = _check_gates(input, gate_weight, kernel_size, prop_step)
+        self._check_shape(input)
+        D, H, W = input.shape[2:]
+        g, x = gate_weight.contiguous(), input.contiguous()
+        ws_bytes = _lib.lib().cspn3d_gates_workspace_bytes(Bi, Ci, D, H, W, kernel_size, int(prop_step))
+        return self._gather('cspn3d_gates_fwd_gather_f32', x.device, [_ptr(g), _ptr(x)],
+                            [Bi, Ci, D, H, W, kernel_size, int(prop_step)], ws_bytes)
 
 
 class ChunkedGather:

@@ -195,6 +195,22 @@ CSPN_API int cspn3d_fwd_f32(const float* guidance, const float* feat, float* out
                    int B, int C, int D, int H, int W, int iters, int norm_type,
                    void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- fused gather of the 3D forwards -------------------------------------------------------------------------------
+ * cspn3d_fwd_gather_f32, cspn3d_k_fwd_gather_f32 and cspn3d_gates_fwd_gather_f32 take the arguments of their plain forward
+ * plus peer_out / n_peer / multicast_out after `out`, exactly as the 2D gathers do (see cspn2d_k_fwd_gather_f32), and give
+ * `out` its bits.  The last step of the forward also stores its result to each peer_out[i] (the same [B][C][D][H][W]
+ * block inside another GPU's gather buffer) and / or to multicast_out; intermediate steps stay local.  Same checks and
+ * codes as in 2D: n_peer 0..7 with a non-null array when non-zero, every peer_out[i] non-null, every peer_out[i] and
+ * multicast_out (may be NULL) 16-byte aligned, else CSPN_ERR_INVALID_ARGUMENT; iters == 0 is CSPN_ERR_UNSUPPORTED.
+ * Workspace as for the plain forward (its *_workspace_bytes), and cspn_last_launches() counts the same launches.
+ * K = 3 in cspn3d_k_fwd_gather_f32 delegates to cspn3d_fwd_gather_f32; every entry takes any W.  Per-channel gates are
+ * B*C volumes with C = 1, as in the plain calls: the output memory, and with it the peer offsets, is the same.  The
+ * caller orders the remote stores before their consumers (a barrier across ranks after the call). */
+CSPN_API int cspn3d_fwd_gather_f32(const float* guidance, const float* feat, float* out,
+                          float* const* peer_out, int n_peer, float* multicast_out,
+                          int B, int C, int D, int H, int W, int iters, int norm_type,
+                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 CSPN_API int cspn3d_fwd_f32_host(const float* guidance, const float* feat, float* out,
                         int B, int C, int D, int H, int W, int iters, int norm_type, int device);
 
@@ -223,6 +239,12 @@ CSPN_API size_t cspn3d_k_workspace_bytes(int B, int C, int D, int H, int W, int 
 CSPN_API int cspn3d_k_fwd_f32(const float* guidance, const float* feat, float* out,
                      int B, int C, int D, int H, int W, int K, int iters, int norm_type,
                      void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+/* cspn3d_k_fwd_f32 fused with the final gather of a data-parallel run: see cspn3d_fwd_gather_f32 */
+CSPN_API int cspn3d_k_fwd_gather_f32(const float* guidance, const float* feat, float* out,
+                            float* const* peer_out, int n_peer, float* multicast_out,
+                            int B, int C, int D, int H, int W, int K, int iters, int norm_type,
+                            void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
 CSPN_API size_t cspn3d_k_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
 
@@ -256,7 +278,7 @@ CSPN_API int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* 
                          int B, int C, int H, int W, int K, int iters,
                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
-/* cspn2d_gates_fwd_f32 fused with the final gather of a data-parallel run: see cspn2d_k_fwd_gather_f32 (2D only) */
+/* cspn2d_gates_fwd_f32 fused with the final gather of a data-parallel run: see cspn2d_k_fwd_gather_f32 */
 CSPN_API int cspn2d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out,
                                 float* const* peer_out, int n_peer, float* multicast_out,
                                 int B, int C, int H, int W, int K, int iters,
@@ -273,6 +295,12 @@ CSPN_API size_t cspn3d_gates_workspace_bytes(int B, int C, int D, int H, int W, 
 CSPN_API int cspn3d_gates_fwd_f32(const float* gates, const float* feat, float* out,
                          int B, int C, int D, int H, int W, int K, int iters,
                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+/* cspn3d_gates_fwd_f32 fused with the final gather of a data-parallel run: see cspn3d_fwd_gather_f32 */
+CSPN_API int cspn3d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out,
+                                float* const* peer_out, int n_peer, float* multicast_out,
+                                int B, int C, int D, int H, int W, int K, int iters,
+                                void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
 CSPN_API size_t cspn3d_gates_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
 
