@@ -57,6 +57,9 @@ SIGNATURES = {
     'cspn_depth_metrics_workspace_bytes': (_sz, []),
     'cspn_depth_metrics_f32': (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     'cspn_masked_l1_bwd_f32': (_i, [_vp] * 5 + [_sz, _vp]),
+    'cspn_unpool_conv3x3_fwd_f32': (_i, [_vp] * 3 + [_i] * 7 + [_vp]),
+    'cspn_unpool_conv3x3_bwd_workspace_bytes': (_sz, [_i] * 7),
+    'cspn_unpool_conv3x3_bwd_f32': (_i, [_vp] * 5 + [_i] * 7 + [_vp, _sz, _vp]),
     'cspn_host_alloc': (_vp, [_sz]),
     'cspn_host_free': (None, [_vp]),
     'cspn_last_error': (_cp, []),

@@ -723,3 +723,104 @@ def affinity_propagate(input, gate_weight, kernel_size=3, prop_step=1):
     if torch.is_grad_enabled() and (input.requires_grad or gate_weight.requires_grad):
         return _AffinityPropagateFn.apply(input, gate_weight, kernel_size, prop_step)
     return _affinity_propagate_fwd(input, gate_weight, kernel_size, prop_step)
+
+
+# ---- the guidance and depth heads: Unpool + crop + 3x3 convolution (torch_resnet_cspn_nyu.py:41-54, 187-205) ----------
+def unpool_output_size(h, w, oheight=0, owidth=0):
+    """The head's output size: the crop (oheight, owidth) when both are non-zero, else the whole unpooled map (2h, 2w)
+    (Simple_Gudi_UpConv_Block_Last_Layer._up_pooling, torch_resnet_cspn_nyu.py:195-200)."""
+    return (oheight, owidth) if oheight != 0 and owidth != 0 else (2 * h, 2 * w)
+
+
+def _check_unpool_conv(x, weight, H, W):
+    if x.dim() != 4 or weight.dim() != 4 or weight.shape[1] != x.shape[1] or tuple(weight.shape[2:]) != (3, 3):
+        raise ValueError(f'x must be (B,Cin,h,w) and weight (Cout,Cin,3,3), got {tuple(x.shape)} and {tuple(weight.shape)}')
+    if not (1 <= H <= 2 * x.shape[2] and 1 <= W <= 2 * x.shape[3]):
+        raise ValueError(f'output {H}x{W} must be at least 1x1 and within the unpooled map {2 * x.shape[2]}x{2 * x.shape[3]}')
+    if x.dtype != torch.float32 or weight.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if x.device != weight.device:
+        raise RuntimeError('x and weight are on different devices')
+    if not x.is_cuda:
+        raise _lib.CspnError('unpool_conv3x3 takes CUDA tensors only (there is no host-buffer entry point for it)')
+
+
+def _unpool_conv_fwd(x, weight, H, W):
+    """Forward only (no autograd) through cspn_unpool_conv3x3_fwd_f32, enqueued on the current stream."""
+    L = _lib.lib()
+    xc, wc = x.contiguous(), weight.contiguous()
+    out = xc.new_empty((xc.shape[0], wc.shape[0], H, W))
+    with torch.cuda.device(xc.device):
+        rc = L.cspn_unpool_conv3x3_fwd_f32(_ptr(xc), _ptr(wc), _ptr(out), *xc.shape, wc.shape[0], H, W, _stream(xc.device))
+    _lib.check(rc, 'cspn_unpool_conv3x3_fwd_f32')
+    return out
+
+
+class _UnpoolConv3x3Fn(torch.autograd.Function):
+    """autograd seam of unpool_conv3x3 without the torch-op shim: native forward + native backward
+    (cspn_unpool_conv3x3_bwd_f32)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, H, W):
+        ctx.save_for_backward(x, weight)
+        ctx.cfg = (H, W)
+        return _unpool_conv_fwd(x, weight, H, W)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        x, weight = ctx.saved_tensors
+        H, W = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        xc, wc, go = x.contiguous(), weight.contiguous(), grad_out.contiguous()
+        gx = torch.empty_like(xc) if ctx.needs_input_grad[0] else None
+        gw = torch.empty_like(wc) if ctx.needs_input_grad[1] else None
+        if gx is None and gw is None:
+            return None, None, None, None
+        shape = (*xc.shape, wc.shape[0], H, W)
+        with torch.cuda.device(xc.device):
+            ws_bytes = L.cspn_unpool_conv3x3_bwd_workspace_bytes(*shape) if gw is not None else 0
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=xc.device) if ws_bytes else None
+            rc = L.cspn_unpool_conv3x3_bwd_f32(_ptr(xc), _ptr(wc), _ptr(go), _ptr(gx), _ptr(gw), *shape, _ptr(ws), ws_bytes,
+                                               _stream(xc.device))
+        _lib.check(rc, 'cspn_unpool_conv3x3_bwd_f32')
+        return gx, gw, None, None
+
+
+def unpool_conv3x3(x, weight, oheight=0, owidth=0):
+    """The reference head's forward in one CUDA kernel: Unpool(x) (a [1,0;0,0] conv_transpose2d, stride 2), cropped to
+    (oheight, owidth) when both are non-zero, then a 3x3 convolution with zero padding and no bias:
+        out(co, p) = sum_ci sum_tap weight[co, ci, ky, kx] * u(ci, p + (ky-1, kx-1)),  u(2i, 2j) = x(i, j), else x(i, j) * 0.
+    x (B, Cin, h, w), weight (Cout, Cin, 3, 3) -> (B, Cout, H, W).  Only the 9 of 36 products per input channel that read a
+    real cell are computed; the NaN a non-finite x or weight gives through the skipped ones is put back (DESIGN.md section
+    4.12).  Differentiable in x and weight; fp32 CUDA tensors only."""
+    if x.dim() != 4:
+        raise ValueError(f'x must be (B,Cin,h,w), got {tuple(x.shape)}')
+    H, W = unpool_output_size(x.shape[2], x.shape[3], oheight, owidth)
+    _check_unpool_conv(x, weight, H, W)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.unpool_conv3x3(x, weight, H, W)
+    if torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad):
+        return _UnpoolConv3x3Fn.apply(x, weight, H, W)
+    return _unpool_conv_fwd(x, weight, H, W)
+
+
+class Simple_Gudi_UpConv_Block_Last_Layer(nn.Module):
+    """Drop-in for the reference's guidance / depth head (torch_resnet_cspn_nyu.py:187-205): the same constructor, the same
+    conv1 = nn.Conv2d(in_channels, out_channels, 3, 1, 1, bias=False) built first (a seeded construction draws the same
+    weights, and state_dict() holds conv1.weight only), and a forward that runs Unpool, crop and conv1 as one CUDA kernel,
+    unpool_conv3x3(x, conv1.weight, oheight, owidth)."""
+
+    def __init__(self, in_channels, out_channels, oheight=0, owidth=0):
+        super().__init__()
+        self.conv1 = nn.Conv2d(in_channels, out_channels, kernel_size=3, stride=1, padding=1, bias=False)
+        self.oheight = oheight
+        self.owidth = owidth
+
+    def forward(self, x):
+        return unpool_conv3x3(x, self.conv1.weight, self.oheight, self.owidth)
+
+    def extra_repr(self):
+        return f'oheight={self.oheight}, owidth={self.owidth}'

@@ -627,6 +627,70 @@ int cspn3d_gates_bwd_f32(const float* gates, const float* feat, const float* gra
     return rc;
 }
 
+// ---- unpool + crop + 3x3 convolution (the guidance and depth heads) ---------------------------------------------------
+static int check_unpool_conv(const void* x, const void* weight, const void* out, int B, int Cin, int h, int w, int Cout, int H,
+                             int W) {
+    if (!x || !weight || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (B <= 0 || Cin <= 0 || h <= 0 || w <= 0 || Cout <= 0 || H <= 0 || W <= 0) {
+        set_error("non-positive size B=%d Cin=%d h=%d w=%d Cout=%d H=%d W=%d", B, Cin, h, w, Cout, H, W);
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (H > 2 * h || W > 2 * w) { set_error("output %dx%d exceeds the unpooled map %dx%d", H, W, 2 * h, 2 * w); return CSPN_ERR_INVALID_ARGUMENT; }
+    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight) | reinterpret_cast<uintptr_t>(out)) & 3) {
+        set_error("tensor pointers must be 4-byte aligned");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    const char* why = "";
+    if (!unpool_conv_launchable(B, Cin, Cout, &why)) { set_error("the launch grid cannot take this shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+int cspn_unpool_conv3x3_fwd_f32(const float* x, const float* weight, float* out, int B, int Cin, int h, int w, int Cout, int H,
+                                int W, cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_unpool_conv(x, weight, out, B, Cin, h, w, Cout, H, W);
+    if (rc != CSPN_OK) return rc;
+    DeviceGuard guard(device_of(x));
+    if (!guard.ok) { set_error("cannot select the device of `x`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = unpool_conv_forward(x, weight, out, B, Cin, h, w, Cout, H, W, (cudaStream_t)stream, &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+size_t cspn_unpool_conv3x3_bwd_workspace_bytes(int B, int Cin, int h, int w, int Cout, int H, int W) {
+    if (B <= 0 || Cin <= 0 || h <= 0 || w <= 0 || Cout <= 0 || H <= 0 || W <= 0 || H > 2 * h || W > 2 * w) return 0;
+    return unpool_conv_bwd_workspace_bytes(B, Cin, H, W, Cout);
+}
+
+int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, const float* grad_out, float* grad_x, float* grad_weight,
+                                int B, int Cin, int h, int w, int Cout, int H, int W, void* workspace, size_t workspace_bytes,
+                                cspn_stream_t stream) {
+    clear_error();
+    g_last_launches = 0;
+    int rc = check_unpool_conv(x, weight, grad_out, B, Cin, h, w, Cout, H, W);
+    if (rc != CSPN_OK) return rc;
+    if ((reinterpret_cast<uintptr_t>(grad_x) | reinterpret_cast<uintptr_t>(grad_weight)) & 3) {
+        set_error("gradient pointers must be 4-byte aligned");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (grad_weight) {
+        const size_t need = unpool_conv_bwd_workspace_bytes(B, Cin, H, W, Cout);
+        if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 3)) {
+            set_error("grad_weight needs %zu bytes of 4-byte aligned workspace (got %zu)", need, workspace_bytes);
+            return CSPN_ERR_WORKSPACE;
+        }
+    }
+    DeviceGuard guard(device_of(x));
+    if (!guard.ok) { set_error("cannot select the device of `x`"); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    rc = unpool_conv_backward(x, weight, grad_out, grad_x, grad_weight, B, Cin, h, w, Cout, H, W, workspace, (cudaStream_t)stream,
+                              &launches);
+    g_last_launches = launches;
+    return rc;
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

@@ -164,4 +164,12 @@ int widek3d_gates_backward(const float* gates, const float* feat, const float* g
                            int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
                            int* launches);
 
+// Unpool + crop + 3x3 convolution of the guidance / depth heads (unpool_conv.cu); shapes checked by the caller
+int unpool_conv_launchable(int B, int Cin, int Cout, const char** why);
+size_t unpool_conv_bwd_workspace_bytes(int B, int Cin, int H, int W, int Cout);
+int unpool_conv_forward(const float* x, const float* w, float* out, int B, int Cin, int h, int wd, int Cout, int H, int W,
+                        cudaStream_t st, int* launches);
+int unpool_conv_backward(const float* x, const float* w, const float* g, float* gx, float* gw, int B, int Cin, int h, int wd,
+                         int Cout, int H, int W, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

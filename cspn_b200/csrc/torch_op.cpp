@@ -31,6 +31,10 @@
 //   affinity_propagate2d_backward(Tensor input, Tensor gate_weight, Tensor grad_out, int kernel_size, int prop_step,
 //                                 bool need_input, bool need_gate) -> (Tensor, Tensor)
 //   affinity_propagate3d / affinity_propagate3d_backward: the same for (B, C, D, H, W), K in {3, 5}
+//   unpool_conv3x3(Tensor x, Tensor weight, int H, int W) -> Tensor
+//       (the guidance / depth head: Unpool, crop to H x W, 3x3 convolution; x (B, Cin, h, w), weight (Cout, Cin, 3, 3))
+//   unpool_conv3x3_backward(Tensor x, Tensor weight, Tensor grad_out, int H, int W, bool need_x, bool need_weight)
+//       -> (Tensor, Tensor)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -419,6 +423,52 @@ std::tuple<at::Tensor, at::Tensor> affinity_propagate3d_backward_cuda(const at::
     return affinity_propagate_backward_cuda(input, gate, grad_out, K, prop_step, need_x, need_g, 3);
 }
 
+// Unpool + crop + 3x3 convolution of the guidance / depth heads: x (B, Cin, h, w), weight (Cout, Cin, 3, 3), out (B, Cout, H, W)
+void check_unpool_conv(const at::Tensor& x, const at::Tensor& weight, int64_t H, int64_t W) {
+    TORCH_CHECK_VALUE(x.dim() == 4 && weight.dim() == 4 && weight.size(1) == x.size(1) && weight.size(2) == 3 && weight.size(3) == 3,
+                      "x must be (B,Cin,h,w) and weight (Cout,Cin,3,3), got ", x.sizes(), " and ", weight.sizes());
+    TORCH_CHECK_VALUE(H >= 1 && W >= 1 && H <= 2 * x.size(2) && W <= 2 * x.size(3), "output ", H, "x", W,
+                      " must be at least 1x1 and within the unpooled map ", 2 * x.size(2), "x", 2 * x.size(3));
+    TORCH_CHECK(x.scalar_type() == at::kFloat && weight.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(x.device() == weight.device(), "x and weight are on different devices");
+}
+
+at::Tensor unpool_conv3x3_cuda(const at::Tensor& x, const at::Tensor& weight, int64_t H, int64_t W) {
+    check_unpool_conv(x, weight, H, W);
+    const c10::cuda::CUDAGuard guard(x.device());
+    const at::Tensor xc = x.contiguous(), wc = weight.contiguous();
+    at::Tensor out = at::empty({xc.size(0), wc.size(0), H, W}, xc.options());
+    check_rc(cspn_unpool_conv3x3_fwd_f32(fptr(xc), fptr(wc), out.data_ptr<float>(), (int)xc.size(0), (int)xc.size(1), (int)xc.size(2),
+                                         (int)xc.size(3), (int)wc.size(0), (int)H, (int)W,
+                                         (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+             "cspn_unpool_conv3x3_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> unpool_conv3x3_backward_cuda(const at::Tensor& x, const at::Tensor& weight,
+                                                                const at::Tensor& grad_out, int64_t H, int64_t W, bool need_x,
+                                                                bool need_w) {
+    check_unpool_conv(x, weight, H, W);
+    TORCH_CHECK(grad_out.dim() == 4 && grad_out.size(0) == x.size(0) && grad_out.size(1) == weight.size(0) && grad_out.size(2) == H &&
+                    grad_out.size(3) == W && grad_out.scalar_type() == at::kFloat && grad_out.device() == x.device(),
+                "grad_out must be (B,Cout,H,W) fp32 on the device of x, got ", grad_out.sizes());
+    const c10::cuda::CUDAGuard guard(x.device());
+    const at::Tensor xc = x.contiguous(), wc = weight.contiguous(), go = grad_out.contiguous();
+    at::Tensor gx = need_x ? at::empty_like(xc) : at::Tensor();
+    at::Tensor gw = need_w ? at::empty_like(wc) : at::Tensor();
+    const int B = (int)xc.size(0), Cin = (int)xc.size(1), h = (int)xc.size(2), w = (int)xc.size(3), Cout = (int)wc.size(0);
+    const size_t ws_bytes = need_w ? cspn_unpool_conv3x3_bwd_workspace_bytes(B, Cin, h, w, Cout, (int)H, (int)W) : 0;
+    at::Tensor ws;
+    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, xc.options().dtype(at::kByte));
+    if (need_x || need_w)
+        check_rc(cspn_unpool_conv3x3_bwd_f32(fptr(xc), fptr(wc), fptr(go), need_x ? gx.data_ptr<float>() : nullptr,
+                                             need_w ? gw.data_ptr<float>() : nullptr, B, Cin, h, w, Cout, (int)H, (int)W,
+                                             ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
+                                             (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+                 "cspn_unpool_conv3x3_bwd_f32");
+    return {need_x ? gx : at::zeros({0}, xc.options()), need_w ? gw : at::zeros({0}, wc.options())};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -444,6 +494,9 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("affinity_propagate3d(Tensor input, Tensor gate_weight, int kernel_size, int prop_step) -> Tensor");
     m.def("affinity_propagate3d_backward(Tensor input, Tensor gate_weight, Tensor grad_out, int kernel_size, int prop_step, "
           "bool need_input, bool need_gate) -> (Tensor, Tensor)");
+    m.def("unpool_conv3x3(Tensor x, Tensor weight, int H, int W) -> Tensor");
+    m.def("unpool_conv3x3_backward(Tensor x, Tensor weight, Tensor grad_out, int H, int W, bool need_x, bool need_weight) "
+          "-> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -461,4 +514,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("affinity_propagate2d_backward", &affinity_propagate2d_backward_cuda);
     m.impl("affinity_propagate3d", &affinity_propagate3d_cuda);
     m.impl("affinity_propagate3d_backward", &affinity_propagate3d_backward_cuda);
+    m.impl("unpool_conv3x3", &unpool_conv3x3_cuda);
+    m.impl("unpool_conv3x3_backward", &unpool_conv3x3_backward_cuda);
 }

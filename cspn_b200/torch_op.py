@@ -187,6 +187,33 @@ def _register():
     for nd in (2, 3):
         _register_gates(lib, nd)
 
+    @lib.register_fake('cspn_b200::unpool_conv3x3')
+    def _(x, weight, H, W):
+        torch._check(x.dim() == 4 and weight.dim() == 4 and weight.shape[1] == x.shape[1] and tuple(weight.shape[2:]) == (3, 3),
+                     lambda: 'x must be (B,Cin,h,w) and weight (Cout,Cin,3,3)')
+        torch._check(1 <= H <= 2 * x.shape[2] and 1 <= W <= 2 * x.shape[3], lambda: 'the output must lie within the unpooled map')
+        return x.new_empty((x.shape[0], weight.shape[0], H, W))
+
+    @lib.register_fake('cspn_b200::unpool_conv3x3_backward')
+    def _(x, weight, grad_out, H, W, need_x, need_weight):
+        gx = torch.empty_like(x, memory_format=torch.contiguous_format) if need_x else x.new_empty(0)
+        gw = torch.empty_like(weight, memory_format=torch.contiguous_format) if need_weight else weight.new_empty(0)
+        return gx, gw
+
+    def setup_unpool(ctx, inputs, output):
+        x, weight, H, W = inputs
+        ctx.save_for_backward(x, weight)
+        ctx.cfg = (H, W)
+
+    def backward_unpool(ctx, grad_out):
+        x, weight = ctx.saved_tensors
+        H, W = ctx.cfg
+        need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        gx, gw = torch.ops.cspn_b200.unpool_conv3x3_backward(x, weight, grad_out.contiguous(), H, W, need_x, need_w)
+        return (gx if need_x else None), (gw if need_w else None), None, None
+
+    lib.register_autograd('cspn_b200::unpool_conv3x3', backward_unpool, setup_context=setup_unpool)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

@@ -308,6 +308,34 @@ CSPN_API int cspn3d_gates_bwd_f32(const float* gates, const float* feat, const f
                          float* grad_gates, float* grad_feat, int B, int C, int D, int H, int W, int K, int iters,
                          void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- the guidance and depth heads: Unpool + crop + 3x3 convolution in one kernel -----------------------------------
+ * Simple_Gudi_UpConv_Block_Last_Layer (torch_resnet_cspn_nyu.py:187-205): u = Unpool(x) (conv_transpose2d with a [1,0;0,0]
+ * kernel, stride 2, groups=Cin: u(2i, 2j) = x(i, j), the other three cells of each 2x2 block x(i, j) * 0), cropped to
+ * H x W, then out = conv2d(u, weight, padding=1, no bias):
+ *   out(co, p) = sum_ci sum_tap weight[co][ci][ky][kx] * u(ci, p + (ky-1, kx-1)),  zero padding.
+ * x [B][Cin][h][w], weight [Cout][Cin][3][3], out / grad_out [B][Cout][H][W] with 1 <= H <= 2h, 1 <= W <= 2w; grad_x has
+ * the shape of x and grad_weight that of weight.  Any Cin, Cout >= 1; every pointer 4-byte aligned.
+ * IEEE as the op sequence: the products with the structural zeros (inserted cells, padding) are skipped, and the forward
+ * puts back the NaN they give for a non-finite x or weight.  The backward is exact for finite inputs only: gradients flow
+ * through the real cells, so a non-finite value is not spread by a product with a structural zero.
+ * Every sum has a fixed order: the forward and grad_x bits of an image do not depend on the rest of the batch, and
+ * grad_weight is the same from run to run (per-CTA partials in the workspace, summed in order by a second kernel).
+ * The forward launches one kernel and needs no workspace.  The backward launches one kernel for grad_x and two for
+ * grad_weight; either gradient may be NULL and its kernels are then skipped.  The workspace (4-byte aligned) is needed only
+ * with grad_weight, cspn_unpool_conv3x3_bwd_workspace_bytes() bytes, which depends on the shape alone (0 for an invalid one).
+ * No allocation, no synchronisation; cspn_last_launches() reports the kernels launched.
+ * CSPN_ERR_INVALID_ARGUMENT for a non-positive size, H > 2h or W > 2w, a null x / weight / out (grad_out in the backward)
+ * or a misaligned pointer; CSPN_ERR_WORKSPACE for a missing or short workspace; CSPN_ERR_UNSUPPORTED for a shape the launch
+ * grid cannot take (B > 65535). */
+CSPN_API int cspn_unpool_conv3x3_fwd_f32(const float* x, const float* weight, float* out, int B, int Cin, int h, int w,
+                                int Cout, int H, int W, cspn_stream_t stream);
+
+CSPN_API size_t cspn_unpool_conv3x3_bwd_workspace_bytes(int B, int Cin, int h, int w, int Cout, int H, int W);
+
+CSPN_API int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, const float* grad_out, float* grad_x,
+                                float* grad_weight, int B, int Cin, int h, int w, int Cout, int H, int W,
+                                void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
