@@ -40,13 +40,33 @@ int device_of(const void* p) {
     return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
 }
 
-int check2d(const float* guidance, const float* blur, float* out, int B, int C, int H, int W, int gch, int iters,
-            int norm_type, int algo) {
-    if (!guidance || !blur || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (gch < 8) { set_error("guidance needs >= 8 channels, got %d (cspn.py:91-98)", gch); return CSPN_ERR_INVALID_ARGUMENT; }
+bool kernel_size_ok(int nd, int K) { return K == 3 || K == 5 || (nd == 2 && K == 7); }
+
+template <class... Ints>
+bool positive(Ints... v) { return ((v > 0) && ...); }
+
+// The argument check of every propagation entry: nd = 2 (D is 1; K in {3, 5, 7}; norm_type '8sum' / '8sum_abs') or 3 (K in
+// {3, 5}; norm_type up to 'paddle').  a, b, c are the entry's three mandatory tensors.  An entry without a kernel size
+// passes K = 3, one without a norm_type passes 0, and gch is the 2D guidance's channel count (K*K-1 where the shape implies it).
+int check_prop(int nd, const void* a, const void* b, const void* c, int B, int C, int D, int H, int W, int K, int gch, int iters,
+               int norm_type) {
+    if (!a || !b || !c) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!positive(B, C, D, H, W)) {
+        if (nd == 2) set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W);
+        else set_error("non-positive shape B=%d C=%d D=%d H=%d W=%d", B, C, D, H, W);
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (!kernel_size_ok(nd, K)) { set_error("%dD kernel size must be %s, got %d", nd, nd == 2 ? "3, 5 or 7" : "3 or 5", K); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (nd == 2 && gch < K * K - 1) { set_error("a %dx%d kernel needs >= %d guidance channels, got %d", K, K, K * K - 1, gch); return CSPN_ERR_INVALID_ARGUMENT; }
     if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (norm_type != CSPN_NORM_8SUM && norm_type != CSPN_NORM_8SUM_ABS) { set_error("unknown norm_type %d (cspn.py:36)", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (norm_type < 0 || norm_type > (nd == 2 ? (int)CSPN_NORM_8SUM_ABS : (int)CSPN_NORM_PADDLE)) {
+        set_error("unknown %snorm_type %d", nd == 2 ? "" : "3D ", norm_type);
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    return CSPN_OK;
+}
+
+int check_algo(int algo) {
     if (algo < CSPN_ALGO_AUTO || algo > CSPN_ALGO_CLUSTER) { set_error("unknown algo %d", algo); return CSPN_ERR_INVALID_ARGUMENT; }
     return CSPN_OK;
 }
@@ -67,6 +87,43 @@ Fan make_fan(float* const* peer_out, int n_peer, float* multicast_out) {
     f.n_peer = n_peer;
     f.mc = multicast_out;
     return f;
+}
+
+// The destinations of a fused gather as the C ABI takes them
+struct Gather {
+    float* const* peer_out;
+    int n_peer;
+    float* multicast_out;
+};
+
+void begin_call() {
+    clear_error();
+    g_last_launches = 0;
+}
+
+// What every device entry does once its arguments are checked (the checks come first: they must not need a device):
+// select the device that holds `anchor`, the tensor the entry calls `name`, run launch(&launches), publish the count.
+template <class Launch>
+int on_device_of(const void* anchor, const char* name, Launch&& launch) {
+    DeviceGuard guard(device_of(anchor));
+    if (!guard.ok) { set_error("cannot select the device of `%s`", name); return CSPN_ERR_CUDA; }
+    int launches = 0;
+    const int rc = launch(&launches);
+    g_last_launches = launches;
+    return rc;
+}
+
+// A forward entry and its _gather twin: launch(fan, &launches) with fan null for the plain forward (gather null),
+// else the checked destinations
+template <class Launch>
+int run_forward(const void* anchor, const char* name, const Gather* gather, int iters, Launch&& launch) {
+    Fan fan{};
+    if (gather) {
+        const int rc = check_gather(gather->peer_out, gather->n_peer, gather->multicast_out, iters);
+        if (rc != CSPN_OK) return rc;
+        fan = make_fan(gather->peer_out, gather->n_peer, gather->multicast_out);
+    }
+    return on_device_of(anchor, name, [&](int* launches) { return launch(gather ? &fan : nullptr, launches); });
 }
 
 // Picks the algorithm actually run for `algo` on this problem.  AUTO prefers the cluster kernel.
@@ -101,8 +158,11 @@ void cspn_host_free(void* p) {
     if (p) cudaFreeHost(p);
 }
 
+// The *_workspace_bytes queries return 0 for arguments their entry would reject.  They differ at iters == 0, where the
+// entries copy and need nothing: the forward queries and most backward ones answer 0 there, while cspn2d_bwd_workspace_bytes
+// and cspn2d_k_bwd_workspace_bytes pass iters == 0 on to the 3x3 backward's own formula.
 size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0) return 0;
+    if (!positive(B, C, H, W, iters)) return 0;
     if (algo != CSPN_ALGO_GENERIC) {
         Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};
         char why[8];
@@ -115,523 +175,362 @@ size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo) {
 int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out, int B, int C, int H,
                    int W, int guidance_channels, int iters, int norm_type, int algo, void* workspace,
                    size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d(guidance, blur, out, B, C, H, W, guidance_channels, iters, norm_type, algo);
+    begin_call();
+    int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
+    if (rc == CSPN_OK) rc = check_algo(algo);
     if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    char why[256] = "";
-    const int chosen = (iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why), workspace);
-    if (chosen < 0) { set_error("cluster kernel unsupported for this problem: %s", why); return chosen; }
-    g_last_algo = chosen;
-    int launches = 0;
-    if (chosen == CSPN_ALGO_GENERIC && algo == CSPN_ALGO_AUTO && iters > 0) {
-        // AUTO sized its workspace for the cluster kernel (cspn2d_workspace_bytes cannot see the pointers); when the
-        // problem then has to take the generic path, say so instead of a bare "workspace too small"
-        const size_t need = generic2d_workspace_bytes(B, C, H, W, iters);
-        if (!workspace || workspace_bytes < need) {
-            set_error("CSPN_ALGO_AUTO falls back to the generic path here (%s), which needs %zu workspace bytes (got %zu): "
-                      "query cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors and workspace",
-                      why[0] ? why : "cluster kernel declined", need, workspace ? workspace_bytes : (size_t)0);
-            return CSPN_ERR_WORKSPACE;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        char why[256] = "";
+        const int chosen = (iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why), workspace);
+        if (chosen < 0) { set_error("cluster kernel unsupported for this problem: %s", why); return chosen; }
+        g_last_algo = chosen;
+        if (chosen == CSPN_ALGO_GENERIC && algo == CSPN_ALGO_AUTO && iters > 0) {
+            // AUTO sized its workspace for the cluster kernel (cspn2d_workspace_bytes cannot see the pointers); when the
+            // problem then has to take the generic path, say so instead of a bare "workspace too small"
+            const size_t need = generic2d_workspace_bytes(B, C, H, W, iters);
+            if (!workspace || workspace_bytes < need) {
+                set_error("CSPN_ALGO_AUTO falls back to the generic path here (%s), which needs %zu workspace bytes (got %zu): "
+                          "query cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors and workspace",
+                          why[0] ? why : "cluster kernel declined", need, workspace ? workspace_bytes : (size_t)0);
+                return (int)CSPN_ERR_WORKSPACE;
+            }
         }
-    }
-    rc = (chosen == CSPN_ALGO_CLUSTER) ? cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, &launches)
-                                       : generic2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+        return (chosen == CSPN_ALGO_CLUSTER) ? cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches)
+                                             : generic2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
 }
 
 int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out, float* const* peer_out,
                           int n_peer, float* multicast_out, int B, int C, int H, int W, int guidance_channels, int iters,
                           int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d(guidance, blur, out, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_CLUSTER);
+    begin_call();
+    int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
+    if (rc == CSPN_OK) rc = check_gather(peer_out, n_peer, multicast_out, iters);
     if (rc != CSPN_OK) return rc;
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    char why[256] = "";
-    if (!cluster2d_supported(p, why, sizeof(why), workspace)) {
-        set_error("the fused gather runs in the cluster kernel's epilogue, which cannot take this problem: %s", why);
-        return CSPN_ERR_UNSUPPORTED;
-    }
-    g_last_algo = CSPN_ALGO_CLUSTER;
-    int launches = 0;
-    rc = cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, &launches, peer_out, n_peer, multicast_out);
-    g_last_launches = launches;
-    return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        char why[256] = "";
+        if (!cluster2d_supported(p, why, sizeof(why), workspace)) {
+            set_error("the fused gather runs in the cluster kernel's epilogue, which cannot take this problem: %s", why);
+            return (int)CSPN_ERR_UNSUPPORTED;
+        }
+        g_last_algo = CSPN_ALGO_CLUSTER;
+        return cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches, peer_out, n_peer, multicast_out);
+    });
 }
 
 size_t cspn2d_bwd_workspace_bytes(int B, int C, int H, int W, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters < 0) return 0;
+    if (!positive(B, C, H, W) || iters < 0) return 0;
     return bwd2d_workspace_bytes(B, C, H, W, iters);
 }
 
 int cspn2d_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
                    float* grad_guidance, float* grad_blur, int B, int C, int H, int W, int guidance_channels,
                    int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    float dummy;
-    int rc = check2d(guidance, blur, &dummy, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_AUTO);
+    begin_call();
+    const int rc = check_prop(2, guidance, blur, grad_out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
     if (rc != CSPN_OK) return rc;
-    if (!grad_out) { set_error("null grad_out"); return CSPN_ERR_INVALID_ARGUMENT; }
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    int launches = 0;
-    rc = bwd2d(p, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        return bwd2d(p, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
 }
 
 // ---- K x K kernels: K = 3 is the operator above, K = 5 / 7 run in cspn2d_wide.cu ----------------------------------
-static bool kernel_size_ok(int K) { return K == 3 || K == 5 || K == 7; }
-
-static int check2d_k(const float* guidance, const float* blur, const void* out, int B, int C, int H, int W, int gch, int K,
-                     int iters, int norm_type) {
-    if (!guidance || !blur || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (!kernel_size_ok(K)) { set_error("kernel size must be 3, 5 or 7, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (gch < K * K - 1) { set_error("a %dx%d kernel needs >= %d guidance channels, got %d", K, K, K * K - 1, gch); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (norm_type != CSPN_NORM_8SUM && norm_type != CSPN_NORM_8SUM_ABS) { set_error("unknown norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
-    return CSPN_OK;
+size_t cspn2d_k_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!positive(B, C, H, W, iters) || !kernel_size_ok(2, K)) return 0;
+    if (K == 3) return cspn2d_workspace_bytes(B, C, H, W, iters, CSPN_ALGO_AUTO);
+    return widek_workspace_bytes(B, C, H, W, K, iters, Family::Normalised);
 }
 
-size_t cspn2d_k_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
-    if (K == 3) return cspn2d_workspace_bytes(B, C, H, W, iters, CSPN_ALGO_AUTO);
-    return widek_workspace_bytes(B, C, H, W, K, iters);
+// gather null: cspn2d_k_fwd_f32
+static int fwd2d_k(const float* guidance, const float* blur, const float* sparse, float* out, const Gather* gather, int B, int C,
+                   int H, int W, int guidance_channels, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                   cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, K, guidance_channels, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3)
+        return gather ? cspn2d_fwd_gather_f32(guidance, blur, sparse, out, gather->peer_out, gather->n_peer, gather->multicast_out, B,
+                                              C, H, W, guidance_channels, iters, norm_type, workspace, workspace_bytes, stream)
+                      : cspn2d_fwd_f32(guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_AUTO,
+                                       workspace, workspace_bytes, stream);
+    return run_forward(blur, "blur", gather, iters, [&](const Fan* fan, int* launches) {
+        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        return widek_forward(p, K, Family::Normalised, workspace, workspace_bytes, (cudaStream_t)stream, launches, fan);
+    });
 }
 
 int cspn2d_k_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out, int B, int C, int H, int W,
                      int guidance_channels, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
                      cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_k(guidance, blur, out, B, C, H, W, guidance_channels, K, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    if (K == 3)
-        return cspn2d_fwd_f32(guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type, CSPN_ALGO_AUTO,
-                              workspace, workspace_bytes, stream);
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    int launches = 0;
-    rc = widek_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return fwd2d_k(guidance, blur, sparse, out, nullptr, B, C, H, W, guidance_channels, K, iters, norm_type, workspace,
+                   workspace_bytes, stream);
 }
 
 int cspn2d_k_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out, float* const* peer_out,
                             int n_peer, float* multicast_out, int B, int C, int H, int W, int guidance_channels, int K,
                             int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_k(guidance, blur, out, B, C, H, W, guidance_channels, K, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    if (K == 3)
-        return cspn2d_fwd_gather_f32(guidance, blur, sparse, out, peer_out, n_peer, multicast_out, B, C, H, W,
-                                     guidance_channels, iters, norm_type, workspace, workspace_bytes, stream);
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = widek_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
-    g_last_launches = launches;
-    return rc;
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return fwd2d_k(guidance, blur, sparse, out, &gather, B, C, H, W, guidance_channels, K, iters, norm_type, workspace,
+                   workspace_bytes, stream);
 }
 
 size_t cspn2d_k_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters < 0 || !kernel_size_ok(K)) return 0;
+    if (!positive(B, C, H, W) || iters < 0 || !kernel_size_ok(2, K)) return 0;
     if (K == 3) return cspn2d_bwd_workspace_bytes(B, C, H, W, iters);
-    return widek_bwd_workspace_bytes(B, C, H, W, K, iters);
+    return widek_bwd_workspace_bytes(B, C, H, W, K, iters, Family::Normalised);
 }
 
 int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
                      float* grad_guidance, float* grad_blur, int B, int C, int H, int W, int guidance_channels, int K,
                      int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_k(guidance, blur, grad_out, B, C, H, W, guidance_channels, K, iters, norm_type);
+    begin_call();
+    const int rc = check_prop(2, guidance, blur, grad_out, B, C, 1, H, W, K, guidance_channels, iters, norm_type);
     if (rc != CSPN_OK) return rc;
     if (K == 3)
         return cspn2d_bwd_f32(guidance, blur, sparse, grad_out, grad_guidance, grad_blur, B, C, H, W, guidance_channels,
                               iters, norm_type, workspace, workspace_bytes, stream);
-    DeviceGuard guard(device_of(blur));
-    if (!guard.ok) { set_error("cannot select the device of `blur`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-    int launches = 0;
-    rc = widek_backward(p, K, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        return widek_backward(p, K, Family::Normalised, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes,
+                              (cudaStream_t)stream, launches);
+    });
 }
 
-// ---- 2D 'paddle' (own-location norm), K in {3, 5, 7}: every K in cspn2d_wide.cu ------------------------------------
-static int check2d_paddle(const float* guidance, const float* feat, const void* out, int B, int C, int H, int W, int K,
-                          int iters) {
-    if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (!kernel_size_ok(K)) { set_error("kernel size must be 3, 5 or 7, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
-    return CSPN_OK;
+// ---- 2D 'paddle' (own-location norm) and caller-supplied gates (fluid.layers.affinity_propagate), K in {3, 5, 7}: every
+// K in cspn2d_wide.cu.  Both take (gates, feat) with K*K-1 gate channels, so they share their entries' bodies ----------
+static size_t own2d_workspace_bytes(Family family, bool bwd, int B, int C, int H, int W, int K, int iters) {
+    if (!positive(B, C, H, W, iters) || !kernel_size_ok(2, K)) return 0;
+    return bwd ? widek_bwd_workspace_bytes(B, C, H, W, K, iters, family) : widek_workspace_bytes(B, C, H, W, K, iters, family);
+}
+
+// gather null: the plain forward
+static int own2d_fwd(Family family, const float* gates, const float* feat, float* out, const Gather* gather, int B, int C, int H,
+                     int W, int K, int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(2, gates, feat, out, B, C, 1, H, W, K, K * K - 1, iters, 0);
+    if (rc != CSPN_OK) return rc;
+    return run_forward(feat, "feat", gather, iters, [&](const Fan* fan, int* launches) {
+        Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
+        return widek_forward(p, K, family, workspace, workspace_bytes, (cudaStream_t)stream, launches, fan);
+    });
+}
+
+static int own2d_bwd(Family family, const float* gates, const float* feat, const float* grad_out, float* grad_gates,
+                     float* grad_feat, int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                     cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(2, gates, feat, grad_out, B, C, 1, H, W, K, K * K - 1, iters, 0);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        Problem2D p{gates, feat, nullptr, nullptr, B, C, H, W, K * K - 1, iters, 0};
+        return widek_backward(p, K, family, grad_out, grad_gates, grad_feat, workspace, workspace_bytes, (cudaStream_t)stream,
+                              launches);
+    });
 }
 
 size_t cspn2d_paddle_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
-    return widek_workspace_bytes(B, C, H, W, K, iters);
+    return own2d_workspace_bytes(Family::Paddle, false, B, C, H, W, K, iters);
 }
 
 int cspn2d_paddle_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int H, int W, int K, int iters,
                           void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_paddle(guidance, feat, out, B, C, H, W, K, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
-    int launches = 0;
-    rc = widek_paddle_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return own2d_fwd(Family::Paddle, guidance, feat, out, nullptr, B, C, H, W, K, iters, workspace, workspace_bytes, stream);
 }
 
 int cspn2d_paddle_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
                                  float* multicast_out, int B, int C, int H, int W, int K, int iters, void* workspace,
                                  size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_paddle(guidance, feat, out, B, C, H, W, K, iters);
-    if (rc != CSPN_OK) return rc;
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = widek_paddle_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
-    g_last_launches = launches;
-    return rc;
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return own2d_fwd(Family::Paddle, guidance, feat, out, &gather, B, C, H, W, K, iters, workspace, workspace_bytes, stream);
 }
 
 size_t cspn2d_paddle_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
-    return widek_bwd_workspace_bytes(B, C, H, W, K, iters);
+    return own2d_workspace_bytes(Family::Paddle, true, B, C, H, W, K, iters);
 }
 
 int cspn2d_paddle_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
                           int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
                           cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d_paddle(guidance, feat, grad_out, B, C, H, W, K, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{guidance, feat, nullptr, nullptr, B, C, H, W, K * K - 1, iters, 0};
-    int launches = 0;
-    rc = widek_paddle_backward(p, K, grad_out, grad_guidance, grad_feat, workspace, workspace_bytes, (cudaStream_t)stream,
-                               &launches);
-    g_last_launches = launches;
-    return rc;
+    return own2d_bwd(Family::Paddle, guidance, feat, grad_out, grad_guidance, grad_feat, B, C, H, W, K, iters, workspace,
+                     workspace_bytes, stream);
 }
 
+size_t cspn2d_gates_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    return own2d_workspace_bytes(Family::Gates, false, B, C, H, W, K, iters);
+}
+
+int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out, int B, int C, int H, int W, int K, int iters,
+                         void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    return own2d_fwd(Family::Gates, gates, feat, out, nullptr, B, C, H, W, K, iters, workspace, workspace_bytes, stream);
+}
+
+int cspn2d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out, float* const* peer_out, int n_peer,
+                                float* multicast_out, int B, int C, int H, int W, int K, int iters, void* workspace,
+                                size_t workspace_bytes, cspn_stream_t stream) {
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return own2d_fwd(Family::Gates, gates, feat, out, &gather, B, C, H, W, K, iters, workspace, workspace_bytes, stream);
+}
+
+size_t cspn2d_gates_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    return own2d_workspace_bytes(Family::Gates, true, B, C, H, W, K, iters);
+}
+
+int cspn2d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out, float* grad_gates, float* grad_feat,
+                         int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                         cspn_stream_t stream) {
+    return own2d_bwd(Family::Gates, gates, feat, grad_out, grad_gates, grad_feat, B, C, H, W, K, iters, workspace, workspace_bytes,
+                     stream);
+}
+
+// ---- 3D: the 3x3x3 operator (cspn3d.cu) -----------------------------------------------------------------------------
 size_t cspn3d_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0) return 0;
+    if (!positive(B, C, D, H, W, iters)) return 0;
     return generic3d_workspace_bytes(B, C, D, H, W, iters);
 }
 
-static int check3d(const float* guidance, const float* feat, const float* out, int B, int C, int D, int H, int W, int iters,
-                   int norm_type) {
-    if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters < 0) { set_error("prop_step must be >= 0"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (norm_type < CSPN_NORM_26SUM || norm_type > CSPN_NORM_PADDLE) { set_error("unknown 3D norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
-    return CSPN_OK;
+// gather null: cspn3d_fwd_f32
+static int fwd3d(const float* guidance, const float* feat, float* out, const Gather* gather, int B, int C, int D, int H, int W,
+                 int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(3, guidance, feat, out, B, C, D, H, W, 3, 0, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    return run_forward(feat, "feat", gather, iters, [&](const Fan* fan, int* launches) {
+        return generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
+                                 (cudaStream_t)stream, launches, fan);
+    });
 }
 
 int cspn3d_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int iters,
                    int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check3d(guidance, feat, out, B, C, D, H, W, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
-                           (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return fwd3d(guidance, feat, out, nullptr, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
 }
 
 int cspn3d_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
                           float* multicast_out, int B, int C, int D, int H, int W, int iters, int norm_type, void* workspace,
                           size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check3d(guidance, feat, out, B, C, D, H, W, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = generic3d_forward(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
-                           (cudaStream_t)stream, &launches, &fan);
-    g_last_launches = launches;
-    return rc;
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return fwd3d(guidance, feat, out, &gather, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
 }
 
 size_t cspn3d_bwd_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0) return 0;
+    if (!positive(B, C, D, H, W, iters)) return 0;
     return bwd3d_workspace_bytes(C, D, H, W, iters);
 }
 
 int cspn3d_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
                    int B, int C, int D, int H, int W, int iters, int norm_type, void* workspace, size_t workspace_bytes,
                    cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    if (!guidance || !feat || !grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters < 0) { set_error("invalid 3D shape / prop_step"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (norm_type < CSPN_NORM_26SUM || norm_type > CSPN_NORM_PADDLE) { set_error("unknown 3D norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    int rc = bwd3d(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
-                   (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    begin_call();
+    const int rc = check_prop(3, guidance, feat, grad_out, B, C, D, H, W, 3, 0, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return bwd3d(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
+                     (cudaStream_t)stream, launches);
+    });
 }
 
-// ---- K x K x K kernels: K = 3 is the 3D operator above, K = 5 runs in cspn3d_wide.cu ------------------------------
-static int check3d_k(const float* guidance, const float* feat, const void* out, int B, int C, int D, int H, int W, int K,
-                     int iters, int norm_type) {
-    if (!guidance || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d D=%d H=%d W=%d", B, C, D, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (K != 3 && K != 5) { set_error("3D kernel size must be 3 or 5, got %d", K); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (norm_type < CSPN_NORM_26SUM || norm_type > CSPN_NORM_PADDLE) { set_error("unknown 3D norm_type %d", norm_type); return CSPN_ERR_INVALID_ARGUMENT; }
-    return CSPN_OK;
+// ---- K x K x K kernels (K = 3 is the 3D operator above, K = 5 runs in cspn3d_wide.cu) and caller-supplied gates (K in
+// {3, 5}, both in cspn3d_wide.cu).  The gates entries have no norm_type and pass 0 -------------------------------------
+static size_t wide3d_workspace_bytes(Family family, bool bwd, int B, int C, int D, int H, int W, int K, int iters) {
+    if (!positive(B, C, D, H, W, iters) || !kernel_size_ok(3, K)) return 0;
+    if (K == 3 && family != Family::Gates) return bwd ? cspn3d_bwd_workspace_bytes(B, C, D, H, W, iters) : cspn3d_workspace_bytes(B, C, D, H, W, iters);
+    return bwd ? widek3d_bwd_workspace_bytes(C, D, H, W, K, iters, family) : widek3d_workspace_bytes(B, C, D, H, W, K, iters, family);
+}
+
+// gather null: the plain forward
+static int wide3d_fwd(Family family, const float* guidance, const float* feat, float* out, const Gather* gather, int B, int C,
+                      int D, int H, int W, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                      cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(3, guidance, feat, out, B, C, D, H, W, K, 0, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3 && family != Family::Gates)
+        return fwd3d(guidance, feat, out, gather, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
+    return run_forward(feat, "feat", gather, iters, [&](const Fan* fan, int* launches) {
+        return widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, family, norm_type, workspace, workspace_bytes,
+                               (cudaStream_t)stream, launches, fan);
+    });
+}
+
+static int wide3d_bwd(Family family, const float* guidance, const float* feat, const float* grad_out, float* grad_guidance,
+                      float* grad_feat, int B, int C, int D, int H, int W, int K, int iters, int norm_type, void* workspace,
+                      size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(3, guidance, feat, grad_out, B, C, D, H, W, K, 0, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    if (K == 3 && family != Family::Gates)
+        return cspn3d_bwd_f32(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace,
+                              workspace_bytes, stream);
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return widek3d_backward(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, K, iters, family, norm_type,
+                                workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
 }
 
 size_t cspn3d_k_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
-    if (K == 3) return cspn3d_workspace_bytes(B, C, D, H, W, iters);
-    return widek3d_workspace_bytes(B, C, D, H, W, K, iters);
+    return wide3d_workspace_bytes(Family::Normalised, false, B, C, D, H, W, K, iters);
 }
 
 int cspn3d_k_fwd_f32(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
                      int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check3d_k(guidance, feat, out, B, C, D, H, W, K, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    if (K == 3) return cspn3d_fwd_f32(guidance, feat, out, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, norm_type, workspace, workspace_bytes, (cudaStream_t)stream,
-                         &launches);
-    g_last_launches = launches;
-    return rc;
+    return wide3d_fwd(Family::Normalised, guidance, feat, out, nullptr, B, C, D, H, W, K, iters, norm_type, workspace,
+                      workspace_bytes, stream);
 }
 
 int cspn3d_k_fwd_gather_f32(const float* guidance, const float* feat, float* out, float* const* peer_out, int n_peer,
                             float* multicast_out, int B, int C, int D, int H, int W, int K, int iters, int norm_type,
                             void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check3d_k(guidance, feat, out, B, C, D, H, W, K, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    if (K == 3)
-        return cspn3d_fwd_gather_f32(guidance, feat, out, peer_out, n_peer, multicast_out, B, C, D, H, W, iters, norm_type,
-                                     workspace, workspace_bytes, stream);
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = widek3d_forward(guidance, feat, out, B, C, D, H, W, K, iters, norm_type, workspace, workspace_bytes, (cudaStream_t)stream,
-                         &launches, &fan);
-    g_last_launches = launches;
-    return rc;
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return wide3d_fwd(Family::Normalised, guidance, feat, out, &gather, B, C, D, H, W, K, iters, norm_type, workspace,
+                      workspace_bytes, stream);
 }
 
 size_t cspn3d_k_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
-    if (K == 3) return cspn3d_bwd_workspace_bytes(B, C, D, H, W, iters);
-    return widek3d_bwd_workspace_bytes(C, D, H, W, K, iters);
+    return wide3d_workspace_bytes(Family::Normalised, true, B, C, D, H, W, K, iters);
 }
 
 int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
                      int B, int C, int D, int H, int W, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
                      cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check3d_k(guidance, feat, grad_out, B, C, D, H, W, K, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    if (K == 3)
-        return cspn3d_bwd_f32(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace,
-                              workspace_bytes, stream);
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = widek3d_backward(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, K, iters, norm_type, workspace,
-                          workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
-}
-
-// ---- caller-supplied gates (fluid.layers.affinity_propagate): 2D K in {3, 5, 7}, 3D K in {3, 5} ----------------------
-static int check_gates(const float* gates, const float* feat, const void* out, int B, int C, int D, int H, int W, int K,
-                       int iters, bool is3d) {
-    if (!gates || !feat || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0) { set_error("non-positive shape B=%d C=%d D=%d H=%d W=%d", B, C, D, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (is3d ? (K != 3 && K != 5) : !kernel_size_ok(K)) { set_error("%s kernel size must be %s, got %d", is3d ? "3D" : "2D", is3d ? "3 or 5" : "3, 5 or 7", K); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (iters < 0) { set_error("prop_step must be >= 0, got %d", iters); return CSPN_ERR_INVALID_ARGUMENT; }
-    return CSPN_OK;
-}
-
-size_t cspn2d_gates_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
-    return widek_gates_workspace_bytes(B, C, H, W, iters);
-}
-
-int cspn2d_gates_fwd_f32(const float* gates, const float* feat, float* out, int B, int C, int H, int W, int K, int iters,
-                         void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, out, B, C, 1, H, W, K, iters, false);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
-    int launches = 0;
-    rc = widek_gates_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
-}
-
-int cspn2d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out, float* const* peer_out, int n_peer,
-                                float* multicast_out, int B, int C, int H, int W, int K, int iters, void* workspace,
-                                size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, out, B, C, 1, H, W, K, iters, false);
-    if (rc != CSPN_OK) return rc;
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{gates, feat, nullptr, out, B, C, H, W, K * K - 1, iters, 0};
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = widek_gates_forward(p, K, workspace, workspace_bytes, (cudaStream_t)stream, &launches, &fan);
-    g_last_launches = launches;
-    return rc;
-}
-
-size_t cspn2d_gates_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || iters <= 0 || !kernel_size_ok(K)) return 0;
-    return widek_gates_bwd_workspace_bytes(B, C, H, W, iters);
-}
-
-int cspn2d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out, float* grad_gates, float* grad_feat,
-                         int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
-                         cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, grad_out, B, C, 1, H, W, K, iters, false);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    Problem2D p{gates, feat, nullptr, nullptr, B, C, H, W, K * K - 1, iters, 0};
-    int launches = 0;
-    rc = widek_gates_backward(p, K, grad_out, grad_gates, grad_feat, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return wide3d_bwd(Family::Normalised, guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, K, iters, norm_type,
+                      workspace, workspace_bytes, stream);
 }
 
 size_t cspn3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
-    return widek3d_gates_workspace_bytes(B, C, D, H, W, iters);
+    return wide3d_workspace_bytes(Family::Gates, false, B, C, D, H, W, K, iters);
 }
 
 int cspn3d_gates_fwd_f32(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
                          void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, out, B, C, D, H, W, K, iters, true);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = widek3d_gates_forward(gates, feat, out, B, C, D, H, W, K, iters, workspace, workspace_bytes, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return wide3d_fwd(Family::Gates, gates, feat, out, nullptr, B, C, D, H, W, K, iters, 0, workspace, workspace_bytes, stream);
 }
 
 int cspn3d_gates_fwd_gather_f32(const float* gates, const float* feat, float* out, float* const* peer_out, int n_peer,
                                 float* multicast_out, int B, int C, int D, int H, int W, int K, int iters, void* workspace,
                                 size_t workspace_bytes, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, out, B, C, D, H, W, K, iters, true);
-    if (rc != CSPN_OK) return rc;
-    rc = check_gather(peer_out, n_peer, multicast_out, iters);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    const Fan fan = make_fan(peer_out, n_peer, multicast_out);
-    int launches = 0;
-    rc = widek3d_gates_forward(gates, feat, out, B, C, D, H, W, K, iters, workspace, workspace_bytes, (cudaStream_t)stream,
-                               &launches, &fan);
-    g_last_launches = launches;
-    return rc;
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return wide3d_fwd(Family::Gates, gates, feat, out, &gather, B, C, D, H, W, K, iters, 0, workspace, workspace_bytes, stream);
 }
 
 size_t cspn3d_gates_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
-    if (B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters <= 0 || (K != 3 && K != 5)) return 0;
-    return widek3d_gates_bwd_workspace_bytes(C, D, H, W, iters);
+    return wide3d_workspace_bytes(Family::Gates, true, B, C, D, H, W, K, iters);
 }
 
 int cspn3d_gates_bwd_f32(const float* gates, const float* feat, const float* grad_out, float* grad_gates, float* grad_feat,
                          int B, int C, int D, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
                          cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_gates(gates, feat, grad_out, B, C, D, H, W, K, iters, true);
-    if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(feat));
-    if (!guard.ok) { set_error("cannot select the device of `feat`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = widek3d_gates_backward(gates, feat, grad_out, grad_gates, grad_feat, B, C, D, H, W, K, iters, workspace, workspace_bytes,
-                                (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return wide3d_bwd(Family::Gates, gates, feat, grad_out, grad_gates, grad_feat, B, C, D, H, W, K, iters, 0, workspace,
+                      workspace_bytes, stream);
 }
 
 // ---- unpool + crop + 3x3 convolution (the guidance and depth heads) ---------------------------------------------------
 static int check_unpool_conv(const void* x, const void* weight, const void* out, int B, int Cin, int h, int w, int Cout, int H,
                              int W) {
     if (!x || !weight || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
-    if (B <= 0 || Cin <= 0 || h <= 0 || w <= 0 || Cout <= 0 || H <= 0 || W <= 0) {
+    if (!positive(B, Cin, h, w, Cout, H, W)) {
         set_error("non-positive size B=%d Cin=%d h=%d w=%d Cout=%d H=%d W=%d", B, Cin, h, w, Cout, H, W);
         return CSPN_ERR_INVALID_ARGUMENT;
     }
@@ -647,29 +546,24 @@ static int check_unpool_conv(const void* x, const void* weight, const void* out,
 
 int cspn_unpool_conv3x3_fwd_f32(const float* x, const float* weight, float* out, int B, int Cin, int h, int w, int Cout, int H,
                                 int W, cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_unpool_conv(x, weight, out, B, Cin, h, w, Cout, H, W);
+    begin_call();
+    const int rc = check_unpool_conv(x, weight, out, B, Cin, h, w, Cout, H, W);
     if (rc != CSPN_OK) return rc;
-    DeviceGuard guard(device_of(x));
-    if (!guard.ok) { set_error("cannot select the device of `x`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = unpool_conv_forward(x, weight, out, B, Cin, h, w, Cout, H, W, (cudaStream_t)stream, &launches);
-    g_last_launches = launches;
-    return rc;
+    return on_device_of(x, "x", [&](int* launches) {
+        return unpool_conv_forward(x, weight, out, B, Cin, h, w, Cout, H, W, (cudaStream_t)stream, launches);
+    });
 }
 
 size_t cspn_unpool_conv3x3_bwd_workspace_bytes(int B, int Cin, int h, int w, int Cout, int H, int W) {
-    if (B <= 0 || Cin <= 0 || h <= 0 || w <= 0 || Cout <= 0 || H <= 0 || W <= 0 || H > 2 * h || W > 2 * w) return 0;
+    if (!positive(B, Cin, h, w, Cout, H, W) || H > 2 * h || W > 2 * w) return 0;
     return unpool_conv_bwd_workspace_bytes(B, Cin, H, W, Cout);
 }
 
 int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, const float* grad_out, float* grad_x, float* grad_weight,
                                 int B, int Cin, int h, int w, int Cout, int H, int W, void* workspace, size_t workspace_bytes,
                                 cspn_stream_t stream) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check_unpool_conv(x, weight, grad_out, B, Cin, h, w, Cout, H, W);
+    begin_call();
+    const int rc = check_unpool_conv(x, weight, grad_out, B, Cin, h, w, Cout, H, W);
     if (rc != CSPN_OK) return rc;
     if ((reinterpret_cast<uintptr_t>(grad_x) | reinterpret_cast<uintptr_t>(grad_weight)) & 3) {
         set_error("gradient pointers must be 4-byte aligned");
@@ -682,13 +576,10 @@ int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, const float
             return CSPN_ERR_WORKSPACE;
         }
     }
-    DeviceGuard guard(device_of(x));
-    if (!guard.ok) { set_error("cannot select the device of `x`"); return CSPN_ERR_CUDA; }
-    int launches = 0;
-    rc = unpool_conv_backward(x, weight, grad_out, grad_x, grad_weight, B, Cin, h, w, Cout, H, W, workspace, (cudaStream_t)stream,
-                              &launches);
-    g_last_launches = launches;
-    return rc;
+    return on_device_of(x, "x", [&](int* launches) {
+        return unpool_conv_backward(x, weight, grad_out, grad_x, grad_weight, B, Cin, h, w, Cout, H, W, workspace,
+                                    (cudaStream_t)stream, launches);
+    });
 }
 
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
@@ -702,17 +593,15 @@ int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* 
                     generic2d_workspace_bytes(B, C, H, W, iters), why[0] ? "; cluster kernel not used: " : "", why);
 }
 
-int cspn2d_plan_json(int H, int W, int iters, char* buf, int buf_len) {
+static int plan_json(int H, int W, int iters, int chained, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
-    if (H <= 0 || W <= 0 || iters <= 0) return snprintf(buf, buf_len, "{\"supported\": false, \"why\": \"invalid shape\"}");
-    return cluster2d_plan_json(H, W, iters, 0, buf, buf_len);
+    if (!positive(H, W, iters)) return snprintf(buf, buf_len, "{\"supported\": false, \"why\": \"invalid shape\"}");
+    return cluster2d_plan_json(H, W, iters, chained, buf, buf_len);
 }
 
-int cspn2d_plan_json_chained(int H, int W, int iters, char* buf, int buf_len) {
-    if (!buf || buf_len <= 0) return 0;
-    if (H <= 0 || W <= 0 || iters <= 0) return snprintf(buf, buf_len, "{\"supported\": false, \"why\": \"invalid shape\"}");
-    return cluster2d_plan_json(H, W, iters, 1, buf, buf_len);
-}
+int cspn2d_plan_json(int H, int W, int iters, char* buf, int buf_len) { return plan_json(H, W, iters, 0, buf, buf_len); }
+
+int cspn2d_plan_json_chained(int H, int W, int iters, char* buf, int buf_len) { return plan_json(H, W, iters, 1, buf, buf_len); }
 
 }  // extern "C"
 
@@ -772,9 +661,9 @@ struct DrainOnExit {
 extern "C" CSPN_API int cspn2d_fwd_f32_host(const float* guidance, const float* blur, const float* sparse, float* out, int B,
                                    int C, int H, int W, int guidance_channels, int iters, int norm_type, int algo,
                                    int device) {
-    clear_error();
-    g_last_launches = 0;
-    int rc = check2d(guidance, blur, out, B, C, H, W, guidance_channels, iters, norm_type, algo);
+    begin_call();
+    int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
+    if (rc == CSPN_OK) rc = check_algo(algo);
     if (rc != CSPN_OK) return rc;
     if (device < 0 || device >= 16) { set_error("device %d out of range", device); return CSPN_ERR_INVALID_ARGUMENT; }
     DeviceGuard guard(device);
@@ -852,12 +741,8 @@ extern "C" CSPN_API int cspn2d_fwd_f32_host(const float* guidance, const float* 
 
 extern "C" CSPN_API int cspn3d_fwd_f32_host(const float* guidance, const float* feat, float* out, int B, int C, int D, int H,
                                    int W, int iters, int norm_type, int device) {
-    clear_error();
-    g_last_launches = 0;
-    if (!guidance || !feat || !out || B <= 0 || C <= 0 || D <= 0 || H <= 0 || W <= 0 || iters < 0) {
-        set_error("invalid 3D arguments");
-        return CSPN_ERR_INVALID_ARGUMENT;
-    }
+    begin_call();
+    if (const int rc = check_prop(3, guidance, feat, out, B, C, D, H, W, 3, 0, iters, norm_type)) return rc;
     if (device < 0 || device >= 16) { set_error("device %d out of range", device); return CSPN_ERR_INVALID_ARGUMENT; }
     DeviceGuard guard(device);
     if (!guard.ok) { set_error("cannot select device %d", device); return CSPN_ERR_CUDA; }

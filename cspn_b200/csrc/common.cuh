@@ -98,7 +98,7 @@ inline Fan offset_fan(const Fan& f, size_t off) {
     return g;
 }
 
-// The FAN epilogue of the 3D step kernels: v, just stored at element o of dst, also to element o of every destination
+// The FAN epilogue of the step kernels: v, just stored at element o of dst, also to element o of every destination
 __device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float4 v) {
 #pragma unroll
     for (int e = 0; e < 7; ++e)          // peer GPUs' gather buffers (NVLink stores); n_peer is uniform
@@ -115,25 +115,20 @@ __device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float v) {
     if (fan.mc) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(fan.mc + o), "f"(v) : "memory");
 }
 
-// K x K kernels, K in {5, 7} (cspn2d_wide.cu); fan non-null: the fused gather
-size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters);
-int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+// The operator families of the wide kernels (cspn2d_wide.cu, cspn3d_wide.cu)
+enum class Family {
+    Normalised,   // weights gathered from the neighbours' guidance and normalised; 2D K in {5, 7}, 3D K = 5 with `mode`
+    Paddle,       // 2D 'paddle' own-location norm, K in {3, 5, 7} (in 3D it is mode 2 of Normalised)
+    Gates,        // caller-supplied gates used as given; 2D K in {3, 5, 7}, 3D K in {3, 5}
+};
+
+// 2D.  Paddle and Gates: p.sparse null, p.gch == K*K-1, p.guidance [B][K*K-1][H][W].  fan non-null: the fused gather
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family);
+int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
                   const Fan* fan = nullptr);
-size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
-int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-                   size_t ws_bytes, cudaStream_t stream, int* launches);
-// 'paddle' own-location norm, K in {3, 5, 7}, on the same kernels and workspaces (p.sparse null, p.gch == K*K-1)
-int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
-                         const Fan* fan = nullptr);
-int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-                          size_t ws_bytes, cudaStream_t stream, int* launches);
-// caller-supplied gates, K in {3, 5, 7}: p.guidance [B][K*K-1][H][W] used as given (p.sparse null, p.gch == K*K-1)
-size_t widek_gates_workspace_bytes(int B, int C, int H, int W, int iters);
-size_t widek_gates_bwd_workspace_bytes(int B, int C, int H, int W, int iters);
-int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
-                        const Fan* fan = nullptr);
-int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,
-                         size_t ws_bytes, cudaStream_t stream, int* launches);
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family);
+int widek_backward(const Problem2D& p, int K, Family family, const float* grad_out, float* grad_guidance, float* grad_blur,
+                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);
@@ -147,22 +142,16 @@ size_t bwd3d_workspace_bytes(int C, int D, int H, int W, int iters);
 int bwd3d(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat, int B, int C,
           int D, int H, int W, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 
-// K x K x K kernels, K = 5 (cspn3d_wide.cu); fan non-null: the fused gather
-size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);
+// 3D, Normalised (guidance [B][K^3-1][D][H][W], mode 0 signed / 1 abs / 2 'paddle') or Gates (gates of that shape, mode
+// unused).  fan non-null: the fused gather
+size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters, Family family);
 int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan = nullptr);
-size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters);
+                    Family family, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                    const Fan* fan = nullptr);
+size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters, Family family);
 int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
-                     int D, int H, int W, int K, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream,
-                     int* launches);
-// caller-supplied gates [B][K^3-1][D][H][W], K in {3, 5} (cspn3d_wide.cu)
-size_t widek3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int iters);
-size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters);
-int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan = nullptr);
-int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,
-                           int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
-                           int* launches);
+                     int D, int H, int W, int K, int iters, Family family, int mode, void* ws, size_t ws_bytes,
+                     cudaStream_t stream, int* launches);
 
 // Unpool + crop + 3x3 convolution of the guidance / depth heads (unpool_conv.cu); shapes checked by the caller
 int unpool_conv_launchable(int B, int Cin, int Cout, const char** why);

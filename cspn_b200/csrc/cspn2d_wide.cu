@@ -175,14 +175,7 @@ stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, con
     const size_t o = (size_t)bc * HW + p;
     const float4 v = make_float4(acc0, acc1, acc2, acc3);
     *reinterpret_cast<float4*>(dst + o) = v;
-    if constexpr (FAN) {
-#pragma unroll
-        for (int e = 0; e < 7; ++e)          // peer GPUs' gather buffers (NVLink stores); n_peer is uniform
-            if (e < fan.n_peer) __stcs(reinterpret_cast<float4*>(fan.peer[e] + o), v);
-        if (fan.mc)                          // NVLS: one store, replicated by the switch
-            asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(fan.mc + o), "f"(v.x), "f"(v.y),
-                         "f"(v.z), "f"(v.w) : "memory");
-    }
+    if constexpr (FAN) fan_store(fan, o, v);
 }
 
 // ---- step / adjoint, one pixel per thread (any W, any alignment).  Tile 32 x 8 pixels + R halo --------------------
@@ -218,12 +211,7 @@ stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, 
     for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
     const size_t o = (size_t)bc * HW + p;
     dst[o] = acc;
-    if constexpr (FAN) {
-#pragma unroll
-        for (int e = 0; e < 7; ++e)
-            if (e < fan.n_peer) __stcs(fan.peer[e] + o, acc);
-        if (fan.mc) asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(fan.mc + o), "f"(acc) : "memory");
-    }
+    if constexpr (FAN) fan_store(fan, o, acc);
 }
 
 // lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only.
@@ -411,12 +399,7 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches, 
                                    wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
             ++*launches;
         }
-        Fan gfan{};
-        if (fan) {
-            gfan.n_peer = fan->n_peer;
-            for (int e = 0; e < fan->n_peer; ++e) gfan.peer[e] = fan->peer[e] + (size_t)b0 * plane;
-            gfan.mc = fan->mc ? fan->mc + (size_t)b0 * plane : nullptr;
-        }
+        const Fan gfan = fan ? offset_fan(*fan, (size_t)b0 * plane) : Fan{};
         const float* cur = blur;
         float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < p.iters; ++it) {
@@ -486,142 +469,101 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
     return CSPN_OK;
 }
 
+// What the three families' fronts do differently; their kernels differ by the PADDLE / RAW flags (see with_kernels)
+struct FamilyTraits {
+    const char* name;        // follows "KxK 2D" in messages
+    bool zero_grad_first;    // grad_guidance is zero-filled before every run, not only at iters == 0: channels >= K*K-1 and
+                             // taps that read the padding get no store.  The other two families write every guidance
+                             // gradient (each g_j(p) feeds pixel p alone; a tap that reads the padding gets 0)
+    bool checks_grid_y;
+    bool no_grad_is_no_op;   // a backward that is asked for neither gradient launches nothing
+};
+
+const FamilyTraits& traits(Family family) {
+    static const FamilyTraits t[] = {{"", true, false, false}, {" 'paddle'", false, false, false}, {" gates", false, true, true}};
+    return t[(int)family];
+}
+
+// f(R, PADDLE, RAW) as integral constants for the K x K kernels of `family`.  The normalised family has no R = 1 kernels:
+// its K = 3 is the 3x3 operator, which the C ABI never sends here.
+template <class F>
+int with_kernels(int K, Family family, F&& f) {
+    using std::integral_constant;
+    constexpr std::true_type yes{};
+    constexpr std::false_type no{};
+    const auto radius = [&](auto paddle, auto raw) {
+        if constexpr (paddle)
+            if (K == 3) return f(integral_constant<int, 1>{}, paddle, raw);
+        return K == 5 ? f(integral_constant<int, 2>{}, paddle, raw) : f(integral_constant<int, 3>{}, paddle, raw);
+    };
+    return family == Family::Normalised ? radius(no, no) : family == Family::Paddle ? radius(yes, no) : radius(yes, yes);
+}
+
+// The workspace holds what `need` says, and the launch grids (z = image*channel, y = rows of 8) take the problem
+int check_launch(const Problem2D& p, int K, const FamilyTraits& t, const char* what, size_t need, const void* ws, size_t ws_bytes) {
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%d 2D%s %s needs %zu workspace bytes, got %zu", K, K, t.name, what, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    if ((long long)p.B * p.C > 65535) {
+        set_error("%dx%d 2D%s %s: B*C=%lld exceeds gridDim.z", K, K, t.name, what, (long long)p.B * p.C);
+        return CSPN_ERR_UNSUPPORTED;
+    }
+    if (t.checks_grid_y && (p.H + kSclTH - 1) / kSclTH > 65535) {
+        set_error("%dx%d 2D%s %s: H=%d exceeds gridDim.y", K, K, t.name, what, p.H);
+        return CSPN_ERR_UNSUPPORTED;
+    }
+    return CSPN_OK;
+}
+
 }  // namespace
 
-size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+// Normalised and 'paddle': K*K weight planes per image and the ping-pong buffer.  Gates: the caller's gates are the weight
+// planes, and a single step writes `out` directly.
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W;
+    if (family == Family::Gates) return iters >= 2 ? sizeof(float) * (size_t)B * C * HW : 0;
     return sizeof(float) * ((size_t)B * K * K * HW + (size_t)B * C * HW);
 }
 
-size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+// The weight planes as above, then d_1..d_{N-1} and the lambdas: 2N planes of B*C images, 2N-2 for gates (see backward_k)
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W;
+    if (family == Family::Gates) return sizeof(float) * (2 * (size_t)iters - 2) * B * C * HW;
     return sizeof(float) * ((size_t)B * K * K * HW + 2 * (size_t)iters * B * C * HW);
 }
 
-int widek_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
-    const size_t n = (size_t)p.B * p.C * p.H * p.W;
+int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
+                  const Fan* fan) {
     if (p.iters == 0) {
-        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%d 2D path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
-    return K == 5 ? forward_k<2, false>(p, ws, stream, launches, fan) : forward_k<3, false>(p, ws, stream, launches, fan);
+    const int rc = check_launch(p, K, traits(family), "path", widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    return with_kernels(K, family, [&](auto R, auto PADDLE, auto RAW) {
+        return forward_k<R(), PADDLE(), RAW()>(p, ws, stream, launches, fan);
+    });
 }
 
-int widek_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-                   size_t ws_bytes, cudaStream_t stream, int* launches) {
+int widek_backward(const Problem2D& p, int K, Family family, const float* grad_out, float* grad_guidance, float* grad_blur,
+                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const FamilyTraits& t = traits(family);
     const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
-    if (grad_guidance)   // channels >= K*K-1 and taps that read the padding get zero gradient
+    if (grad_guidance && (t.zero_grad_first || p.iters == 0))
         CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
-    if (p.iters == 0) {
-        if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%d 2D backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D backward: B*C exceeds gridDim.z", K, K); return CSPN_ERR_UNSUPPORTED; }
-    return K == 5 ? backward_k<2, false>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
-                  : backward_k<3, false>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
-}
-
-// 'paddle': p.sparse is null and p.gch == K*K-1 (the C ABI sets both); same workspaces as the K x K path
-int widek_paddle_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
-                         const Fan* fan) {
-    if (p.iters == 0) {
-        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%d 2D 'paddle' path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D 'paddle' path: B*C=%lld exceeds gridDim.z", K, K, (long long)p.B * p.C); return CSPN_ERR_UNSUPPORTED; }
-    if (K == 3) return forward_k<1, true>(p, ws, stream, launches, fan);
-    return K == 5 ? forward_k<2, true>(p, ws, stream, launches, fan) : forward_k<3, true>(p, ws, stream, launches, fan);
-}
-
-int widek_paddle_backward(const Problem2D& p, int K, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-                          size_t ws_bytes, cudaStream_t stream, int* launches) {
-    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
     if (p.iters == 0) {   // the identity: no dependence on the guidance
-        if (grad_guidance) CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
         if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%d 2D 'paddle' backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D 'paddle' backward: B*C exceeds gridDim.z", K, K); return CSPN_ERR_UNSUPPORTED; }
-    // every guidance gradient is written by the finalize (each g_j(p) feeds pixel p alone): no zero fill
-    if (K == 3) return backward_k<1, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
-    return K == 5 ? backward_k<2, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches)
-                  : backward_k<3, true>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
-}
-
-// Caller-supplied gates: p.guidance [B][K*K-1][H][W] used as given, p.sparse null, p.gch == K*K-1 (the C ABI sets both)
-size_t widek_gates_workspace_bytes(int B, int C, int H, int W, int iters) {
-    return iters >= 2 ? sizeof(float) * (size_t)B * C * H * W : 0;
-}
-
-size_t widek_gates_bwd_workspace_bytes(int B, int C, int H, int W, int iters) {
-    return iters >= 2 ? sizeof(float) * (2 * (size_t)iters - 2) * B * C * H * W : 0;
-}
-
-static bool gates_grid_ok(const Problem2D& p, int K, const char* what) {
-    if ((long long)p.B * p.C > 65535) { set_error("%dx%d 2D gates %s: B*C=%lld exceeds gridDim.z", K, K, what, (long long)p.B * p.C); return false; }
-    if ((p.H + kSclTH - 1) / kSclTH > 65535) { set_error("%dx%d 2D gates %s: H=%d exceeds gridDim.y", K, K, what, p.H); return false; }
-    return true;
-}
-
-int widek_gates_forward(const Problem2D& p, int K, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
-                        const Fan* fan) {
-    if (p.iters == 0) {
-        CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek_gates_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
-    if (need && (!ws || ws_bytes < need)) {
-        set_error("%dx%d 2D gates path needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!gates_grid_ok(p, K, "path")) return CSPN_ERR_UNSUPPORTED;
-    if (K == 3) return forward_k<1, true, true>(p, ws, stream, launches, fan);
-    return K == 5 ? forward_k<2, true, true>(p, ws, stream, launches, fan)
-                  : forward_k<3, true, true>(p, ws, stream, launches, fan);
-}
-
-int widek_gates_backward(const Problem2D& p, int K, const float* grad_out, float* grad_gates, float* grad_feat, void* ws,
-                         size_t ws_bytes, cudaStream_t stream, int* launches) {
-    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
-    if (p.iters == 0) {   // the identity: no dependence on the gates
-        if (grad_gates) CSPN_CUDA_TRY(cudaMemsetAsync(grad_gates, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
-        if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek_gates_bwd_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
-    if (need && (!ws || ws_bytes < need)) {
-        set_error("%dx%d 2D gates backward needs %zu workspace bytes, got %zu", K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!gates_grid_ok(p, K, "backward")) return CSPN_ERR_UNSUPPORTED;
-    if (!grad_gates && !grad_feat) return CSPN_OK;
-    // every gate gradient is written by the gather (g_k(p) feeds pixel p alone; a tap that reads the padding gets 0)
-    if (K == 3) return backward_k<1, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches);
-    return K == 5 ? backward_k<2, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches)
-                  : backward_k<3, true, true>(p, grad_out, grad_gates, grad_feat, ws, stream, launches);
+    const int rc = check_launch(p, K, t, "backward", widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    if (t.no_grad_is_no_op && !grad_guidance && !grad_blur) return CSPN_OK;
+    return with_kernels(K, family, [&](auto R, auto PADDLE, auto RAW) {
+        return backward_k<R(), PADDLE(), RAW()>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+    });
 }
 
 }  // namespace cspn

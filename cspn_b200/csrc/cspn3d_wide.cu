@@ -565,112 +565,84 @@ int backward_gates_3k(const float* gates, const float* feat, const float* grad_o
     return CSPN_OK;
 }
 
-bool grid_ok(int C, int D, int H, const char* what, int K) {
+// K = 3 -> R = 1, K = 5 -> R = 2: f(R) as an integral constant (the gates kernels; the normalised ones exist for R = 2 only)
+template <class F>
+int with_radius(int K, F&& f) {
+    return K == 3 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
+}
+
+const char* name_of(Family family) { return family == Family::Gates ? " gates" : ""; }   // follows "KxKxK 3D" in messages
+
+// The workspace holds what `need` says (nothing, for one step on the caller's gates), and the launch grids take the problem
+int check_launch(int C, int D, int H, int K, Family family, const char* what, size_t need, const void* ws, size_t ws_bytes) {
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("%dx%dx%d 3D%s %s needs %zu workspace bytes, got %zu", K, K, K, name_of(family), what, need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
     if ((long long)D * C > 65535) {
-        set_error("%dx%dx%d 3D %s: D*C=%lld exceeds gridDim.z", K, K, K, what, (long long)D * C);
-        return false;
+        set_error("%dx%dx%d 3D%s %s: D*C=%lld exceeds gridDim.z", K, K, K, name_of(family), what, (long long)D * C);
+        return CSPN_ERR_UNSUPPORTED;
     }
     if ((H + kSclTH - 1) / kSclTH > 65535) {
-        set_error("%dx%dx%d 3D %s: H=%d exceeds gridDim.y", K, K, K, what, H);
-        return false;
+        set_error("%dx%dx%d 3D%s %s: H=%d exceeds gridDim.y", K, K, K, name_of(family), what, H);
+        return CSPN_ERR_UNSUPPORTED;
     }
-    return true;
+    return CSPN_OK;
 }
 
 }  // namespace
 
-size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
+// Normalised (every mode): K^3 weight planes and, past one step, the ping-pong buffer per volume of a group.  Gates: the
+// caller's gates are the weight planes.
+size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters, Family family) {
     if (iters <= 0) return 0;
     const size_t V = (size_t)D * H * W, np = (size_t)K * K * K;
+    if (family == Family::Gates) return iters > 1 ? sizeof(float) * (size_t)gates_group(B, C, D, H, W, iters) * C * V : 0;
     return sizeof(float) * (size_t)group3d(B, C, D, H, W, iters, (int)np) * (np * V + (iters > 1 ? (size_t)C * V : 0));
 }
 
-size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters) {
+// One volume at a time: the weight planes, d_1..d_{N-1} and every lambda_t; gates keep no weight planes and no lambda_0
+size_t widek3d_bwd_workspace_bytes(int C, int D, int H, int W, int K, int iters, Family family) {
     if (iters <= 0) return 0;
     const size_t V = (size_t)D * H * W;
+    if (family == Family::Gates) return sizeof(float) * (2 * (size_t)iters - 2) * C * V;
     return sizeof(float) * ((size_t)K * K * K * V + (2 * (size_t)iters - 1) * C * V);
 }
 
 int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                    int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
+                    Family family, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
     if (iters == 0) {
         CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * D * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = widek3d_workspace_bytes(B, C, D, H, W, K, iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%dx%d 3D path needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!grid_ok(C, D, H, "path", K)) return CSPN_ERR_UNSUPPORTED;
-    return forward_3k<2>(guidance, feat, out, B, C, D, H, W, iters, mode, ws, stream, launches, fan);
+    const int rc = check_launch(C, D, H, K, family, "path", widek3d_workspace_bytes(B, C, D, H, W, K, iters, family), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    if (family != Family::Gates) return forward_3k<2>(guidance, feat, out, B, C, D, H, W, iters, mode, ws, stream, launches, fan);
+    return with_radius(K, [&](auto R) {
+        return forward_gates_3k<R()>(guidance, feat, out, B, C, D, H, W, iters, ws, stream, launches, fan);
+    });
 }
 
 int widek3d_backward(const float* guidance, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B, int C,
-                     int D, int H, int W, int K, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream,
-                     int* launches) {
+                     int D, int H, int W, int K, int iters, Family family, int mode, void* ws, size_t ws_bytes,
+                     cudaStream_t stream, int* launches) {
+    const bool gates = family == Family::Gates;
     const size_t V = (size_t)D * H * W;
-    if (grad_g)   // gathered norms: guidance values that no voxel reads get zero gradient
+    // gathered norms: guidance values that no voxel reads get zero gradient.  Every gate gradient is written by the gathers
+    // (g_k(p) feeds voxel p alone; a tap that reads the padding gets 0), so gates need the fill for the identity only
+    if (grad_g && (!gates || iters == 0))
         CSPN_CUDA_TRY(cudaMemsetAsync(grad_g, 0, (size_t)B * (K * K * K - 1) * V * sizeof(float), stream));
-    if (iters == 0) {
+    if (iters == 0) {   // the identity: no dependence on the guidance
         if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, (size_t)B * C * V * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = widek3d_bwd_workspace_bytes(C, D, H, W, K, iters);
-    if (!ws || ws_bytes < need) {
-        set_error("%dx%dx%d 3D backward needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!grid_ok(C, D, H, "backward", K)) return CSPN_ERR_UNSUPPORTED;
-    return backward_3k<2>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, mode, ws, stream, launches);
-}
-
-// Caller-supplied gates [B][K^3-1][D][H][W], used as given, K in {3, 5}
-size_t widek3d_gates_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
-    if (iters <= 1) return 0;
-    return sizeof(float) * (size_t)gates_group(B, C, D, H, W, iters) * C * D * H * W;
-}
-
-size_t widek3d_gates_bwd_workspace_bytes(int C, int D, int H, int W, int iters) {
-    if (iters <= 1) return 0;
-    return sizeof(float) * (2 * (size_t)iters - 2) * C * D * H * W;
-}
-
-int widek3d_gates_forward(const float* gates, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
-                          void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, const Fan* fan) {
-    if (iters == 0) {
-        CSPN_CUDA_TRY(cudaMemcpyAsync(out, feat, (size_t)B * C * D * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek3d_gates_workspace_bytes(B, C, D, H, W, iters);
-    if (need && (!ws || ws_bytes < need)) {
-        set_error("%dx%dx%d 3D gates path needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!grid_ok(C, D, H, "gates path", K)) return CSPN_ERR_UNSUPPORTED;
-    return K == 3 ? forward_gates_3k<1>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches, fan)
-                  : forward_gates_3k<2>(gates, feat, out, B, C, D, H, W, iters, ws, stream, launches, fan);
-}
-
-int widek3d_gates_backward(const float* gates, const float* feat, const float* grad_out, float* grad_g, float* grad_feat, int B,
-                           int C, int D, int H, int W, int K, int iters, void* ws, size_t ws_bytes, cudaStream_t stream,
-                           int* launches) {
-    const size_t V = (size_t)D * H * W;
-    if (iters == 0) {   // the identity: no dependence on the gates
-        if (grad_g) CSPN_CUDA_TRY(cudaMemsetAsync(grad_g, 0, (size_t)B * (K * K * K - 1) * V * sizeof(float), stream));
-        if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, (size_t)B * C * V * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = widek3d_gates_bwd_workspace_bytes(C, D, H, W, iters);
-    if (need && (!ws || ws_bytes < need)) {
-        set_error("%dx%dx%d 3D gates backward needs %zu workspace bytes, got %zu", K, K, K, need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (!grid_ok(C, D, H, "gates backward", K)) return CSPN_ERR_UNSUPPORTED;
+    const int rc = check_launch(C, D, H, K, family, "backward", widek3d_bwd_workspace_bytes(C, D, H, W, K, iters, family), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    if (!gates) return backward_3k<2>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, mode, ws, stream, launches);
     if (!grad_g && !grad_feat) return CSPN_OK;
-    // every gate gradient is written by the gathers (g_k(p) feeds voxel p alone; a tap that reads the padding gets 0)
-    return K == 3 ? backward_gates_3k<1>(gates, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches)
-                  : backward_gates_3k<2>(gates, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches);
+    return with_radius(K, [&](auto R) {
+        return backward_gates_3k<R()>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches);
+    });
 }
 
 }  // namespace cspn

@@ -49,7 +49,9 @@
 
 namespace {
 
-const float* fptr(const at::Tensor& t) { return t.data_ptr<float>(); }
+// null for an undefined tensor: an absent sparse_depth, a gradient that is not wanted
+const float* fptr(const at::Tensor& t) { return t.defined() ? t.data_ptr<float>() : nullptr; }
+float* mptr(const at::Tensor& t) { return t.defined() ? t.data_ptr<float>() : nullptr; }
 
 void check_rc(int rc, const char* what) {
     if (rc == CSPN_OK) return;
@@ -57,6 +59,32 @@ void check_rc(int rc, const char* what) {
     TORCH_CHECK(rc != CSPN_ERR_INVALID_ARGUMENT, what, ": ", msg);
     TORCH_CHECK(false, what, " failed (status ", rc, "): ", msg);
 }
+
+// The byte workspace a C ABI call asks for, on the device of `like`; no tensor and a null pointer when it asks for none
+struct Workspace {
+    size_t bytes;
+    at::Tensor t;
+    Workspace(size_t bytes, const at::Tensor& like) : bytes(bytes) {
+        if (bytes) t = at::empty({(int64_t)bytes}, like.options().dtype(at::kByte));
+    }
+    void* ptr() const { return bytes ? t.data_ptr() : nullptr; }
+};
+
+cspn_stream_t current_stream() { return (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream(); }
+
+void check_grad_out(const at::Tensor& grad_out, const at::Tensor& x, const char* name) {
+    TORCH_CHECK(grad_out.sizes() == x.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == x.device(),
+                "grad_out must match ", name);
+}
+
+// The gradient of x: allocated when wanted, undefined otherwise.  An unused gradient is returned as an empty tensor (the
+// Python autograd formula maps it to None).
+at::Tensor new_grad(bool need, const at::Tensor& x) { return need ? at::empty_like(x) : at::Tensor(); }
+at::Tensor grad_or_empty(const at::Tensor& grad, const at::Tensor& x) { return grad.defined() ? grad : at::zeros({0}, x.options()); }
+
+// Neighbours of a kernel of size K in nd dimensions, and the sizes the kernels exist for
+int64_t neighbours(int64_t K, int nd) { return (nd == 2 ? K * K : K * K * K) - 1; }
+bool kernel_size_ok(int64_t K, int nd) { return K == 3 || K == 5 || (nd == 2 && K == 7); }
 
 void check2d(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse) {
     TORCH_CHECK(guidance.dim() == 4 && blur.dim() == 4, "guidance and blur_depth must be (B,C,H,W)");
@@ -87,12 +115,9 @@ at::Tensor propagate2d_cuda(const at::Tensor& guidance, const at::Tensor& blur, 
     int a = (int)algo;
     auto misaligned = [](const at::Tensor& t) { return t.defined() && (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0; };
     if (a == CSPN_ALGO_AUTO && (misaligned(g) || misaligned(d) || misaligned(s) || misaligned(out))) a = CSPN_ALGO_GENERIC;
-    const size_t ws_bytes = cspn2d_workspace_bytes(B, C, H, W, (int)prop_time, a);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
-    check_rc(cspn2d_fwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, out.data_ptr<float>(), B, C, H, W, (int)g.size(1),
-                            (int)prop_time, (int)norm_type, a, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                            (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_workspace_bytes(B, C, H, W, (int)prop_time, a), d);
+    check_rc(cspn2d_fwd_f32(fptr(g), fptr(d), fptr(s), mptr(out), B, C, H, W, (int)g.size(1), (int)prop_time, (int)norm_type, a,
+                            ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_fwd_f32");
     return out;
 }
@@ -101,36 +126,30 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_backward_cuda(const at::Tensor& g
                                                              const std::optional<at::Tensor>& sparse, const at::Tensor& grad_out,
                                                              int64_t prop_time, int64_t norm_type, bool need_g, bool need_d) {
     check2d(guidance, blur, sparse);
-    TORCH_CHECK(grad_out.sizes() == blur.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == blur.device(),
-                "grad_out must match blur_depth");
+    check_grad_out(grad_out, blur, "blur_depth");
     const c10::cuda::CUDAGuard guard(blur.device());
     const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
     const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    at::Tensor gd = need_d ? at::empty_like(d) : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gd = new_grad(need_d, d);
     if (prop_time == 0) {                              // identity: d out / d blur = 1, no dependence on the guidance
         if (need_g) gg.zero_();
         if (need_d) gd.copy_(go);
-        return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
+        return {grad_or_empty(gg, g), grad_or_empty(gd, d)};
     }
     const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
-    const size_t ws_bytes = cspn2d_bwd_workspace_bytes(B, C, H, W, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
-    check_rc(cspn2d_bwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
-                            need_d ? gd.data_ptr<float>() : nullptr, B, C, H, W, (int)g.size(1), (int)prop_time, (int)norm_type,
-                            ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_bwd_workspace_bytes(B, C, H, W, (int)prop_time), d);
+    check_rc(cspn2d_bwd_f32(fptr(g), fptr(d), fptr(s), fptr(go), mptr(gg), mptr(gd), B, C, H, W, (int)g.size(1), (int)prop_time,
+                            (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_bwd_f32");
-    // an unused gradient is returned as an empty tensor (the Python autograd formula maps it to None)
-    return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
+    return {grad_or_empty(gg, g), grad_or_empty(gd, d)};
 }
 
 // K x K kernels: K = 3 is the 3x3 operator above (same kernels, same bits); K = 5 / 7 go through cspn2d_k_*_f32
 void check2d_k(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse, int64_t K) {
-    TORCH_CHECK(K == 3 || K == 5 || K == 7, "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK(kernel_size_ok(K, 2), "kernel_size must be 3, 5 or 7, got ", K);
     check2d(guidance, blur, sparse);
-    TORCH_CHECK(guidance.size(1) >= K * K - 1, "a ", K, "x", K, " kernel needs guidance (B,>=", K * K - 1, ",H,W), got ",
-                guidance.sizes());
+    TORCH_CHECK(guidance.size(1) >= neighbours(K, 2), "a ", K, "x", K, " kernel needs guidance (B,>=", neighbours(K, 2),
+                ",H,W), got ", guidance.sizes());
 }
 
 at::Tensor propagate2d_k_cuda(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
@@ -143,12 +162,9 @@ at::Tensor propagate2d_k_cuda(const at::Tensor& guidance, const at::Tensor& blur
     const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
     at::Tensor out = at::empty_like(d);
     const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
-    const size_t ws_bytes = cspn2d_k_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
-    check_rc(cspn2d_k_fwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, out.data_ptr<float>(), B, C, H, W,
-                              (int)g.size(1), (int)K, (int)prop_time, (int)norm_type, ws_bytes ? ws.data_ptr() : nullptr,
-                              ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_k_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), d);
+    check_rc(cspn2d_k_fwd_f32(fptr(g), fptr(d), fptr(s), mptr(out), B, C, H, W, (int)g.size(1), (int)K, (int)prop_time,
+                              (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_k_fwd_f32");
     return out;
 }
@@ -159,33 +175,27 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_k_backward_cuda(const at::Tensor&
                                                                bool need_d) {
     check2d_k(guidance, blur, sparse, K);
     if (K == 3) return propagate2d_backward_cuda(guidance, blur, sparse, grad_out, prop_time, norm_type, need_g, need_d);
-    TORCH_CHECK(grad_out.sizes() == blur.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == blur.device(),
-                "grad_out must match blur_depth");
+    check_grad_out(grad_out, blur, "blur_depth");
     const c10::cuda::CUDAGuard guard(blur.device());
     const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
     const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    at::Tensor gd = need_d ? at::empty_like(d) : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gd = new_grad(need_d, d);
     const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
-    const size_t ws_bytes = cspn2d_k_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, d.options().dtype(at::kByte));
-    check_rc(cspn2d_k_bwd_f32(fptr(g), fptr(d), s.defined() ? fptr(s) : nullptr, fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
-                              need_d ? gd.data_ptr<float>() : nullptr, B, C, H, W, (int)g.size(1), (int)K, (int)prop_time,
-                              (int)norm_type, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                              (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_k_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), d);
+    check_rc(cspn2d_k_bwd_f32(fptr(g), fptr(d), fptr(s), fptr(go), mptr(gg), mptr(gd), B, C, H, W, (int)g.size(1), (int)K,
+                              (int)prop_time, (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_k_bwd_f32");
-    return {need_g ? gg : at::zeros({0}, g.options()), need_d ? gd : at::zeros({0}, d.options())};
+    return {grad_or_empty(gg, g), grad_or_empty(gd, d)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
 // (B, (K*K-1)*C, H, W) with C > 1 gives channel c its own gate (demo.py:28-45), which in memory is B*C images of one
 // channel.  Returns the (images, channels) the C ABI is called with.
 std::pair<int, int> check2d_paddle(const at::Tensor& guidance, const at::Tensor& feat, int64_t K) {
-    TORCH_CHECK_VALUE(K == 3 || K == 5 || K == 7, "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK_VALUE(kernel_size_ok(K, 2), "kernel_size must be 3, 5 or 7, got ", K);
     TORCH_CHECK_VALUE(guidance.dim() == 4 && feat.dim() == 4, "guidance and feat must be (B,C,H,W)");
     TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
-    const int64_t nt = K * K - 1, B = feat.size(0), C = feat.size(1);
+    const int64_t nt = neighbours(K, 2), B = feat.size(0), C = feat.size(1);
     const bool shape_ok = guidance.size(0) == B && guidance.size(2) == feat.size(2) && guidance.size(3) == feat.size(3);
     const bool per_channel = C > 1 && guidance.size(1) == nt * C;
     TORCH_CHECK_VALUE(shape_ok && (guidance.size(1) == nt || per_channel), "a ", K, "x", K, " 'paddle' kernel needs guidance (B,",
@@ -202,11 +212,9 @@ at::Tensor propagate2d_paddle_cuda(const at::Tensor& guidance, const at::Tensor&
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous();
     at::Tensor out = at::empty_like(f);
     const int H = (int)f.size(2), W = (int)f.size(3);
-    const size_t ws_bytes = cspn2d_paddle_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn2d_paddle_fwd_f32(fptr(g), fptr(f), out.data_ptr<float>(), B, C, H, W, (int)K, (int)prop_time,
-                                   ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_paddle_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), f);
+    check_rc(cspn2d_paddle_fwd_f32(fptr(g), fptr(f), mptr(out), B, C, H, W, (int)K, (int)prop_time, ws.ptr(), ws.bytes,
+                                   current_stream()),
              "cspn2d_paddle_fwd_f32");
     return out;
 }
@@ -215,21 +223,16 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_paddle_backward_cuda(const at::Te
                                                                     const at::Tensor& grad_out, int64_t K, int64_t prop_time,
                                                                     bool need_g, bool need_f) {
     const auto [B, C] = check2d_paddle(guidance, feat, K);
-    TORCH_CHECK(grad_out.sizes() == feat.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == feat.device(),
-                "grad_out must match feat");
+    check_grad_out(grad_out, feat, "feat");
     const c10::cuda::CUDAGuard guard(feat.device());
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous(), go = grad_out.contiguous();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    at::Tensor gf = need_f ? at::empty_like(f) : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gf = new_grad(need_f, f);
     const int H = (int)f.size(2), W = (int)f.size(3);
-    const size_t ws_bytes = cspn2d_paddle_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn2d_paddle_bwd_f32(fptr(g), fptr(f), fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
-                                   need_f ? gf.data_ptr<float>() : nullptr, B, C, H, W, (int)K, (int)prop_time,
-                                   ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn2d_paddle_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), f);
+    check_rc(cspn2d_paddle_bwd_f32(fptr(g), fptr(f), fptr(go), mptr(gg), mptr(gf), B, C, H, W, (int)K, (int)prop_time, ws.ptr(),
+                                   ws.bytes, current_stream()),
              "cspn2d_paddle_bwd_f32");
-    return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+    return {grad_or_empty(gg, g), grad_or_empty(gf, f)};
 }
 
 void check3d(const at::Tensor& guidance, const at::Tensor& feat) {
@@ -248,11 +251,9 @@ at::Tensor propagate3d_cuda(const at::Tensor& guidance, const at::Tensor& feat, 
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous();
     at::Tensor out = at::empty_like(f);
     const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
-    const size_t ws_bytes = cspn3d_workspace_bytes(B, C, D, H, W, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn3d_fwd_f32(fptr(g), fptr(f), out.data_ptr<float>(), B, C, D, H, W, (int)prop_time, (int)norm_type,
-                            ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn3d_workspace_bytes(B, C, D, H, W, (int)prop_time), f);
+    check_rc(cspn3d_fwd_f32(fptr(g), fptr(f), mptr(out), B, C, D, H, W, (int)prop_time, (int)norm_type, ws.ptr(), ws.bytes,
+                            current_stream()),
              "cspn3d_fwd_f32");
     return out;
 }
@@ -261,34 +262,29 @@ std::tuple<at::Tensor, at::Tensor> propagate3d_backward_cuda(const at::Tensor& g
                                                              const at::Tensor& grad_out, int64_t prop_time, int64_t norm_type,
                                                              bool need_g, bool need_f) {
     check3d(guidance, feat);
-    TORCH_CHECK(grad_out.sizes() == feat.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == feat.device(),
-                "grad_out must match feat");
+    check_grad_out(grad_out, feat, "feat");
     const c10::cuda::CUDAGuard guard(feat.device());
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous(), go = grad_out.contiguous();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    at::Tensor gf = need_f ? at::empty_like(f) : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gf = new_grad(need_f, f);
     if (prop_time == 0) {
         if (need_g) gg.zero_();
         if (need_f) gf.copy_(go);
-        return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+        return {grad_or_empty(gg, g), grad_or_empty(gf, f)};
     }
     const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
-    const size_t ws_bytes = cspn3d_bwd_workspace_bytes(B, C, D, H, W, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn3d_bwd_f32(fptr(g), fptr(f), fptr(go), need_g ? gg.data_ptr<float>() : nullptr, need_f ? gf.data_ptr<float>() : nullptr,
-                            B, C, D, H, W, (int)prop_time, (int)norm_type, ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                            (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn3d_bwd_workspace_bytes(B, C, D, H, W, (int)prop_time), f);
+    check_rc(cspn3d_bwd_f32(fptr(g), fptr(f), fptr(go), mptr(gg), mptr(gf), B, C, D, H, W, (int)prop_time, (int)norm_type,
+                            ws.ptr(), ws.bytes, current_stream()),
              "cspn3d_bwd_f32");
-    return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+    return {grad_or_empty(gg, g), grad_or_empty(gf, f)};
 }
 
 // K x K x K kernels: K = 3 is the 3D operator above (same kernels, same bits); K = 5 goes through cspn3d_k_*_f32
 void check3d_k(const at::Tensor& guidance, const at::Tensor& feat, int64_t K) {
-    TORCH_CHECK_VALUE(K == 3 || K == 5, "3D kernel_size must be 3 or 5, got ", K);
+    TORCH_CHECK_VALUE(kernel_size_ok(K, 3), "3D kernel_size must be 3 or 5, got ", K);
     TORCH_CHECK_VALUE(guidance.dim() == 5 && feat.dim() == 5, "guidance and feat must be (B,C,D,H,W)");
     TORCH_CHECK(guidance.scalar_type() == at::kFloat && feat.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
-    const int64_t nt = K * K * K - 1;
+    const int64_t nt = neighbours(K, 3);
     TORCH_CHECK_VALUE(guidance.size(0) == feat.size(0) && guidance.size(1) == nt && guidance.size(2) == feat.size(2) &&
                           guidance.size(3) == feat.size(3) && guidance.size(4) == feat.size(4),
                       "a ", K, "x", K, "x", K, " kernel needs guidance (B,", nt, ",D,H,W), got ", guidance.sizes(), " for feat ",
@@ -304,11 +300,9 @@ at::Tensor propagate3d_k_cuda(const at::Tensor& guidance, const at::Tensor& feat
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous();
     at::Tensor out = at::empty_like(f);
     const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
-    const size_t ws_bytes = cspn3d_k_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn3d_k_fwd_f32(fptr(g), fptr(f), out.data_ptr<float>(), B, C, D, H, W, (int)K, (int)prop_time, (int)norm_type,
-                              ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn3d_k_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time), f);
+    check_rc(cspn3d_k_fwd_f32(fptr(g), fptr(f), mptr(out), B, C, D, H, W, (int)K, (int)prop_time, (int)norm_type, ws.ptr(),
+                              ws.bytes, current_stream()),
              "cspn3d_k_fwd_f32");
     return out;
 }
@@ -318,21 +312,16 @@ std::tuple<at::Tensor, at::Tensor> propagate3d_k_backward_cuda(const at::Tensor&
                                                                int64_t norm_type, bool need_g, bool need_f) {
     check3d_k(guidance, feat, K);
     if (K == 3) return propagate3d_backward_cuda(guidance, feat, grad_out, prop_time, norm_type, need_g, need_f);
-    TORCH_CHECK(grad_out.sizes() == feat.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == feat.device(),
-                "grad_out must match feat");
+    check_grad_out(grad_out, feat, "feat");
     const c10::cuda::CUDAGuard guard(feat.device());
     const at::Tensor g = guidance.contiguous(), f = feat.contiguous(), go = grad_out.contiguous();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    at::Tensor gf = need_f ? at::empty_like(f) : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gf = new_grad(need_f, f);
     const int B = (int)f.size(0), C = (int)f.size(1), D = (int)f.size(2), H = (int)f.size(3), W = (int)f.size(4);
-    const size_t ws_bytes = cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, f.options().dtype(at::kByte));
-    check_rc(cspn3d_k_bwd_f32(fptr(g), fptr(f), fptr(go), need_g ? gg.data_ptr<float>() : nullptr,
-                              need_f ? gf.data_ptr<float>() : nullptr, B, C, D, H, W, (int)K, (int)prop_time, (int)norm_type,
-                              ws_bytes ? ws.data_ptr() : nullptr, ws_bytes, (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    const Workspace ws(cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_time), f);
+    check_rc(cspn3d_k_bwd_f32(fptr(g), fptr(f), fptr(go), mptr(gg), mptr(gf), B, C, D, H, W, (int)K, (int)prop_time,
+                              (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn3d_k_bwd_f32");
-    return {need_g ? gg : at::zeros({0}, g.options()), need_f ? gf : at::zeros({0}, f.options())};
+    return {grad_or_empty(gg, g), grad_or_empty(gf, f)};
 }
 
 // caller-supplied gates (fluid.layers.affinity_propagate), nd = 2 (K in {3, 5, 7}) or 3 (K in {3, 5}).  Returns the
@@ -340,11 +329,11 @@ std::tuple<at::Tensor, at::Tensor> propagate3d_k_backward_cuda(const at::Tensor&
 std::pair<int, int> check_gates(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step, int nd) {
     TORCH_CHECK_VALUE(input.dim() == nd + 2 && gate.dim() == nd + 2, "input and gate_weight must be ",
                       nd == 2 ? "(B,C,H,W)" : "(B,C,D,H,W)");
-    TORCH_CHECK_VALUE(nd == 2 ? (K == 3 || K == 5 || K == 7) : (K == 3 || K == 5), "kernel_size of a ", nd,
-                      "D affinity_propagate must be ", nd == 2 ? "3, 5 or 7" : "3 or 5", ", got ", K);
+    TORCH_CHECK_VALUE(kernel_size_ok(K, nd), "kernel_size of a ", nd, "D affinity_propagate must be ",
+                      nd == 2 ? "3, 5 or 7" : "3 or 5", ", got ", K);
     TORCH_CHECK_VALUE(prop_step >= 0, "prop_step must be >= 0, got ", prop_step);
     TORCH_CHECK(input.scalar_type() == at::kFloat && gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
-    const int64_t nt = (nd == 2 ? K * K : K * K * K) - 1, B = input.size(0), C = input.size(1);
+    const int64_t nt = neighbours(K, nd), B = input.size(0), C = input.size(1);
     bool shape_ok = gate.size(0) == B;
     for (int i = 2; i < nd + 2; ++i) shape_ok = shape_ok && gate.size(i) == input.size(i);
     const bool per_channel = C > 1 && gate.size(1) == nt * C;
@@ -360,19 +349,17 @@ at::Tensor affinity_propagate_cuda(const at::Tensor& input, const at::Tensor& ga
     const c10::cuda::CUDAGuard guard(input.device());
     const at::Tensor g = gate.contiguous(), x = input.contiguous();
     at::Tensor out = at::empty_like(x);
-    const auto stream = (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream();
     const int H = (int)x.size(nd), W = (int)x.size(nd + 1), D = nd == 3 ? (int)x.size(2) : 1;
-    const size_t ws_bytes = nd == 2 ? cspn2d_gates_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
-                                    : cspn3d_gates_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, x.options().dtype(at::kByte));
-    void* w = ws_bytes ? ws.data_ptr() : nullptr;
+    const Workspace ws(nd == 2 ? cspn2d_gates_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
+                               : cspn3d_gates_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step),
+                       x);
     if (nd == 2)
-        check_rc(cspn2d_gates_fwd_f32(fptr(g), fptr(x), out.data_ptr<float>(), B, C, H, W, (int)K, (int)prop_step, w, ws_bytes, stream),
+        check_rc(cspn2d_gates_fwd_f32(fptr(g), fptr(x), mptr(out), B, C, H, W, (int)K, (int)prop_step, ws.ptr(), ws.bytes,
+                                      current_stream()),
                  "cspn2d_gates_fwd_f32");
     else
-        check_rc(cspn3d_gates_fwd_f32(fptr(g), fptr(x), out.data_ptr<float>(), B, C, D, H, W, (int)K, (int)prop_step, w, ws_bytes,
-                                      stream),
+        check_rc(cspn3d_gates_fwd_f32(fptr(g), fptr(x), mptr(out), B, C, D, H, W, (int)K, (int)prop_step, ws.ptr(), ws.bytes,
+                                      current_stream()),
                  "cspn3d_gates_fwd_f32");
     return out;
 }
@@ -381,29 +368,23 @@ std::tuple<at::Tensor, at::Tensor> affinity_propagate_backward_cuda(const at::Te
                                                                     const at::Tensor& grad_out, int64_t K, int64_t prop_step,
                                                                     bool need_x, bool need_g, int nd) {
     const auto [B, C] = check_gates(input, gate, K, prop_step, nd);
-    TORCH_CHECK(grad_out.sizes() == input.sizes() && grad_out.scalar_type() == at::kFloat && grad_out.device() == input.device(),
-                "grad_out must match input");
+    check_grad_out(grad_out, input, "input");
     const c10::cuda::CUDAGuard guard(input.device());
     const at::Tensor g = gate.contiguous(), x = input.contiguous(), go = grad_out.contiguous();
-    at::Tensor gx = need_x ? at::empty_like(x) : at::Tensor();
-    at::Tensor gg = need_g ? at::empty_like(g) : at::Tensor();
-    const auto stream = (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream();
+    at::Tensor gx = new_grad(need_x, x), gg = new_grad(need_g, g);
     const int H = (int)x.size(nd), W = (int)x.size(nd + 1), D = nd == 3 ? (int)x.size(2) : 1;
-    const size_t ws_bytes = nd == 2 ? cspn2d_gates_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
-                                    : cspn3d_gates_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step);
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, x.options().dtype(at::kByte));
-    void* w = ws_bytes ? ws.data_ptr() : nullptr;
-    float* pgg = need_g ? gg.data_ptr<float>() : nullptr;
-    float* pgx = need_x ? gx.data_ptr<float>() : nullptr;
+    const Workspace ws(nd == 2 ? cspn2d_gates_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_step)
+                               : cspn3d_gates_bwd_workspace_bytes(B, C, D, H, W, (int)K, (int)prop_step),
+                       x);
     if (nd == 2)
-        check_rc(cspn2d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), pgg, pgx, B, C, H, W, (int)K, (int)prop_step, w, ws_bytes, stream),
+        check_rc(cspn2d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), mptr(gg), mptr(gx), B, C, H, W, (int)K, (int)prop_step, ws.ptr(),
+                                      ws.bytes, current_stream()),
                  "cspn2d_gates_bwd_f32");
     else
-        check_rc(cspn3d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), pgg, pgx, B, C, D, H, W, (int)K, (int)prop_step, w, ws_bytes,
-                                      stream),
+        check_rc(cspn3d_gates_bwd_f32(fptr(g), fptr(x), fptr(go), mptr(gg), mptr(gx), B, C, D, H, W, (int)K, (int)prop_step,
+                                      ws.ptr(), ws.bytes, current_stream()),
                  "cspn3d_gates_bwd_f32");
-    return {need_x ? gx : at::zeros({0}, x.options()), need_g ? gg : at::zeros({0}, g.options())};
+    return {grad_or_empty(gx, x), grad_or_empty(gg, g)};
 }
 
 at::Tensor affinity_propagate2d_cuda(const at::Tensor& input, const at::Tensor& gate, int64_t K, int64_t prop_step) {
@@ -438,9 +419,8 @@ at::Tensor unpool_conv3x3_cuda(const at::Tensor& x, const at::Tensor& weight, in
     const c10::cuda::CUDAGuard guard(x.device());
     const at::Tensor xc = x.contiguous(), wc = weight.contiguous();
     at::Tensor out = at::empty({xc.size(0), wc.size(0), H, W}, xc.options());
-    check_rc(cspn_unpool_conv3x3_fwd_f32(fptr(xc), fptr(wc), out.data_ptr<float>(), (int)xc.size(0), (int)xc.size(1), (int)xc.size(2),
-                                         (int)xc.size(3), (int)wc.size(0), (int)H, (int)W,
-                                         (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+    check_rc(cspn_unpool_conv3x3_fwd_f32(fptr(xc), fptr(wc), mptr(out), (int)xc.size(0), (int)xc.size(1), (int)xc.size(2),
+                                         (int)xc.size(3), (int)wc.size(0), (int)H, (int)W, current_stream()),
              "cspn_unpool_conv3x3_fwd_f32");
     return out;
 }
@@ -454,19 +434,14 @@ std::tuple<at::Tensor, at::Tensor> unpool_conv3x3_backward_cuda(const at::Tensor
                 "grad_out must be (B,Cout,H,W) fp32 on the device of x, got ", grad_out.sizes());
     const c10::cuda::CUDAGuard guard(x.device());
     const at::Tensor xc = x.contiguous(), wc = weight.contiguous(), go = grad_out.contiguous();
-    at::Tensor gx = need_x ? at::empty_like(xc) : at::Tensor();
-    at::Tensor gw = need_w ? at::empty_like(wc) : at::Tensor();
+    at::Tensor gx = new_grad(need_x, xc), gw = new_grad(need_w, wc);
     const int B = (int)xc.size(0), Cin = (int)xc.size(1), h = (int)xc.size(2), w = (int)xc.size(3), Cout = (int)wc.size(0);
-    const size_t ws_bytes = need_w ? cspn_unpool_conv3x3_bwd_workspace_bytes(B, Cin, h, w, Cout, (int)H, (int)W) : 0;
-    at::Tensor ws;
-    if (ws_bytes) ws = at::empty({(int64_t)ws_bytes}, xc.options().dtype(at::kByte));
+    const Workspace ws(need_w ? cspn_unpool_conv3x3_bwd_workspace_bytes(B, Cin, h, w, Cout, (int)H, (int)W) : 0, xc);
     if (need_x || need_w)
-        check_rc(cspn_unpool_conv3x3_bwd_f32(fptr(xc), fptr(wc), fptr(go), need_x ? gx.data_ptr<float>() : nullptr,
-                                             need_w ? gw.data_ptr<float>() : nullptr, B, Cin, h, w, Cout, (int)H, (int)W,
-                                             ws_bytes ? ws.data_ptr() : nullptr, ws_bytes,
-                                             (cspn_stream_t)c10::cuda::getCurrentCUDAStream().stream()),
+        check_rc(cspn_unpool_conv3x3_bwd_f32(fptr(xc), fptr(wc), fptr(go), mptr(gx), mptr(gw), B, Cin, h, w, Cout, (int)H, (int)W,
+                                             ws.ptr(), ws.bytes, current_stream()),
                  "cspn_unpool_conv3x3_bwd_f32");
-    return {need_x ? gx : at::zeros({0}, xc.options()), need_w ? gw : at::zeros({0}, wc.options())};
+    return {grad_or_empty(gx, xc), grad_or_empty(gw, wc)};
 }
 
 }  // namespace

@@ -106,6 +106,17 @@ def test_c_abi_rejects_bad_arguments_without_a_device():
     assert f(o=None) == -1 and b(go=None) == -1
     assert b'null' in L.cspn_last_error()
 
+    def b3(g=p, d=p, go=p, **over):     # the 3x3x3 backward names the offending argument like its siblings
+        a = dict(ok_args, **over)
+        rc = L.cspn3d_bwd_f32(g, d, go, p, p, a['B'], a['C'], a['D'], a['H'], a['W'], a['iters'], a['norm'], None, 0, None)
+        return rc, L.cspn_last_error()
+
+    for kw, msg in ([(dict(g=None), b'null'), (dict(d=None), b'null'), (dict(go=None), b'null'), (dict(iters=-1), b'>= 0')] +
+                    [({dim: v}, b'non-positive shape') for dim in ('B', 'C', 'D', 'H', 'W') for v in (0, -3)] +
+                    [(dict(norm=n), b'unknown 3D norm_type') for n in (-1, 3, 7)]):
+        rc, err = b3(**kw)
+        assert rc == -1 and msg in err, (kw, rc, err)
+
 
 def test_workspace_formulas():
     L = _lib.lib()
