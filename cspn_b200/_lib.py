@@ -28,6 +28,11 @@ SIGNATURES = {
     'cspn2d_k_fwd_gather_f32': (_i, [_vp] * 5 + [_i, _vp] + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn2d_k_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_k_bwd_f32': (_i, [_vp] * 6 + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn2d_keep_workspace_bytes': (_sz, [_i] * 7),
+    'cspn2d_keep_fwd_f32': (_i, [_vp] * 4 + [_i] * 9 + [_vp, _sz, _vp]),
+    'cspn2d_keep_fwd_gather_f32': (_i, [_vp] * 5 + [_i, _vp] + [_i] * 8 + [_vp, _sz, _vp]),
+    'cspn2d_keep_bwd_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_keep_bwd_f32': (_i, [_vp] * 7 + [_i] * 8 + [_vp, _sz, _vp]),
     'cspn2d_paddle_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_paddle_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_paddle_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 6 + [_vp, _sz, _vp]),

@@ -63,12 +63,17 @@ def _check_out(out, like, *inputs):
             raise ValueError('`out` must not alias an input tensor')
 
 
-def propagate2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum', algo=ALGO_AUTO, out=None):
+def propagate2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum', algo=ALGO_AUTO, out=None,
+                keep_sparse=False):
     """Forward only, no autograd.  CUDA tensors: enqueued on the current stream of their device.
     CPU tensors: shipped through the library's chunked H2D/compute/D2H pipeline on cuda:0
     (the C ABI's host-buffer entry point) -- still the GPU kernels, never a CPU implementation.
     `out` (optional) receives the result instead of a freshly allocated tensor: same shape/dtype/device as
-    blur_depth, contiguous (serving loops reuse one pinned buffer: allocating 55 MB of pinned memory costs milliseconds)."""
+    blur_depth, contiguous (serving loops reuse one pinned buffer: allocating 55 MB of pinned memory costs milliseconds).
+    keep_sparse=True: the CSPN paper's replacement step, which keeps the samples in the output (DESIGN.md section 4.13;
+    CUDA tensors only)."""
+    if keep_sparse:
+        return _propagate2d_keep(guidance, blur_depth, sparse_depth, 3, prop_time, NORM2D[norm_type], algo, out)
     _check_inputs_2d(guidance, blur_depth, sparse_depth)
     if prop_time == 0:
         if out is None:
@@ -103,6 +108,87 @@ def propagate2d(guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type
                               NORM2D[norm_type], algo, _ptr(ws), ws_bytes, _stream(d.device))
     _lib.check(rc, 'cspn2d_fwd_f32')
     return out
+
+
+def _propagate2d_keep(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo=ALGO_AUTO, out=None):
+    """The keep-sparse mode (cspn2d_keep_fwd_f32), forward only: m = 1[sparse_depth > 0], and every step sets
+    d <- (1 - m) d + m sparse_depth, so the result passes through the samples.  CUDA tensors only."""
+    nt = prop_kernel * prop_kernel - 1
+    if guidance.dim() == 4 and guidance.shape[1] < nt:
+        raise ValueError(f'a {prop_kernel}x{prop_kernel} kernel needs guidance (B,>={nt},H,W), got {tuple(guidance.shape)}')
+    _check_inputs_2d(guidance, blur_depth, sparse_depth)
+    if not (guidance.is_cuda and blur_depth.is_cuda and (sparse_depth is None or sparse_depth.is_cuda)):
+        raise _lib.CspnError('keep_sparse takes CUDA tensors only (there is no host-buffer entry point for it)')
+    if prop_time == 0:
+        if out is None:
+            return blur_depth
+        _check_out(out, blur_depth, guidance, sparse_depth)
+        out.copy_(blur_depth)
+        return out
+    L = _lib.lib()
+    B, C, H, W = blur_depth.shape
+    g, d = guidance.contiguous(), blur_depth.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    if out is None:
+        out = torch.empty_like(d)
+    _check_out(out, d, g, s)
+    if algo == ALGO_AUTO and any(t is not None and t.data_ptr() % 16 for t in (g, d, s, out)):
+        algo = ALGO_GENERIC   # views at odd storage offsets: the cluster kernel's TMA / float4 accesses need 16-byte bases
+    with torch.cuda.device(d.device):
+        ws_bytes = L.cspn2d_keep_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time), algo)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+        rc = L.cspn2d_keep_fwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(out), B, C, H, W, g.shape[1], prop_kernel, int(prop_time),
+                                   code, algo, _ptr(ws), ws_bytes, _stream(d.device))
+    _lib.check(rc, 'cspn2d_keep_fwd_f32')
+    return out
+
+
+class _Propagate2dKeepFn(torch.autograd.Function):
+    """autograd seam of the keep-sparse mode without the torch-op shim: native forward + native adjoint
+    (cspn2d_keep_bwd_f32), differentiable in guidance, blur_depth and sparse_depth."""
+
+    @staticmethod
+    def forward(ctx, guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo):
+        ctx.save_for_backward(guidance, blur_depth, sparse_depth)
+        ctx.cfg = (prop_kernel, prop_time, code)
+        return _propagate2d_keep(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        guidance, blur_depth, sparse_depth = ctx.saved_tensors
+        prop_kernel, prop_time, code = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        B, C, H, W = blur_depth.shape
+        g, d, go = guidance.contiguous(), blur_depth.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        need_g, need_d, need_s = ctx.needs_input_grad[:3]
+        gg = torch.empty_like(g) if need_g else None
+        gd = torch.empty_like(d) if need_d else None
+        gs = torch.empty_like(s) if need_s and s is not None else None
+        with torch.cuda.device(d.device):
+            ws_bytes = L.cspn2d_keep_bwd_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+            rc = L.cspn2d_keep_bwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(go), _ptr(gg), _ptr(gd), _ptr(gs), B, C, H, W, g.shape[1],
+                                       prop_kernel, int(prop_time), code, _ptr(ws), ws_bytes, _stream(d.device))
+        _lib.check(rc, 'cspn2d_keep_bwd_f32')
+        return gg, gd, gs, None, None, None, None
+
+
+def _keep_forward(use_op, guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo):
+    """The keep-sparse forward of the modules: the registered op, else the ctypes autograd seam; sparse_depth is not
+    detached (its gradient is m * sum_c Gc_c)."""
+    if prop_time == 0:
+        return blur_depth
+    if not blur_depth.is_cuda:
+        raise _lib.CspnError('keep_sparse takes CUDA tensors only (there is no host-buffer entry point for it)')
+    if use_op:
+        return torch.ops.cspn_b200.propagate2d_keep(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (guidance, blur_depth, sparse_depth)):
+        return _Propagate2dKeepFn.apply(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo)
+    return _propagate2d_keep(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, algo)
 
 
 class _Propagate2dFn(torch.autograd.Function):
@@ -150,7 +236,7 @@ def _use_torch_op():
 class Affinity_Propagate(nn.Module):
     """Same surface as the reference class (cspn.py:14-39): no parameters, no buffers."""
 
-    def __init__(self, prop_time, prop_kernel, norm_type='8sum', algo=ALGO_AUTO):
+    def __init__(self, prop_time, prop_kernel, norm_type='8sum', algo=ALGO_AUTO, keep_sparse=False):
         super(Affinity_Propagate, self).__init__()
         self.prop_time = prop_time
         self.prop_kernel = prop_kernel
@@ -160,12 +246,18 @@ class Affinity_Propagate(nn.Module):
         self.in_feature = 1
         self.out_feature = 1
         self.algo = algo
+        # keep_sparse: the CSPN paper's replacement step, d <- (1 - m) d + m sparse_depth with m = 1[sparse_depth > 0], so
+        # the output passes through the samples (DESIGN.md section 4.13); the reference module replaces with blur_depth
+        self.keep_sparse = keep_sparse
         # torch.ops.cspn_b200.propagate2d (csrc/torch_op.cpp) when the shim is built: one dispatcher op with fake kernel
         # and autograd formula, so torch.compile / export trace through the module.  Same C ABI underneath; without the
         # shim the ctypes binding below is used (still the CUDA kernels -- there is no non-native path).
         self._use_op = _use_torch_op()
 
     def forward(self, guidance, blur_depth, sparse_depth=None):
+        if self.keep_sparse:
+            return _keep_forward(self._use_op, guidance, blur_depth, sparse_depth, 3, self.prop_time, NORM2D[self.norm_type],
+                                 self.algo)
         if self._use_op and blur_depth.is_cuda and self.prop_time > 0:
             sd = None if sparse_depth is None else sparse_depth.detach()   # train.py never differentiates it (:351 clones the input)
             return torch.ops.cspn_b200.propagate2d(guidance, blur_depth, sd, self.prop_time, NORM2D[self.norm_type], self.algo)
@@ -176,7 +268,8 @@ class Affinity_Propagate(nn.Module):
         return propagate2d(guidance, blur_depth, sparse_depth, self.prop_time, self.norm_type, self.algo)
 
     def extra_repr(self):
-        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'
+        keep = ', keep_sparse=True' if self.keep_sparse else ''
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}{keep}'
 
 
 def propagate3d(guidance, feat, prop_time=12, norm_type='26sum_abs'):
@@ -306,11 +399,15 @@ def _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel):
                              '(there is no host-buffer entry point for it)')
 
 
-def propagate2d_k(guidance, blur_depth, sparse_depth=None, prop_kernel=5, prop_time=24, norm_type=None, out=None):
+def propagate2d_k(guidance, blur_depth, sparse_depth=None, prop_kernel=5, prop_time=24, norm_type=None, out=None,
+                  keep_sparse=False):
     """2D CSPN with a K x K affinity kernel, forward only (no autograd), CUDA tensors only, enqueued on the current stream.
     guidance (B, >=K*K-1, H, W): channels 0..K*K-2 are used, shared by the C channels of blur_depth (B, C, H, W);
-    norm_type f'{K*K-1}sum' (default) or f'{K*K-1}sum_abs'.  K = 3 is propagate2d itself (same kernels, same bits)."""
+    norm_type f'{K*K-1}sum' (default) or f'{K*K-1}sum_abs'.  K = 3 is propagate2d itself (same kernels, same bits).
+    keep_sparse=True: the samples are kept in the output, as in propagate2d."""
     code = norm_code_2d_k(prop_kernel, norm_type)
+    if keep_sparse:
+        return _propagate2d_keep(guidance, blur_depth, sparse_depth, prop_kernel, prop_time, code, ALGO_AUTO, out)
     _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel)
     if prop_kernel == 3:
         return propagate2d(guidance, blur_depth, sparse_depth, prop_time, ('8sum', '8sum_abs')[code], ALGO_AUTO, out)
@@ -376,19 +473,22 @@ class Affinity_PropagateK(nn.Module):
     f'{K*K-1}sum_abs'.  No parameters, no buffers; prop_time == 0 returns blur_depth itself.  Forward and backward run
     in CUDA kernels (K = 3 in those of Affinity_Propagate, with the same bits)."""
 
-    def __init__(self, prop_time, prop_kernel, norm_type=None):
+    def __init__(self, prop_time, prop_kernel, norm_type=None, keep_sparse=False):
         super().__init__()
         norm_code_2d_k(prop_kernel, norm_type)      # AssertionError for K not in {3, 5, 7} or a name that does not match K
         self.prop_time = prop_time
         self.prop_kernel = prop_kernel
         self.norm_type = norm_type or f'{prop_kernel * prop_kernel - 1}sum'
+        self.keep_sparse = keep_sparse              # as in Affinity_Propagate
         self._use_op = _use_torch_op()
 
     def forward(self, guidance, blur_depth, sparse_depth=None):
         if self.prop_time == 0:
             return blur_depth
-        sd = None if sparse_depth is None else sparse_depth.detach()
         code = norm_code_2d_k(self.prop_kernel, self.norm_type)
+        if self.keep_sparse:
+            return _keep_forward(self._use_op, guidance, blur_depth, sparse_depth, self.prop_kernel, self.prop_time, code, ALGO_AUTO)
+        sd = None if sparse_depth is None else sparse_depth.detach()
         if self._use_op and blur_depth.is_cuda:
             return torch.ops.cspn_b200.propagate2d_k(guidance, blur_depth, sd, self.prop_kernel, self.prop_time, code)
         if torch.is_grad_enabled() and (guidance.requires_grad or blur_depth.requires_grad):
@@ -396,7 +496,8 @@ class Affinity_PropagateK(nn.Module):
         return propagate2d_k(guidance, blur_depth, sparse_depth, self.prop_kernel, self.prop_time, self.norm_type)
 
     def extra_repr(self):
-        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}'
+        keep = ', keep_sparse=True' if self.keep_sparse else ''
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}{keep}'
 
 
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------

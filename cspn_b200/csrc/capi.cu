@@ -161,7 +161,7 @@ void cspn_host_free(void* p) {
 // The *_workspace_bytes queries return 0 for arguments their entry would reject.  They differ at iters == 0, where the
 // entries copy and need nothing: the forward queries and most backward ones answer 0 there, while cspn2d_bwd_workspace_bytes
 // and cspn2d_k_bwd_workspace_bytes pass iters == 0 on to the 3x3 backward's own formula.
-size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo) {
+static size_t workspace2d(int B, int C, int H, int W, int iters, int algo, bool keep) {
     if (!positive(B, C, H, W, iters)) return 0;
     if (algo != CSPN_ALGO_GENERIC) {
         Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};
@@ -169,7 +169,44 @@ size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo) {
         if (cluster2d_supported(p, why, sizeof(why))) return cluster2d_workspace_bytes(B, C, H, W, iters);
         if (algo == CSPN_ALGO_CLUSTER) return 0;   // the forward call will report why it is unsupported
     }
-    return generic2d_workspace_bytes(B, C, H, W, iters);
+    return generic2d_workspace_bytes(B, C, H, W, iters, keep);
+}
+
+size_t cspn2d_workspace_bytes(int B, int C, int H, int W, int iters, int algo) { return workspace2d(B, C, H, W, iters, algo, false); }
+
+// The 3x3 forward once its arguments are checked: cspn2d_fwd_f32 (gather null), cspn2d_fwd_gather_f32 and the 3x3 calls of
+// the keep-sparse entries (p.keep)
+static int fwd2d_3x3(const Problem2D& p, int algo, const Gather* gather, void* workspace, size_t workspace_bytes,
+                     cspn_stream_t stream) {
+    return on_device_of(p.blur, "blur", [&](int* launches) {
+        char why[256] = "";
+        if (gather) {
+            if (!cluster2d_supported(p, why, sizeof(why), workspace)) {
+                set_error("the fused gather runs in the cluster kernel's epilogue, which cannot take this problem: %s", why);
+                return (int)CSPN_ERR_UNSUPPORTED;
+            }
+            g_last_algo = CSPN_ALGO_CLUSTER;
+            return cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches, gather->peer_out, gather->n_peer,
+                                     gather->multicast_out);
+        }
+        const int chosen = (p.iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why), workspace);
+        if (chosen < 0) { set_error("cluster kernel unsupported for this problem: %s", why); return chosen; }
+        g_last_algo = chosen;
+        if (chosen == CSPN_ALGO_GENERIC && algo == CSPN_ALGO_AUTO && p.iters > 0) {
+            // AUTO sized its workspace for the cluster kernel (cspn2d_workspace_bytes cannot see the pointers); when the
+            // problem then has to take the generic path, say so instead of a bare "workspace too small"
+            const size_t need = generic2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters, p.keep);
+            if (!workspace || workspace_bytes < need) {
+                set_error("CSPN_ALGO_AUTO falls back to the generic path here (%s), which needs %zu workspace bytes (got %zu): "
+                          "query %s(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors and workspace",
+                          why[0] ? why : "cluster kernel declined", need, workspace ? workspace_bytes : (size_t)0,
+                          p.keep ? "cspn2d_keep_workspace_bytes" : "cspn2d_workspace_bytes");
+                return (int)CSPN_ERR_WORKSPACE;
+            }
+        }
+        return (chosen == CSPN_ALGO_CLUSTER) ? cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches)
+                                             : generic2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
 }
 
 int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out, int B, int C, int H,
@@ -179,26 +216,8 @@ int cspn2d_fwd_f32(const float* guidance, const float* blur, const float* sparse
     int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
     if (rc == CSPN_OK) rc = check_algo(algo);
     if (rc != CSPN_OK) return rc;
-    return on_device_of(blur, "blur", [&](int* launches) {
-        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-        char why[256] = "";
-        const int chosen = (iters == 0) ? CSPN_ALGO_GENERIC : resolve_algo(p, algo, why, sizeof(why), workspace);
-        if (chosen < 0) { set_error("cluster kernel unsupported for this problem: %s", why); return chosen; }
-        g_last_algo = chosen;
-        if (chosen == CSPN_ALGO_GENERIC && algo == CSPN_ALGO_AUTO && iters > 0) {
-            // AUTO sized its workspace for the cluster kernel (cspn2d_workspace_bytes cannot see the pointers); when the
-            // problem then has to take the generic path, say so instead of a bare "workspace too small"
-            const size_t need = generic2d_workspace_bytes(B, C, H, W, iters);
-            if (!workspace || workspace_bytes < need) {
-                set_error("CSPN_ALGO_AUTO falls back to the generic path here (%s), which needs %zu workspace bytes (got %zu): "
-                          "query cspn2d_workspace_bytes(..., CSPN_ALGO_GENERIC) or pass 16-byte aligned tensors and workspace",
-                          why[0] ? why : "cluster kernel declined", need, workspace ? workspace_bytes : (size_t)0);
-                return (int)CSPN_ERR_WORKSPACE;
-            }
-        }
-        return (chosen == CSPN_ALGO_CLUSTER) ? cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches)
-                                             : generic2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches);
-    });
+    const Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    return fwd2d_3x3(p, algo, nullptr, workspace, workspace_bytes, stream);
 }
 
 int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out, float* const* peer_out,
@@ -208,16 +227,9 @@ int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, const float*
     int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, 3, guidance_channels, iters, norm_type);
     if (rc == CSPN_OK) rc = check_gather(peer_out, n_peer, multicast_out, iters);
     if (rc != CSPN_OK) return rc;
-    return on_device_of(blur, "blur", [&](int* launches) {
-        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
-        char why[256] = "";
-        if (!cluster2d_supported(p, why, sizeof(why), workspace)) {
-            set_error("the fused gather runs in the cluster kernel's epilogue, which cannot take this problem: %s", why);
-            return (int)CSPN_ERR_UNSUPPORTED;
-        }
-        g_last_algo = CSPN_ALGO_CLUSTER;
-        return cluster2d_forward(p, workspace, workspace_bytes, (cudaStream_t)stream, launches, peer_out, n_peer, multicast_out);
-    });
+    const Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return fwd2d_3x3(p, CSPN_ALGO_CLUSTER, &gather, workspace, workspace_bytes, stream);
 }
 
 size_t cspn2d_bwd_workspace_bytes(int B, int C, int H, int W, int iters) {
@@ -296,6 +308,73 @@ int cspn2d_k_bwd_f32(const float* guidance, const float* blur, const float* spar
         Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
         return widek_backward(p, K, Family::Normalised, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes,
                               (cudaStream_t)stream, launches);
+    });
+}
+
+// ---- 2D keep-sparse mode, K in {3, 5, 7} (DESIGN.md section 4.13): the 3x3 operator above (cluster or generic path) and
+// the K x K one (cspn2d_wide.cu) with m = 1[sparse > 0] and the samples themselves as the replacement.  A null sparse is the
+// default mode ----------------------------------------------------------------------------------------------------------
+size_t cspn2d_keep_workspace_bytes(int B, int C, int H, int W, int K, int iters, int algo) {
+    if (!positive(B, C, H, W, iters) || !kernel_size_ok(2, K) || algo < CSPN_ALGO_AUTO || algo > CSPN_ALGO_CLUSTER) return 0;
+    if (K == 3) return workspace2d(B, C, H, W, iters, algo, true);
+    return widek_workspace_bytes(B, C, H, W, K, iters, Family::Normalised, true);
+}
+
+// gather null: cspn2d_keep_fwd_f32
+static int fwd2d_keep(const float* guidance, const float* blur, const float* sparse, float* out, const Gather* gather, int B, int C,
+                      int H, int W, int guidance_channels, int K, int iters, int norm_type, int algo, void* workspace,
+                      size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    int rc = check_prop(2, guidance, blur, out, B, C, 1, H, W, K, guidance_channels, iters, norm_type);
+    if (rc == CSPN_OK) rc = check_algo(algo);
+    if (rc == CSPN_OK && gather) rc = check_gather(gather->peer_out, gather->n_peer, gather->multicast_out, iters);
+    if (rc != CSPN_OK) return rc;
+    Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+    p.keep = sparse != nullptr;
+    if (K == 3) return fwd2d_3x3(p, gather ? CSPN_ALGO_CLUSTER : algo, gather, workspace, workspace_bytes, stream);
+    return run_forward(blur, "blur", gather, iters, [&](const Fan* fan, int* launches) {
+        return widek_forward(p, K, Family::Normalised, workspace, workspace_bytes, (cudaStream_t)stream, launches, fan);
+    });
+}
+
+int cspn2d_keep_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out, int B, int C, int H, int W,
+                        int guidance_channels, int K, int iters, int norm_type, int algo, void* workspace, size_t workspace_bytes,
+                        cspn_stream_t stream) {
+    return fwd2d_keep(guidance, blur, sparse, out, nullptr, B, C, H, W, guidance_channels, K, iters, norm_type, algo, workspace,
+                      workspace_bytes, stream);
+}
+
+int cspn2d_keep_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out, float* const* peer_out,
+                               int n_peer, float* multicast_out, int B, int C, int H, int W, int guidance_channels, int K,
+                               int iters, int norm_type, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    const Gather gather{peer_out, n_peer, multicast_out};
+    return fwd2d_keep(guidance, blur, sparse, out, &gather, B, C, H, W, guidance_channels, K, iters, norm_type, CSPN_ALGO_AUTO,
+                      workspace, workspace_bytes, stream);
+}
+
+size_t cspn2d_keep_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!positive(B, C, H, W) || iters < 0 || !kernel_size_ok(2, K)) return 0;
+    if (K == 3) return bwd2d_workspace_bytes(B, C, H, W, iters, true);
+    return widek_bwd_workspace_bytes(B, C, H, W, K, iters, Family::Normalised, true);
+}
+
+int cspn2d_keep_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
+                        float* grad_guidance, float* grad_blur, float* grad_sparse, int B, int C, int H, int W,
+                        int guidance_channels, int K, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                        cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_prop(2, guidance, blur, grad_out, B, C, 1, H, W, K, guidance_channels, iters, norm_type);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) -> int {
+        Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, iters, norm_type == CSPN_NORM_8SUM_ABS};
+        p.keep = sparse != nullptr;
+        // no samples, or no step: the output does not depend on sparse
+        if (grad_sparse && (!p.keep || iters == 0))
+            CSPN_CUDA_TRY(cudaMemsetAsync(grad_sparse, 0, (size_t)B * H * W * sizeof(float), (cudaStream_t)stream));
+        if (K == 3)
+            return bwd2d(p, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes, (cudaStream_t)stream, launches, grad_sparse);
+        return widek_backward(p, K, Family::Normalised, grad_out, grad_guidance, grad_blur, workspace, workspace_bytes,
+                              (cudaStream_t)stream, launches, grad_sparse);
     });
 }
 

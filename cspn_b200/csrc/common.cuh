@@ -52,10 +52,12 @@ struct Problem2D {
     const float* sparse;    // [B][1][H][W] or nullptr
     float* out;             // [B][C][H][W]
     int B, C, H, W, gch, iters, norm_abs;
+    int keep = 0;           // keep the sparse samples (DESIGN.md section 4.13): m = 1[sparse > 0], replaced by sparse itself
 };
 
 // ---- per-algorithm launchers (each returns a cspn_status; enqueue only, no sync) -------------
-size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters);
+// keep: the keep-sparse mode, which needs one more B*C*H*W plane (d0', see launch_prep_keep)
+size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep = false);
 int generic2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
 
 // ws: the caller's workspace (nullptr when not known yet); a plan of several passes keeps its intermediate result there
@@ -76,9 +78,16 @@ void launch_prep2d(const float* guidance, const float* sparse, float* wk, int B,
 void launch_step2d(const float* wk, const float* d0, const float* cur, float* dst, int B, int C, int H, int W,
                    cudaStream_t stream);
 
-size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters);
+// Keep-sparse prep of the K x K and 3x3 launch-per-step paths (cspn2d_wide.cu): the K*K planes of prep2d_kernel /
+// prepk_kernel with m = 1[sparse > 0] (w'_k, kappa), and d0 [B][C][H][W] = (1-m) blur + m sparse, the value the constant
+// term kappa * d0 of the unchanged step kernels multiplies
+void launch_prep_keep(int K, const float* guidance, const float* sparse, const float* blur, float* wk, float* d0, int B, int C,
+                      int H, int W, int gch, int norm_abs, cudaStream_t stream);
+
+// keep: as for generic2d_workspace_bytes.  grad_sparse: [B][1][H][W], written in keep mode only (may be null)
+size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep = false);
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-          size_t ws_bytes, cudaStream_t stream, int* launches);
+          size_t ws_bytes, cudaStream_t stream, int* launches, float* grad_sparse = nullptr);
 
 // Fused gather of the K x K, 'paddle' and gates forwards (cspn2d_{k,paddle,gates}_fwd_gather_f32): the last step also
 // stores its result to these destinations, each addressed like p.out -- up to 7 peer-mapped bases (NVLink stores) and one
@@ -123,12 +132,13 @@ enum class Family {
 };
 
 // 2D.  Paddle and Gates: p.sparse null, p.gch == K*K-1, p.guidance [B][K*K-1][H][W].  fan non-null: the fused gather
-size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family);
+// keep (Normalised, p.keep): one more B*C*H*W plane in either workspace; grad_sparse as in bwd2d
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family, bool keep = false);
 int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
                   const Fan* fan = nullptr);
-size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family);
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family, bool keep = false);
 int widek_backward(const Problem2D& p, int K, Family family, const float* grad_out, float* grad_guidance, float* grad_blur,
-                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
+                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, float* grad_sparse = nullptr);
 
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);

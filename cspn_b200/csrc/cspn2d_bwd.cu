@@ -68,24 +68,34 @@ bwd_step_kernel(const float* __restrict__ wk, const float* __restrict__ d_t, con
     for (int k = 0; k < 8; ++k) Gw[((size_t)b * 8 + k) * HW + p] = gw[k];
 }
 
-__global__ void __launch_bounds__(256)
-bwd_finalize_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
-                    const float* __restrict__ wk, const float* __restrict__ Gw, const float* __restrict__ Gc,
-                    const float* __restrict__ lam0, float* __restrict__ grad_guidance, float* __restrict__ grad_blur, int C,
-                    int H, int W, int gch, int norm_abs) {
+// KEEP (keep-sparse mode, sparse non-null): m = 1[sparse > 0], grad_blur's coefficient is (1-m)(1-s) = kappa - m, and
+// grad_sparse (may be null) receives m * sum_c Gc_c, the channels summed in order
+template <bool KEEP>
+__device__ __forceinline__ void bwd_finalize_body(const float* __restrict__ guidance, const float* __restrict__ blur,
+                                                  const float* __restrict__ sparse, const float* __restrict__ wk,
+                                                  const float* __restrict__ Gw, const float* __restrict__ Gc,
+                                                  const float* __restrict__ lam0, float* __restrict__ grad_guidance,
+                                                  float* __restrict__ grad_blur, float* __restrict__ grad_sparse, int C, int H, int W,
+                                                  int gch, int norm_abs) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int b = blockIdx.z;
     if (x >= W || y >= H) return;
     const size_t HW = (size_t)H * W, p = (size_t)y * W + x;
     const float kappa = __ldg(wk + ((size_t)b * 9 + 8) * HW + p);
+    [[maybe_unused]] float m_keep = 0.f, gsum = 0.f;
+    if constexpr (KEEP) m_keep = __ldg(sparse + (size_t)b * HW + p) > 0.f ? 1.f : 0.f;
+    const float cblur = KEEP ? kappa - m_keep : kappa;
     float gkappa = 0.f;
     for (int c = 0; c < C; ++c) {
         const size_t plane = ((size_t)b * C + c) * HW;
         const float gc = __ldg(Gc + plane + p);
         gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
-        if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam0 + plane + p));
+        if (grad_blur) grad_blur[plane + p] = fmaf(cblur, gc, __ldg(lam0 + plane + p));
+        if constexpr (KEEP) gsum += gc;
     }
+    if constexpr (KEEP)
+        if (grad_sparse) grad_sparse[(size_t)b * HW + p] = m_keep * gsum;
     if (!grad_guidance) return;
     const float* g = guidance + (size_t)b * gch * HW;
     float a[8], sg[8], S = 0.f;
@@ -101,7 +111,7 @@ bwd_finalize_kernel(const float* __restrict__ guidance, const float* __restrict_
         a[k] = v;
         S += fabsf(v);
     }
-    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    const float m = KEEP ? m_keep : sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
     const float om = 1.f - m;
     float Hk[8], T = 0.f;
 #pragma unroll
@@ -119,13 +129,32 @@ bwd_finalize_kernel(const float* __restrict__ guidance, const float* __restrict_
     }
 }
 
+__global__ void __launch_bounds__(256)
+bwd_finalize_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+                    const float* __restrict__ wk, const float* __restrict__ Gw, const float* __restrict__ Gc,
+                    const float* __restrict__ lam0, float* __restrict__ grad_guidance, float* __restrict__ grad_blur, int C,
+                    int H, int W, int gch, int norm_abs) {
+    bwd_finalize_body<false>(guidance, blur, sparse, wk, Gw, Gc, lam0, grad_guidance, grad_blur, nullptr, C, H, W, gch, norm_abs);
+}
+
+__global__ void __launch_bounds__(256)
+bwd_finalize_keep_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+                         const float* __restrict__ wk, const float* __restrict__ Gw, const float* __restrict__ Gc,
+                         const float* __restrict__ lam0, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+                         float* __restrict__ grad_sparse, int C, int H, int W, int gch, int norm_abs) {
+    bwd_finalize_body<true>(guidance, blur, sparse, wk, Gw, Gc, lam0, grad_guidance, grad_blur, grad_sparse, C, H, W, gch, norm_abs);
+}
+
 // Staged cluster formulation, last stage: Gw / Gc gathered over all steps in registers, then the finalize arithmetic
 // of bwd_finalize_kernel.  steps[t] = d_{t+1}, lam[t] = lambda_t (planes of n = B*C*H*W floats), lambda_N = grad_out.
-__global__ void __launch_bounds__(256)
-bwd_gather_finalize_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
-                           const float* __restrict__ steps, const float* __restrict__ lam, const float* __restrict__ grad_out,
-                           float* __restrict__ grad_guidance, float* __restrict__ grad_blur, long long n, int N, int C, int H,
-                           int W, int gch, int norm_abs) {
+// KEEP: as in bwd_finalize_body, with grad_blur's coefficient (1-m)(1 - sum_k w_k) formed from the quotients
+template <bool KEEP>
+__device__ __forceinline__ void bwd_gather_finalize_body(const float* __restrict__ guidance, const float* __restrict__ blur,
+                                                         const float* __restrict__ sparse, const float* __restrict__ steps,
+                                                         const float* __restrict__ lam, const float* __restrict__ grad_out,
+                                                         float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+                                                         float* __restrict__ grad_sparse, long long n, int N, int C, int H, int W,
+                                                         int gch, int norm_abs) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int b = blockIdx.z;
@@ -147,12 +176,15 @@ bwd_gather_finalize_kernel(const float* __restrict__ guidance, const float* __re
         a[k] = v;
         S += fabsf(v);
     }
-    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    float m;
+    if constexpr (KEEP) m = __ldg(sparse + (size_t)b * HW + p) > 0.f ? 1.f : 0.f;
+    else m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
     const float om = 1.f - m;
     float wsum = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) wsum += __fdiv_rn(a[k], S);
-    const float kappa = om * (1.f - wsum) + m;
+    const float kappa = KEEP ? om * (1.f - wsum) : om * (1.f - wsum) + m;
+    [[maybe_unused]] float gsum = 0.f;
 
     float gw[8], gkappa = 0.f;
 #pragma unroll
@@ -170,7 +202,10 @@ bwd_gather_finalize_kernel(const float* __restrict__ guidance, const float* __re
         }
         gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
         if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
+        if constexpr (KEEP) gsum += gc;
     }
+    if constexpr (KEEP)
+        if (grad_sparse) grad_sparse[(size_t)b * HW + p] = m * gsum;
     if (!grad_guidance) return;
     float Hk[8], T = 0.f;
 #pragma unroll
@@ -186,6 +221,27 @@ bwd_gather_finalize_kernel(const float* __restrict__ guidance, const float* __re
         }
 }
 
+__global__ void __launch_bounds__(256)
+bwd_gather_finalize_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+                           const float* __restrict__ steps, const float* __restrict__ lam, const float* __restrict__ grad_out,
+                           float* __restrict__ grad_guidance, float* __restrict__ grad_blur, long long n, int N, int C, int H,
+                           int W, int gch, int norm_abs) {
+    bwd_gather_finalize_body<false>(guidance, blur, sparse, steps, lam, grad_out, grad_guidance, grad_blur, nullptr, n, N, C, H, W,
+                                    gch, norm_abs);
+}
+
+// at least three CTAs per SM (the default kernel gets four at its 62 registers): left alone, ptxas gives this one 98
+// registers and two CTAs, and the gather's load latency is then exposed (1.5x the default kernel's time on an H100).  Four
+// would cap it at 64 registers, where it spills.
+__global__ void __launch_bounds__(256, 3)
+bwd_gather_finalize_keep_kernel(const float* __restrict__ guidance, const float* __restrict__ blur,
+                                const float* __restrict__ sparse, const float* __restrict__ steps, const float* __restrict__ lam,
+                                const float* __restrict__ grad_out, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+                                float* __restrict__ grad_sparse, long long n, int N, int C, int H, int W, int gch, int norm_abs) {
+    bwd_gather_finalize_body<true>(guidance, blur, sparse, steps, lam, grad_out, grad_guidance, grad_blur, grad_sparse, n, N, C, H,
+                                   W, gch, norm_abs);
+}
+
 // The register-resident formulation is the default; CSPN_B200_BWD=steps forces the launch-per-step one (cross-check in
 // tests/test_cluster_backward_gpu.py, and the path shapes outside the cluster kernel's take anyway).
 bool cluster_backward_enabled() {
@@ -195,19 +251,20 @@ bool cluster_backward_enabled() {
 
 }  // namespace
 
-size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters) {
+size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W, n = (size_t)B * C * HW;
-    // wk (9 planes/image) + d_1..d_{N-1} + lambda ping-pong + Gw + Gc
-    const size_t per_step = sizeof(float) * ((size_t)B * 9 * HW + (size_t)(iters - 1) * n + 2 * n + (size_t)B * 8 * HW + n);
+    // wk (9 planes/image) + d_1..d_{N-1} + lambda ping-pong + Gw + Gc (+ d0' in the keep-sparse mode)
+    const size_t per_step = sizeof(float) * ((size_t)B * 9 * HW + (size_t)(iters - 1) * n + 2 * n + (size_t)B * 8 * HW + n +
+                                             (keep ? n : 0));
     const size_t cluster = cluster_backward_enabled() ? sizeof(float) * 2 * (size_t)iters * n : 0;   // d_1..d_N, lambda_0..lambda_{N-1}
     return per_step > cluster ? per_step : cluster;
 }
 
 // Cluster formulation (see the file header).  Returns CSPN_ERR_UNSUPPORTED when the shape / alignment is not
 // the cluster kernel's; the caller then falls back to the launch-per-step path.
-static int bwd2d_cluster(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-                         cudaStream_t stream, int* launches) {
+static int bwd2d_cluster(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, float* grad_sparse,
+                         void* ws, cudaStream_t stream, int* launches) {
     char why[200] = "";
     if ((reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(ws)) & 15) return CSPN_ERR_UNSUPPORTED;
     if (!cluster2d_supported(p, why, sizeof(why))) return CSPN_ERR_UNSUPPORTED;
@@ -220,15 +277,20 @@ static int bwd2d_cluster(const Problem2D& p, const float* grad_out, float* grad_
     if (rc != CSPN_OK) return rc;
     const dim3 block(32, 8);
     const dim3 grid((p.W + 31) / 32, (p.H + 7) / 8, p.B);
-    bwd_gather_finalize_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, steps, lam, grad_out, grad_guidance,
-                                                            grad_blur, n, p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
+    if (p.keep)
+        bwd_gather_finalize_keep_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, steps, lam, grad_out, grad_guidance,
+                                                                     grad_blur, grad_sparse, n, p.iters, p.C, p.H, p.W, p.gch,
+                                                                     p.norm_abs);
+    else
+        bwd_gather_finalize_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, steps, lam, grad_out, grad_guidance,
+                                                                grad_blur, n, p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
     ++*launches;
     CSPN_CUDA_TRY(cudaGetLastError());
     return CSPN_OK;
 }
 
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws, size_t ws_bytes,
-          cudaStream_t stream, int* launches) {
+          cudaStream_t stream, int* launches, float* grad_sparse) {
     const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
     if (grad_guidance)
         CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
@@ -236,14 +298,14 @@ int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float
         if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = bwd2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
+    const size_t need = bwd2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters, p.keep);
     if (!ws || ws_bytes < need) {
         set_error("2D backward needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
         return CSPN_ERR_WORKSPACE;
     }
     if (p.B > 65535 || (long)p.B * p.C > 65535) { set_error("backward: B*C exceeds gridDim.z"); return CSPN_ERR_UNSUPPORTED; }
     if (cluster_backward_enabled()) {
-        const int rc = bwd2d_cluster(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+        const int rc = bwd2d_cluster(p, grad_out, grad_guidance, grad_blur, grad_sparse, ws, stream, launches);
         if (rc != CSPN_ERR_UNSUPPORTED) return rc;
         clear_error();   // shape / alignment outside the cluster kernel's: the launch-per-step path below handles it
     }
@@ -253,10 +315,17 @@ int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float
     float* Gw = lam[1] + n;
     float* Gc = Gw + (size_t)p.B * 8 * HW;
 
-    launch_prep2d(p.guidance, p.sparse, wk, p.B, p.H, p.W, p.gch, p.norm_abs, stream);
+    // keep-sparse mode: the constant term of the forward steps reads d0' = (1-m) blur + m sparse (after Gc)
+    const float* d0 = p.blur;
+    if (p.keep) {
+        launch_prep_keep(3, p.guidance, p.sparse, p.blur, wk, Gc + n, p.B, p.C, p.H, p.W, p.gch, p.norm_abs, stream);
+        d0 = Gc + n;
+    } else {
+        launch_prep2d(p.guidance, p.sparse, wk, p.B, p.H, p.W, p.gch, p.norm_abs, stream);
+    }
     ++*launches;
     for (int t = 0; t + 1 < p.iters; ++t) {           // d_{t+1} = step(d_t)
-        launch_step2d(wk, p.blur, t == 0 ? p.blur : D + (size_t)(t - 1) * n, D + (size_t)t * n, p.B, p.C, p.H, p.W, stream);
+        launch_step2d(wk, d0, t == 0 ? p.blur : D + (size_t)(t - 1) * n, D + (size_t)t * n, p.B, p.C, p.H, p.W, stream);
         ++*launches;
     }
     const dim3 block(32, 8);
@@ -269,8 +338,12 @@ int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float
         ++*launches;
         lam_in = lam_out;
     }
-    bwd_finalize_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, wk, Gw, Gc, lam_in, grad_guidance, grad_blur,
-                                                    p.C, p.H, p.W, p.gch, p.norm_abs);
+    if (p.keep)
+        bwd_finalize_keep_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, wk, Gw, Gc, lam_in, grad_guidance,
+                                                             grad_blur, grad_sparse, p.C, p.H, p.W, p.gch, p.norm_abs);
+    else
+        bwd_finalize_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, wk, Gw, Gc, lam_in, grad_guidance, grad_blur,
+                                                        p.C, p.H, p.W, p.gch, p.norm_abs);
     ++*launches;
     CSPN_CUDA_TRY(cudaGetLastError());
     return CSPN_OK;

@@ -556,7 +556,24 @@ __device__ __forceinline__ void step_fwd(Xch& x, int wy, uint32_t phase, const f
 //                that the backward pass needs)
 //   kAdjoint     lambda <- sum_k shift_{-k}(w'_k lambda), `iters` times, every step's result written out: the
 //                transpose of the forward step (cspn2d_bwd.cu has the derivation); `blur` carries lambda's start value
-enum ClusterMode { kForward = 0, kStoreSteps = 1, kAdjoint = 2 };
+// kKeep, or-ed into any of them, keeps the sparse samples (DESIGN.md section 4.13): m = 1[sparse > 0] instead of
+// sign(sparse) (mask_of), and the constant term takes d0' = (1-m) d_0 + m sparse instead of d_0 (keep_d0).  The iterate
+// still starts at d_0.
+enum ClusterMode { kForward = 0, kStoreSteps = 1, kAdjoint = 2, kKeep = 4 };
+
+// The mask of one sparse_depth value: sign(v) in the default mode, 1[v > 0] in keep mode (NaN, 0 and negatives -> 0)
+template <bool KEEP>
+__device__ __forceinline__ float mask_of(float v) {
+    if constexpr (KEEP) return v > 0.f ? 1.f : 0.f;
+    else return signf(v);
+}
+// Keep mode: the d_0 of the constant term of one patch row, d0' = (1-m) d_0 + m sparse
+template <int PC>
+__device__ __forceinline__ void keep_d0(const float4 sv, const float (&m)[PC], const float (&d)[PC], float (&d0)[PC]) {
+    const float s[4] = {sv.x, sv.y, sv.z, sv.w};
+#pragma unroll
+    for (int j = 0; j < PC; ++j) d0[j] = __fadd_rn(__fmul_rn(1.f - m[j], d[j]), __fmul_rn(m[j], s[j]));
+}
 
 // Adjoint of scatter_row: the SOURCE pixels (weights w, values l) of one row push w_k * l into the destination row DY
 // rows further down (off_k = (DY, dx)): destination column = source column + dx.  Columns -1 and PC belong to the
@@ -719,10 +736,13 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 
 // GENERAL = false compiles out row bands and the continuation input of multi-pass plans: the common single-pass,
 // single-band launch (every BASELINE 2D config) pays nothing for them.
-template <int PR, int PC, int NW, bool ABS, bool GENERAL, int MODE = kForward, bool CHAIN = false>
+// FLAGS: a ClusterMode, with kKeep or-ed in for the keep-sparse variant.
+template <int PR, int PC, int NW, bool ABS, bool GENERAL, int FLAGS = kForward, bool CHAIN = false>
 __global__ void __launch_bounds__(Cfg<PR, PC, NW>::kBlockThreads, 1)
 cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __grid_constant__ CUtensorMap tm_blur,
                       const __grid_constant__ CUtensorMap tm_sparse, const __grid_constant__ ClusterParams prm) {
+    constexpr int MODE = FLAGS & ~kKeep;
+    constexpr bool KEEP = (FLAGS & kKeep) != 0;
     using K = Cfg<PR, PC, NW>;
     constexpr int RB = K::RB, TW = K::TW, TWP = K::TWP, TWX = K::TWX;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -877,8 +897,8 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                     issue_stage(t);
                 }
                 float* cb = cbuf + (size_t)nb * RB * TW;
-                // blur_depth rows go straight into this thread's slots of d0buf, sparse_depth rows (only their sign is used)
-                // into its slots of the c' buffer: both are read back by this thread only, before c' overwrites them
+                // blur_depth rows go straight into this thread's slots of d0buf, sparse_depth rows (only their mask is used, and in
+                // keep mode the samples) into its slots of the c' buffer: both are read back by this thread only, before c' overwrites them
                 const float* blur = prm.blur + (size_t)bc * HW;
                 const float* sparse = prm.sparse ? prm.sparse + (size_t)(bc / prm.C) * HW : nullptr;
 #pragma unroll
@@ -933,8 +953,14 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
                         gather_row<PC, ABS>(row0, (size_t)RB * TWP, lane, a, S);
                         load_row_smem(dc, d);
                         const float4 sv = *reinterpret_cast<const float4*>(sc);
-                        const float mrow[PC] = {signf(sv.x), signf(sv.y), signf(sv.z), signf(sv.w)};
-                        fold_row<PC>(a, S, mrow, d, in, w, cj);
+                        const float mrow[PC] = {mask_of<KEEP>(sv.x), mask_of<KEEP>(sv.y), mask_of<KEEP>(sv.z), mask_of<KEEP>(sv.w)};
+                        if constexpr (KEEP) {
+                            float d0[PC];
+                            keep_d0(sv, mrow, d, d0);
+                            fold_row<PC>(a, S, mrow, d0, in, w, cj);
+                        } else {
+                            fold_row<PC>(a, S, mrow, d, in, w, cj);
+                        }
 #pragma unroll
                         for (int k = 0; k < 8; ++k)
                             *reinterpret_cast<float4*>(row0 + k * (size_t)RB * TWP) = make_float4(w[0][k], w[1][k], w[2][k], w[3][k]);
@@ -1059,7 +1085,7 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
 
         // blur_depth rows go global -> shared with cp.async, straight into this thread's slots of the c' buffer (free until
         // the prologue writes c' there): nothing holds them in flight, and the prologue reads each row back when it needs
-        // it.  sparse_depth rows (only their sign is used) wait in registers and are converted row by row.  Both were
+        // it.  sparse_depth rows (only their mask is used, and in keep mode the samples) wait in registers and are converted row by row.  Both were
         // pulled into L2 one task ago by the TMA prefetch below, so what is hidden here is an L2 latency.
         // W % 4 == 0 and x_thr % 4 == 0: a float4 is entirely inside or outside the image.
         const bool col_in = (x_thr >= 0) && (x_thr < W);
@@ -1113,14 +1139,20 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
             // this row's blur_depth (from the c' slot the cp.async filled) and mask
             if (r == 0) cp_async_wait_all();            // this thread's own copies: no barrier needed
             load_row_smem(my_c + r * TW, d[r]);
-            const float mrow[PC] = {signf(sv[r].x), signf(sv[r].y), signf(sv[r].z), signf(sv[r].w)};
+            const float mrow[PC] = {mask_of<KEEP>(sv[r].x), mask_of<KEEP>(sv[r].y), mask_of<KEEP>(sv[r].z), mask_of<KEEP>(sv[r].w)};
             if (r == 0 && early_publish) {
                 float bot[PC];
                 load_row_smem(my_c + (PR - 1) * TW, bot);
                 publish<PR, PC, NW, 0>(xc, wy, d[0], bot);
             }
             float cj[PC];
-            fold_row<PC>(a, S, mrow, d[r], col_in && (y < H), w[r], cj);
+            if constexpr (KEEP) {
+                float d0[PC];
+                keep_d0(sv[r], mrow, d[r], d0);
+                fold_row<PC>(a, S, mrow, d0, col_in && (y < H), w[r], cj);
+            } else {
+                fold_row<PC>(a, S, mrow, d[r], col_in && (y < H), w[r], cj);
+            }
             // only this thread ever reads these values back: no barrier needed
             if constexpr (MODE != kAdjoint) {
                 store_row_smem(const_cast<float*>(xc.cbuf) + r * TW, cj);   // the adjoint has no constant term
@@ -1300,37 +1332,53 @@ cspn2d_cluster_kernel(const __grid_constant__ CUtensorMap tm_guidance, const __g
 
 // ---- host side: configurations, planner, launch ---------------------------------------------------
 
+// Every table is indexed by [keep] first: 0 the default mode, 1 the keep-sparse variant (kKeep)
 struct KernelCfg {
     int PR, PC, NW;
-    const void* fn[2][2];      // kForward: [general][norm_abs]
-    const void* fn_steps[2];   // kStoreSteps [norm_abs]
-    const void* fn_adj[2];     // kAdjoint    [norm_abs]
-    const void* fn_chain[2][2];   // kForward with chained strips: [general][norm_abs]; null when the configuration has no such kernel
+    const void* fn[2][2][2];      // kForward: [keep][general][norm_abs]
+    const void* fn_steps[2][2];   // kStoreSteps [keep][norm_abs]
+    const void* fn_adj[2][2];     // kAdjoint    [keep][norm_abs]
+    const void* fn_chain[2][2][2];   // kForward with chained strips: [keep][general][norm_abs]; null when the configuration has no such kernel
     size_t smem, smem_chain;
     int threads;               // per CTA: the consumer warps, plus the producer warpgroup of kSplit configurations
     int RB() const { return PR * NW; }
     int TW() const { return 32 * PC; }
 };
 
+// KF: 0 or kKeep
+template <int PR, int PC, int NW, int KF>
+void set_kernels(KernelCfg& k) {
+    const int i = KF ? 1 : 0;
+    k.fn[i][0][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, false, kForward | KF>;
+    k.fn[i][0][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, false, kForward | KF>;
+    k.fn[i][1][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kForward | KF>;
+    k.fn[i][1][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kForward | KF>;
+    k.fn_steps[i][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kStoreSteps | KF>;
+    k.fn_steps[i][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kStoreSteps | KF>;
+    k.fn_adj[i][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kAdjoint | KF>;
+    k.fn_adj[i][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kAdjoint | KF>;
+}
+template <int PR, int PC, int NW, int KF>
+void set_chain_kernels(KernelCfg& k) {
+    const int i = KF ? 1 : 0;
+    k.fn_chain[i][0][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, false, kForward | KF, true>;
+    k.fn_chain[i][0][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, false, kForward | KF, true>;
+    k.fn_chain[i][1][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kForward | KF, true>;
+    k.fn_chain[i][1][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kForward | KF, true>;
+}
+
 template <int PR, int PC, int NW>
 KernelCfg make_cfg() {
-    return KernelCfg{PR, PC, NW,
-                     {{(const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, false>, (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, false>},
-                      {(const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true>, (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true>}},
-                     {(const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kStoreSteps>,
-                      (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kStoreSteps>},
-                     {(const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kAdjoint>,
-                      (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kAdjoint>},
-                     {{nullptr, nullptr}, {nullptr, nullptr}},
-                     Cfg<PR, PC, NW>::kSmemBytes, 0, Cfg<PR, PC, NW>::kBlockThreads};
+    KernelCfg k{PR, PC, NW, {}, {}, {}, {}, Cfg<PR, PC, NW>::kSmemBytes, 0, Cfg<PR, PC, NW>::kBlockThreads};
+    set_kernels<PR, PC, NW, 0>(k);
+    set_kernels<PR, PC, NW, kKeep>(k);
+    return k;
 }
 template <int PR, int PC, int NW>
 KernelCfg make_cfg_chain() {
     KernelCfg k = make_cfg<PR, PC, NW>();
-    k.fn_chain[0][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, false, kForward, true>;
-    k.fn_chain[0][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, false, kForward, true>;
-    k.fn_chain[1][0] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, false, true, kForward, true>;
-    k.fn_chain[1][1] = (const void*)&cspn2d_cluster_kernel<PR, PC, NW, true, true, kForward, true>;
+    set_chain_kernels<PR, PC, NW, 0>(k);
+    set_chain_kernels<PR, PC, NW, kKeep>(k);
     k.smem_chain = Cfg<PR, PC, NW>::kSmemBytesChain;
     return k;
 }
@@ -1341,10 +1389,9 @@ KernelCfg make_cfg_chain() {
 // developer build for offline SASS studies (tools/sass_loop.py on a 10-second compile): only the headline kernels
 const std::vector<KernelCfg>& configs() {
     static const std::vector<KernelCfg> v = [] {
-        KernelCfg k{5, 4, 8, {{nullptr, nullptr}, {nullptr, nullptr}}, {nullptr, nullptr}, {nullptr, nullptr}, {{nullptr, nullptr}, {nullptr, nullptr}},
-                    Cfg<5, 4, 8>::kSmemBytes, Cfg<5, 4, 8>::kSmemBytesChain, Cfg<5, 4, 8>::kBlockThreads};
-        k.fn[0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false>;
-        k.fn_chain[0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false, kForward, true>;
+        KernelCfg k{5, 4, 8, {}, {}, {}, {}, Cfg<5, 4, 8>::kSmemBytes, Cfg<5, 4, 8>::kSmemBytesChain, Cfg<5, 4, 8>::kBlockThreads};
+        k.fn[0][0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false>;
+        k.fn_chain[0][0][0] = (const void*)&cspn2d_cluster_kernel<5, 4, 8, false, false, kForward, true>;
         return std::vector<KernelCfg>{k};
     }();
     return v;
@@ -1403,14 +1450,21 @@ int max_active_clusters(int ci, int cs, int dev, bool chained = false) {
     for (auto& e : g_occ_cache)
         if (e.first.cfg == ci && e.first.cs == cs && e.first.dev == dev && e.first.chained == (int)chained) return e.second;
     const KernelCfg& k = configs()[ci];
-    if (chained && !k.fn_chain[0][0]) return 0;
+    if (chained && !k.fn_chain[0][0][0]) return 0;
     if (!g_attr_set[dev & 15][ci]) {
-        const void* all[12] = {k.fn[0][0], k.fn[0][1], k.fn[1][0], k.fn[1][1], k.fn_steps[0], k.fn_steps[1], k.fn_adj[0], k.fn_adj[1],
-                               k.fn_chain[0][0], k.fn_chain[0][1], k.fn_chain[1][0], k.fn_chain[1][1]};
-        for (int i = 0; i < 12; ++i) {
+        // [keep] tables side by side: 8 unchained kernels, then 4 chained ones, per mode
+        const void* all[24];
+        for (int m = 0; m < 2; ++m) {
+            const void* const* base = &k.fn[m][0][0];
+            for (int i = 0; i < 4; ++i) all[12 * m + i] = base[i];
+            all[12 * m + 4] = k.fn_steps[m][0]; all[12 * m + 5] = k.fn_steps[m][1];
+            all[12 * m + 6] = k.fn_adj[m][0];   all[12 * m + 7] = k.fn_adj[m][1];
+            for (int i = 0; i < 4; ++i) all[12 * m + 8 + i] = (&k.fn_chain[m][0][0])[i];
+        }
+        for (int i = 0; i < 24; ++i) {
             const void* f = all[i];
             if (!f) continue;
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(i >= 8 ? k.smem_chain : k.smem)) != cudaSuccess ||
+            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(i % 12 >= 8 ? k.smem_chain : k.smem)) != cudaSuccess ||
                 cudaFuncSetAttribute(f, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
                 cudaGetLastError();
                 return 0;
@@ -1430,7 +1484,7 @@ int max_active_clusters(int ci, int cs, int dev, bool chained = false) {
     cfg.attrs = at;
     cfg.numAttrs = 1;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, chained ? k.fn_chain[1][0] : k.fn[1][0], &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+    if (cudaOccupancyMaxActiveClusters(&n, chained ? k.fn_chain[0][1][0] : k.fn[0][1][0], &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
     g_occ_cache.push_back({OccKey{ci, cs, dev, (int)chained}, n});
     return n;
 }
@@ -1491,7 +1545,7 @@ bool plan_pass(int H, int W, int iters, int dev, int forced, bool chained, PassP
         PassPlan p;
         // columns: 4-aligned strip origins (TMA / float4), at least 16 useful columns per strip
         if (chained) {
-            if (!k.fn_chain[0][0] || iters > kChainMaxIters) continue;
+            if (!k.fn_chain[0][0][0] || iters > kChainMaxIters) continue;
             if (!layout_1d_chained(W, k.TW(), iters, 4, 16, kMaxStrips, p.n_strips, p.tile_x0, p.ux0, p.ux1)) continue;
             p.chained = true;
             p.chain_lane = (k.TW() - (iters + 3) / 4 * 4) / 4 - 1;   // its 4th column is the one left of the next tile
@@ -1919,7 +1973,7 @@ int cluster2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_
         Scatter sc;
         if (ip == plan.n_pass - 1) { sc.peer = peer_out; sc.n_peer = n_peer; sc.mc = mc_out; }   // only the final result travels
         const KernelCfg& kc = configs()[pp.cfg];
-        rc = launch_pass(p, pp, (pp.chained ? kc.fn_chain : kc.fn)[general ? 1 : 0][p.norm_abs ? 1 : 0], p.blur, prev, dst, nullptr, 0, stream, sc,
+        rc = launch_pass(p, pp, (pp.chained ? kc.fn_chain : kc.fn)[p.keep ? 1 : 0][general ? 1 : 0][p.norm_abs ? 1 : 0], p.blur, prev, dst, nullptr, 0, stream, sc,
                          pp.chained ? cb : ChainBuf());
         if (rc != CSPN_OK && pp.chained && ip == 0) {
             // the cooperative launch was refused (the grid cannot be made resident as a whole: SM partitioning, MPS limits, ...):
@@ -1950,7 +2004,7 @@ int cluster2d_forward_steps(const Problem2D& p, float* steps, cudaStream_t strea
     int done = 0;
     for (int ip = 0; ip < plan.n_pass; ++ip) {
         const PassPlan& pp = plan.pass(ip);
-        rc = launch_pass(p, pp, configs()[pp.cfg].fn_steps[p.norm_abs ? 1 : 0], p.blur, done ? steps + (done - 1) * n : nullptr,
+        rc = launch_pass(p, pp, configs()[pp.cfg].fn_steps[p.keep ? 1 : 0][p.norm_abs ? 1 : 0], p.blur, done ? steps + (done - 1) * n : nullptr,
                          steps + (done + pp.iters - 1) * n, steps + done * n, n, stream);
         if (rc != CSPN_OK) return rc;
         ++*launches;
@@ -1969,7 +2023,7 @@ int cluster2d_adjoint_steps(const Problem2D& p, const float* grad_out, float* la
     int done = 0;   // adjoint steps taken so far: lambda_{N-done} is the current state
     for (int ip = 0; ip < plan.n_pass; ++ip) {
         const PassPlan& pp = plan.pass(ip);
-        rc = launch_pass(p, pp, configs()[pp.cfg].fn_adj[p.norm_abs ? 1 : 0], done ? lam + (long long)(N - done) * n : grad_out, nullptr,
+        rc = launch_pass(p, pp, configs()[pp.cfg].fn_adj[p.keep ? 1 : 0][p.norm_abs ? 1 : 0], done ? lam + (long long)(N - done) * n : grad_out, nullptr,
                          lam + (long long)(N - done - pp.iters) * n, lam + (long long)(N - done - 1) * n, -n, stream);
         if (rc != CSPN_OK) return rc;
         ++*launches;

@@ -87,10 +87,11 @@ void launch_step2d(const float* wk, const float* d0, const float* cur, float* ds
     step2d_kernel<<<dim3((W + 31) / 32, (H + 7) / 8, B * C), block, 0, stream>>>(wk, d0, cur, dst, C, H, W);
 }
 
-size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters) {
+// keep: the d0' planes of the keep-sparse mode follow the ping-pong buffer
+size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W;
-    return sizeof(float) * ((size_t)B * 9 * HW + (iters > 1 ? (size_t)B * C * HW : 0));
+    return sizeof(float) * ((size_t)B * 9 * HW + (iters > 1 ? (size_t)B * C * HW : 0) + (keep ? (size_t)B * C * HW : 0));
 }
 
 int generic2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
@@ -100,7 +101,7 @@ int generic2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_
         CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const size_t need = generic2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters);
+    const size_t need = generic2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters, p.keep);
     if (!ws || ws_bytes < need) {
         set_error("generic 2D path needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
         return CSPN_ERR_WORKSPACE;
@@ -113,14 +114,22 @@ int generic2d_forward(const Problem2D& p, void* ws, size_t ws_bytes, cudaStream_
         set_error("generic 2D path: B*C=%d exceeds gridDim.z", p.B * p.C);
         return CSPN_ERR_UNSUPPORTED;
     }
-    prep2d_kernel<<<dim3(gx.x, gx.y, p.B), block, 0, stream>>>(p.guidance, p.sparse, wk, p.H, p.W, p.gch,
-                                                                p.norm_abs);
+    // keep-sparse mode: the same step kernel, its constant term kappa * d0 reading d0' = (1-m) blur + m sparse
+    const float* d0 = p.blur;
+    if (p.keep) {
+        float* d0k = tmp + (p.iters > 1 ? n : 0);
+        launch_prep_keep(3, p.guidance, p.sparse, p.blur, wk, d0k, p.B, p.C, p.H, p.W, p.gch, p.norm_abs, stream);
+        d0 = d0k;
+    } else {
+        prep2d_kernel<<<dim3(gx.x, gx.y, p.B), block, 0, stream>>>(p.guidance, p.sparse, wk, p.H, p.W, p.gch,
+                                                                    p.norm_abs);
+    }
     ++*launches;
     // ping-pong so that the last iteration writes p.out
     const float* cur = p.blur;
     float* dst = (p.iters & 1) ? p.out : tmp;
     for (int it = 0; it < p.iters; ++it) {
-        step2d_kernel<<<dim3(gx.x, gx.y, p.B * p.C), block, 0, stream>>>(wk, p.blur, cur, dst, p.C, p.H, p.W);
+        step2d_kernel<<<dim3(gx.x, gx.y, p.B * p.C), block, 0, stream>>>(wk, d0, cur, dst, p.C, p.H, p.W);
         ++*launches;
         cur = dst;
         dst = (dst == p.out) ? tmp : p.out;

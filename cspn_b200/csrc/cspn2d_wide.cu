@@ -59,10 +59,12 @@ struct Taps {
 __device__ __forceinline__ bool inside(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
 
 // ---- prep: prep2d_kernel with NT taps.  grid z = image of the group (pointers offset to the group) ----------------
-template <int R>
-__global__ void __launch_bounds__(256)
-prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ sparse, float* __restrict__ wk, int H, int W,
-             int gch, int norm_abs) {
+// KEEP (keep-sparse mode, DESIGN.md section 4.13): m = 1[sparse > 0], and d0 [image][C][H][W] receives
+// (1-m) blur + m sparse, which the step kernels' constant term kappa * d0 then reads in place of blur.
+template <int R, bool KEEP>
+__device__ __forceinline__ void prepk_body(const float* __restrict__ guidance, const float* __restrict__ sparse,
+                                           float* __restrict__ wk, const float* __restrict__ blur, float* __restrict__ d0, int C,
+                                           int H, int W, int gch, int norm_abs) {
     using T = Taps<R>;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
@@ -83,7 +85,13 @@ prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ spars
         S += fabsf(v);
     }
     const size_t p = (size_t)y * W + x;
-    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    float m, sv = 0.f;
+    if constexpr (KEEP) {
+        sv = __ldg(sparse + (size_t)b * HW + p);
+        m = sv > 0.f ? 1.f : 0.f;             // NaN, 0 and negative samples are not samples
+    } else {
+        m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    }
     const float om = 1.f - m;
     float s = 0.f;
     float* o = wk + (size_t)b * T::NP * HW + p;
@@ -94,6 +102,26 @@ prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ spars
         o[k * HW] = om * w;
     }
     o[T::NT * HW] = om * (1.f - s) + m;
+    if constexpr (KEEP)
+        for (int c = 0; c < C; ++c) {
+            const size_t q = ((size_t)b * C + c) * HW + p;
+            d0[q] = __fadd_rn(__fmul_rn(om, __ldg(blur + q)), __fmul_rn(m, sv));
+        }
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+prepk_kernel(const float* __restrict__ guidance, const float* __restrict__ sparse, float* __restrict__ wk, int H, int W,
+             int gch, int norm_abs) {
+    prepk_body<R, false>(guidance, sparse, wk, nullptr, nullptr, 1, H, W, gch, norm_abs);
+}
+
+// sparse non-null
+template <int R>
+__global__ void __launch_bounds__(256)
+prepk_keep_kernel(const float* __restrict__ guidance, const float* __restrict__ sparse, const float* __restrict__ blur,
+                  float* __restrict__ wk, float* __restrict__ d0, int C, int H, int W, int gch, int norm_abs) {
+    prepk_body<R, true>(guidance, sparse, wk, blur, d0, C, H, W, gch, norm_abs);
 }
 
 // 'paddle' prep: w_k = |g_k(p)| / sum_j |g_j(p)|, kappa = 0.  guidance [image][NT][H][W]; grid z = image of the group
@@ -245,12 +273,15 @@ adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, floa
 // PADDLE (sparse null, gch = NT): the own-location chain rule of cspn3d_wide.cu's fin3k_kernel mode 2 -- no centre term,
 // grad_g_j lands at p, grad_blur = lambda_0.
 // RAW (with PADDLE, grad_blur null): the gates are the caller's, so grad_g_k(p) = Gw_k(p); guidance and wk are not read.
-template <int R, bool PADDLE = false, bool RAW = false>
-__global__ void __launch_bounds__(256)
-gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
-               const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
-               const float* __restrict__ grad_out, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
-               long long n, int N, int C, int H, int W, int gch, int norm_abs) {
+// KEEP (keep-sparse mode, sparse non-null): m = 1[sparse > 0], grad_blur's coefficient is (1-m)(1-s) = kappa - m, and
+// grad_sparse (may be null) receives m * sum_c Gc_c, the channels summed in order.
+template <int R, bool PADDLE, bool RAW, bool KEEP>
+__device__ __forceinline__ void gatherk_body(const float* __restrict__ guidance, const float* __restrict__ blur,
+                                             const float* __restrict__ sparse, const float* __restrict__ wk,
+                                             const float* __restrict__ steps, const float* __restrict__ lam,
+                                             const float* __restrict__ grad_out, float* __restrict__ grad_guidance,
+                                             float* __restrict__ grad_blur, float* __restrict__ grad_sparse, long long n, int N,
+                                             int C, int H, int W, int gch, int norm_abs) {
     using T = Taps<R>;
     __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
     const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, b = blockIdx.z;
@@ -261,6 +292,9 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) gw[k] = 0.f;
     const float kappa = in && !PADDLE ? __ldg(wk + ((size_t)b * T::NP + T::NT) * HW + p) : 0.f;
+    [[maybe_unused]] float m_keep = 0.f, gsum = 0.f;
+    if constexpr (KEEP) m_keep = in && __ldg(sparse + (size_t)b * HW + p) > 0.f ? 1.f : 0.f;
+    const float cblur = KEEP ? kappa - m_keep : kappa;
     float gkappa = 0.f;
     for (int c = 0; c < C; ++c) {
         const size_t plane = ((size_t)b * C + c) * HW;
@@ -283,8 +317,11 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
             continue;
         }
         gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
-        if (grad_blur) grad_blur[plane + p] = fmaf(kappa, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
+        if (grad_blur) grad_blur[plane + p] = fmaf(cblur, gc, __ldg(lam + plane + p));   // lam[0] = lambda_0
+        if constexpr (KEEP) gsum += gc;
     }
+    if constexpr (KEEP)
+        if (in && grad_sparse) grad_sparse[(size_t)b * HW + p] = m_keep * gsum;
     if (!in || !grad_guidance) return;
     if (RAW) {
 #pragma unroll
@@ -318,7 +355,7 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
         a[k] = v;
         S += fabsf(v);
     }
-    const float m = sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
+    const float m = KEEP ? m_keep : sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
     const float om = 1.f - m;
     float Tsum = 0.f;
 #pragma unroll
@@ -337,6 +374,26 @@ gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blu
             grad_guidance[((size_t)b * gch + k) * HW + q] = ga * sg;
         }
     }
+}
+
+template <int R, bool PADDLE = false, bool RAW = false>
+__global__ void __launch_bounds__(256)
+gatherk_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+               const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
+               const float* __restrict__ grad_out, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+               long long n, int N, int C, int H, int W, int gch, int norm_abs) {
+    gatherk_body<R, PADDLE, RAW, false>(guidance, blur, sparse, wk, steps, lam, grad_out, grad_guidance, grad_blur, nullptr, n, N,
+                                        C, H, W, gch, norm_abs);
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+gatherk_keep_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
+                    const float* __restrict__ wk, const float* __restrict__ steps, const float* __restrict__ lam,
+                    const float* __restrict__ grad_out, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
+                    float* __restrict__ grad_sparse, long long n, int N, int C, int H, int W, int gch, int norm_abs) {
+    gatherk_body<R, false, false, true>(guidance, blur, sparse, wk, steps, lam, grad_out, grad_guidance, grad_blur, grad_sparse, n,
+                                        N, C, H, W, gch, norm_abs);
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -387,6 +444,8 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches, 
     const float* wk_all = RAW ? p.guidance : wk_ws;
     float* tmp_all = RAW ? wk_ws : wk_ws + (size_t)p.B * NPL * HW;
     const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(p.out) && aligned16(ws) && (!RAW || aligned16(p.guidance));
+    const bool keep = !PADDLE && p.keep;                 // d0' planes after the ping-pong buffer
+    float* d0_all = tmp_all + (size_t)p.B * plane;
     const int G = group_size(p.B);
     for (int b0 = 0; b0 < p.B; b0 += G) {
         const int nimg = p.B - b0 < G ? p.B - b0 : G;
@@ -394,16 +453,21 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches, 
         const float* blur = p.blur + (size_t)b0 * plane;
         float* out = p.out + (size_t)b0 * plane;
         float* tmp = tmp_all + (size_t)b0 * plane;
+        float* d0 = keep ? d0_all + (size_t)b0 * plane : nullptr;
         if constexpr (!RAW) {
-            launch_prep<R, PADDLE>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr,
-                                   wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+            if (keep)
+                launch_prep_keep(2 * R + 1, p.guidance + (size_t)b0 * p.gch * HW, p.sparse + (size_t)b0 * HW, blur,
+                                 wk_ws + (size_t)b0 * NPL * HW, d0, nimg, p.C, p.H, p.W, p.gch, p.norm_abs, stream);
+            else
+                launch_prep<R, PADDLE>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr,
+                                       wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
             ++*launches;
         }
         const Fan gfan = fan ? offset_fan(*fan, (size_t)b0 * plane) : Fan{};
         const float* cur = blur;
         float* dst = (p.iters & 1) ? out : tmp;   // ping-pong so that the last step writes out
         for (int it = 0; it < p.iters; ++it) {
-            launch_step<R, PADDLE, RAW>(vec, wk, blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream,
+            launch_step<R, PADDLE, RAW>(vec, wk, keep ? d0 : blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream,
                                         fan && it == p.iters - 1 ? &gfan : nullptr);
             ++*launches;
             cur = dst;
@@ -419,7 +483,7 @@ int forward_k(const Problem2D& p, void* ws, cudaStream_t stream, int* launches, 
 // forward steps and the gather, which only feed the gate gradient, are skipped.
 template <int R, bool PADDLE, bool RAW = false>
 int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
-               cudaStream_t stream, int* launches) {
+               cudaStream_t stream, int* launches, float* grad_sparse) {
     constexpr int NPL = RAW ? Taps<R>::NT : Taps<R>::NP;   // weight planes per image
     const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
     const long long n = (long long)p.B * plane;
@@ -430,6 +494,8 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
     float* lam = RAW ? steps + (size_t)(p.iters >= 2 ? p.iters - 2 : 0) * n : steps + (size_t)p.iters * n;
     const bool gates_grad = !RAW || grad_guidance;   // the steps and the gather feed the guidance gradient
     const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(ws) && (!RAW || aligned16(p.guidance));
+    const bool keep = !PADDLE && p.keep;             // d0' planes after the lambdas
+    float* d0_all = lam + (size_t)p.iters * n;
     const int G = group_size(p.B);
     for (int b0 = 0; b0 < p.B; b0 += G) {
         const int nimg = p.B - b0 < G ? p.B - b0 : G;
@@ -438,13 +504,18 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
         const float* blur = p.blur + off;
         const float* guidance = p.guidance + (size_t)b0 * p.gch * HW;
         const float* sparse = p.sparse ? p.sparse + (size_t)b0 * HW : nullptr;
+        float* d0 = keep ? d0_all + off : nullptr;
         if constexpr (!RAW) {
-            launch_prep<R, PADDLE>(guidance, sparse, wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+            if (keep)
+                launch_prep_keep(2 * R + 1, guidance, sparse, blur, wk_ws + (size_t)b0 * NPL * HW, d0, nimg, p.C, p.H, p.W, p.gch,
+                                 p.norm_abs, stream);
+            else
+                launch_prep<R, PADDLE>(guidance, sparse, wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
             ++*launches;
         }
         for (int t = 0; gates_grad && t + 1 < p.iters; ++t) {   // d_{t+1} = step(d_t)
-            launch_step<R, PADDLE, RAW>(vec, wk, blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off, steps + (size_t)t * n + off,
-                           nimg * p.C, p.C, p.H, p.W, stream);
+            launch_step<R, PADDLE, RAW>(vec, wk, keep ? d0 : blur, t == 0 ? blur : steps + (size_t)(t - 1) * n + off,
+                                        steps + (size_t)t * n + off, nimg * p.C, p.C, p.H, p.W, stream);
             ++*launches;
         }
         const dim3 grid((p.W + kSclTW - 1) / kSclTW, (p.H + kSclTH - 1) / kSclTH, nimg * p.C);
@@ -459,10 +530,19 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
             ++*launches;
         }
         if (!gates_grad) continue;
+        float* gg = grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr;
+        if constexpr (!PADDLE) {
+            if (keep) {
+                gatherk_keep_kernel<R><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
+                    guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off, gg, grad_blur ? grad_blur + off : nullptr,
+                    grad_sparse ? grad_sparse + (size_t)b0 * HW : nullptr, n, p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
+                ++*launches;
+                continue;
+            }
+        }
         gatherk_kernel<R, PADDLE, RAW><<<dim3(grid.x, grid.y, nimg), dim3(kSclTW, kSclTH), 0, stream>>>(
-            guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off,
-            grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr, grad_blur && !RAW ? grad_blur + off : nullptr, n,
-            p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
+                guidance, blur, sparse, wk, steps + off, lam + off, grad_out + off, gg, grad_blur && !RAW ? grad_blur + off : nullptr,
+                n, p.iters, p.C, p.H, p.W, p.gch, p.norm_abs);
         ++*launches;
     }
     CSPN_CUDA_TRY(cudaGetLastError());
@@ -520,19 +600,28 @@ int check_launch(const Problem2D& p, int K, const FamilyTraits& t, const char* w
 
 // Normalised and 'paddle': K*K weight planes per image and the ping-pong buffer.  Gates: the caller's gates are the weight
 // planes, and a single step writes `out` directly.
-size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family) {
+// keep (Normalised): the d0' planes of the keep-sparse mode follow
+void launch_prep_keep(int K, const float* guidance, const float* sparse, const float* blur, float* wk, float* d0, int B, int C,
+                      int H, int W, int gch, int norm_abs, cudaStream_t stream) {
+    const dim3 grid((W + 31) / 32, (H + 7) / 8, B), block(32, 8);
+    if (K == 3) prepk_keep_kernel<1><<<grid, block, 0, stream>>>(guidance, sparse, blur, wk, d0, C, H, W, gch, norm_abs);
+    else if (K == 5) prepk_keep_kernel<2><<<grid, block, 0, stream>>>(guidance, sparse, blur, wk, d0, C, H, W, gch, norm_abs);
+    else prepk_keep_kernel<3><<<grid, block, 0, stream>>>(guidance, sparse, blur, wk, d0, C, H, W, gch, norm_abs);
+}
+
+size_t widek_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family, bool keep) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W;
     if (family == Family::Gates) return iters >= 2 ? sizeof(float) * (size_t)B * C * HW : 0;
-    return sizeof(float) * ((size_t)B * K * K * HW + (size_t)B * C * HW);
+    return sizeof(float) * ((size_t)B * K * K * HW + (keep ? 2 : 1) * (size_t)B * C * HW);
 }
 
 // The weight planes as above, then d_1..d_{N-1} and the lambdas: 2N planes of B*C images, 2N-2 for gates (see backward_k)
-size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family) {
+size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, Family family, bool keep) {
     if (iters <= 0) return 0;
     const size_t HW = (size_t)H * W;
     if (family == Family::Gates) return sizeof(float) * (2 * (size_t)iters - 2) * B * C * HW;
-    return sizeof(float) * ((size_t)B * K * K * HW + 2 * (size_t)iters * B * C * HW);
+    return sizeof(float) * ((size_t)B * K * K * HW + (2 * (size_t)iters + (keep ? 1 : 0)) * B * C * HW);
 }
 
 int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
@@ -541,7 +630,8 @@ int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_
         CSPN_CUDA_TRY(cudaMemcpyAsync(p.out, p.blur, (size_t)p.B * p.C * p.H * p.W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const int rc = check_launch(p, K, traits(family), "path", widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family), ws, ws_bytes);
+    const int rc = check_launch(p, K, traits(family), "path", widek_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family, p.keep),
+                                ws, ws_bytes);
     if (rc != CSPN_OK) return rc;
     return with_kernels(K, family, [&](auto R, auto PADDLE, auto RAW) {
         return forward_k<R(), PADDLE(), RAW()>(p, ws, stream, launches, fan);
@@ -549,7 +639,7 @@ int widek_forward(const Problem2D& p, int K, Family family, void* ws, size_t ws_
 }
 
 int widek_backward(const Problem2D& p, int K, Family family, const float* grad_out, float* grad_guidance, float* grad_blur,
-                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
+                   void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, float* grad_sparse) {
     const FamilyTraits& t = traits(family);
     const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
     if (grad_guidance && (t.zero_grad_first || p.iters == 0))
@@ -558,11 +648,12 @@ int widek_backward(const Problem2D& p, int K, Family family, const float* grad_o
         if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
         return CSPN_OK;
     }
-    const int rc = check_launch(p, K, t, "backward", widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family), ws, ws_bytes);
+    const int rc = check_launch(p, K, t, "backward", widek_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, family, p.keep), ws,
+                                ws_bytes);
     if (rc != CSPN_OK) return rc;
     if (t.no_grad_is_no_op && !grad_guidance && !grad_blur) return CSPN_OK;
     return with_kernels(K, family, [&](auto R, auto PADDLE, auto RAW) {
-        return backward_k<R(), PADDLE(), RAW()>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches);
+        return backward_k<R(), PADDLE(), RAW()>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches, grad_sparse);
     });
 }
 

@@ -14,6 +14,11 @@
 //       -> Tensor                                                    (K x K kernel, K in {3, 5, 7}; K = 3 is propagate2d)
 //   propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size,
 //                          int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)
+//   propagate2d_keep(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int kernel_size, int prop_time, int norm_type,
+//                    int algo) -> Tensor           (keep-sparse mode: the samples stay in the output, K in {3, 5, 7})
+//   propagate2d_keep_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size,
+//                             int prop_time, int norm_type, bool need_guidance, bool need_blur, bool need_sparse)
+//       -> (Tensor, Tensor, Tensor)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -186,6 +191,44 @@ std::tuple<at::Tensor, at::Tensor> propagate2d_k_backward_cuda(const at::Tensor&
                               (int)prop_time, (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_k_bwd_f32");
     return {grad_or_empty(gg, g), grad_or_empty(gd, d)};
+}
+
+// Keep-sparse mode, K in {3, 5, 7}: cspn2d_keep_*_f32.  algo picks the 3x3 path as in propagate2d (misaligned views take the
+// generic one under AUTO); a missing sparse_depth is the default mode
+at::Tensor propagate2d_keep_cuda(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                                 int64_t K, int64_t prop_time, int64_t norm_type, int64_t algo) {
+    check2d_k(guidance, blur, sparse, K);
+    if (prop_time == 0) return blur.clone();
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(d);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    int a = (int)algo;
+    auto misaligned = [](const at::Tensor& t) { return t.defined() && (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0; };
+    if (a == CSPN_ALGO_AUTO && (misaligned(g) || misaligned(d) || misaligned(s) || misaligned(out))) a = CSPN_ALGO_GENERIC;
+    const Workspace ws(cspn2d_keep_workspace_bytes(B, C, H, W, (int)K, (int)prop_time, a), d);
+    check_rc(cspn2d_keep_fwd_f32(fptr(g), fptr(d), fptr(s), mptr(out), B, C, H, W, (int)g.size(1), (int)K, (int)prop_time,
+                                 (int)norm_type, a, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_keep_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor> propagate2d_keep_backward_cuda(
+        const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse, const at::Tensor& grad_out,
+        int64_t K, int64_t prop_time, int64_t norm_type, bool need_g, bool need_d, bool need_s) {
+    check2d_k(guidance, blur, sparse, K);
+    check_grad_out(grad_out, blur, "blur_depth");
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gd = new_grad(need_d, d), gs = s.defined() ? new_grad(need_s, s) : at::Tensor();
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const Workspace ws(cspn2d_keep_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), d);
+    check_rc(cspn2d_keep_bwd_f32(fptr(g), fptr(d), fptr(s), fptr(go), mptr(gg), mptr(gd), mptr(gs), B, C, H, W, (int)g.size(1),
+                                 (int)K, (int)prop_time, (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_keep_bwd_f32");
+    return {grad_or_empty(gg, g), grad_or_empty(gd, d), grad_or_empty(gs, d)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -454,6 +497,10 @@ TORCH_LIBRARY(cspn_b200, m) {
           "int norm_type) -> Tensor");
     m.def("propagate2d_k_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size, "
           "int prop_time, int norm_type, bool need_guidance, bool need_blur) -> (Tensor, Tensor)");
+    m.def("propagate2d_keep(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, int kernel_size, int prop_time, "
+          "int norm_type, int algo) -> Tensor");
+    m.def("propagate2d_keep_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size, "
+          "int prop_time, int norm_type, bool need_guidance, bool need_blur, bool need_sparse) -> (Tensor, Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -479,6 +526,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_backward", &propagate2d_backward_cuda);
     m.impl("propagate2d_k", &propagate2d_k_cuda);
     m.impl("propagate2d_k_backward", &propagate2d_k_backward_cuda);
+    m.impl("propagate2d_keep", &propagate2d_keep_cuda);
+    m.impl("propagate2d_keep_backward", &propagate2d_keep_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

@@ -79,8 +79,11 @@ class FusedGather:
         self.hdl.barrier()            # every rank's kernel (and with it its remote stores) is complete
         return self.buf
 
-    def propagate(self, guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum'):
-        """propagate2d (3x3) on the cluster kernel, which must be able to take the shape."""
+    def propagate(self, guidance, blur_depth, sparse_depth=None, prop_time=24, norm_type='8sum', keep_sparse=False):
+        """propagate2d (3x3) on the cluster kernel, which must be able to take the shape.  keep_sparse: as in propagate2d."""
+        if keep_sparse:
+            return self.propagate_k(guidance, blur_depth, sparse_depth, 3, prop_time, ('8sum', '8sum_abs')[_lib.NORM2D[norm_type]],
+                                    keep_sparse=True)
         self._check_shape(blur_depth)
         B, C, H, W = self.shape
         g, d = guidance.contiguous(), blur_depth.contiguous()
@@ -89,14 +92,19 @@ class FusedGather:
         return self._gather('cspn2d_fwd_gather_f32', d.device, [_ptr(g), _ptr(d), _ptr(s)],
                             [B, C, H, W, g.shape[1], int(prop_time), _lib.NORM2D[norm_type]], ws_bytes)
 
-    def propagate_k(self, guidance, blur_depth, sparse_depth=None, prop_kernel=5, prop_time=24, norm_type=None):
-        """propagate2d_k.  K = 3 is `propagate` (the cluster kernel); K = 5 and 7 take any W."""
+    def propagate_k(self, guidance, blur_depth, sparse_depth=None, prop_kernel=5, prop_time=24, norm_type=None, keep_sparse=False):
+        """propagate2d_k.  K = 3 is `propagate` (the cluster kernel); K = 5 and 7 take any W.  keep_sparse: as in
+        propagate2d_k (cspn2d_keep_fwd_gather_f32)."""
         code = norm_code_2d_k(prop_kernel, norm_type)
         _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel)
         self._check_shape(blur_depth)
         B, C, H, W = self.shape
         g, d = guidance.contiguous(), blur_depth.contiguous()
         s = None if sparse_depth is None else sparse_depth.contiguous()
+        if keep_sparse:
+            ws_bytes = _lib.lib().cspn2d_keep_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time), _lib.ALGO_CLUSTER)
+            return self._gather('cspn2d_keep_fwd_gather_f32', d.device, [_ptr(g), _ptr(d), _ptr(s)],
+                                [B, C, H, W, g.shape[1], prop_kernel, int(prop_time), code], ws_bytes)
         ws_bytes = _lib.lib().cspn2d_k_workspace_bytes(B, C, H, W, prop_kernel, int(prop_time))
         return self._gather('cspn2d_k_fwd_gather_f32', d.device, [_ptr(g), _ptr(d), _ptr(s)],
                             [B, C, H, W, g.shape[1], prop_kernel, int(prop_time), code], ws_bytes)

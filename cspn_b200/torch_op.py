@@ -69,6 +69,37 @@ def _register():
         gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
         return gg, gd
 
+    @lib.register_fake('cspn_b200::propagate2d_keep')
+    def _(guidance, blur_depth, sparse_depth, kernel_size, prop_time, norm_type, algo):
+        torch._check(guidance.dim() == 4 and blur_depth.dim() == 4, lambda: 'guidance and blur_depth must be (B,C,H,W)')
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        torch._check(guidance.shape[1] >= kernel_size * kernel_size - 1,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs >= {kernel_size * kernel_size - 1} guidance channels')
+        return torch.empty_like(blur_depth, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_keep_backward')
+    def _(guidance, blur_depth, sparse_depth, grad_out, kernel_size, prop_time, norm_type, need_guidance, need_blur, need_sparse):
+        gg = torch.empty_like(guidance, memory_format=torch.contiguous_format) if need_guidance else guidance.new_empty(0)
+        gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
+        gs = (torch.empty_like(sparse_depth, memory_format=torch.contiguous_format) if need_sparse and sparse_depth is not None
+              else blur_depth.new_empty(0))
+        return gg, gd, gs
+
+    def setup2d_keep(ctx, inputs, output):
+        guidance, blur_depth, sparse_depth, kernel_size, prop_time, norm_type, algo = inputs
+        ctx.save_for_backward(guidance, blur_depth, sparse_depth)
+        ctx.cfg = (kernel_size, prop_time, norm_type)
+
+    def backward2d_keep(ctx, grad_out):
+        guidance, blur_depth, sparse_depth = ctx.saved_tensors
+        kernel_size, prop_time, norm_type = ctx.cfg
+        need_g, need_d, need_s = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        gg, gd, gs = torch.ops.cspn_b200.propagate2d_keep_backward(guidance, blur_depth, sparse_depth, grad_out.contiguous(),
+                                                                   kernel_size, prop_time, norm_type, need_g, need_d, need_s)
+        return (gg if need_g else None), (gd if need_d else None), (gs if need_s else None), None, None, None, None
+
+    lib.register_autograd('cspn_b200::propagate2d_keep', backward2d_keep, setup_context=setup2d_keep)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

@@ -159,6 +159,42 @@ CSPN_API int cspn2d_k_fwd_gather_f32(const float* guidance, const float* blur, c
                             int B, int C, int H, int W, int guidance_channels, int K, int iters, int norm_type,
                             void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D keep-sparse mode, K in {3, 5, 7}: the sparse samples are kept in the output (DESIGN.md section 4.13) ---------
+ * The replacement step of the CSPN paper, H <- (1 - m) H + m sparse with m = 1[sparse > 0], in place of the reference
+ * module's m = sign(sparse) and "+ m * blur":
+ *   m = 1[sparse > 0] (NaN, 0 and negative samples -> 0);  d = blur;
+ *   each of iters steps:  e = (1 - s) blur + sum_k w_k shift_k(d),  d = (1 - m) e + m sparse
+ * with w_k, s = sum_k w_k and the taps of the K x K calls above, IEEE as written (0 * NaN = NaN, 0 * inf = NaN).  sparse
+ * [B][1][H][W] is shared by the C channels of blur; a NULL sparse gives the default mode's bits (the K x K and 3x3 calls
+ * above).  Arguments, shapes and status codes as in cspn2d_k_fwd_f32 / cspn2d_k_bwd_f32; `algo` (cspn_algo) chooses the
+ * 3x3 path as in cspn2d_fwd_f32 and is ignored for K = 5 / 7, where the CSPN_B200_FORCE_* hooks do not apply either.
+ * Workspace: K = 3 cluster plans as cspn2d_workspace_bytes; the launch-per-step paths (3x3 generic, K = 5 / 7) one
+ * B*C*H*W plane more than the default mode's (d0' = (1 - m) blur + m sparse).  CSPN_ALGO_AUTO reports
+ * CSPN_ERR_WORKSPACE as cspn2d_fwd_f32 does when a problem it sized for the cluster kernel falls back to the generic path.
+ * The gather entry takes peer_out / n_peer / multicast_out after `out` as cspn2d_k_fwd_gather_f32 does (K = 3 on the
+ * cluster kernel's epilogue, CSPN_ERR_UNSUPPORTED for a shape it cannot take; K = 5 / 7 on the last step).
+ * The backward writes grad_guidance [B][guidance_channels][H][W], grad_blur [B][C][H][W] and
+ * grad_sparse [B][1][H][W] = m * sum_c Gc_c (Gc_c = sum_t lambda_{t+1,c}; the channels summed in order, no atomics); any
+ * of the three may be NULL.  grad_sparse is zero for a NULL sparse or iters == 0.  CUDA device pointers only: there is no
+ * host-buffer entry. */
+CSPN_API size_t cspn2d_keep_workspace_bytes(int B, int C, int H, int W, int K, int iters, int algo);
+
+CSPN_API int cspn2d_keep_fwd_f32(const float* guidance, const float* blur, const float* sparse, float* out,
+                        int B, int C, int H, int W, int guidance_channels, int K, int iters, int norm_type,
+                        int algo, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API int cspn2d_keep_fwd_gather_f32(const float* guidance, const float* blur, const float* sparse, float* out,
+                               float* const* peer_out, int n_peer, float* multicast_out,
+                               int B, int C, int H, int W, int guidance_channels, int K, int iters, int norm_type,
+                               void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_keep_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_keep_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
+                        float* grad_guidance, float* grad_blur, float* grad_sparse, int B, int C, int H, int W,
+                        int guidance_channels, int K, int iters, int norm_type,
+                        void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
