@@ -15,6 +15,10 @@
 // Semantics follow the reference line by line: valid = gt > 0.0001 (utils.py:21, loss.py:17); diff = |gt - pred|;
 // rel = diff / gt; max_ratio = max(gt / pred, pred / gt) with IEEE division (the deltas count `max_ratio < t`, so the
 // quotient's rounding decides ties and must be the reference's); n_valid == 0 leaves everything 0 (utils.py:31).
+// Deviations, all specified in DESIGN.md section 4.7: diff is squared and everything summed in double, and RMSE is the root
+// of the double mean (the reference squares and sums in float: a diff above 1.8e19 makes its MSE and RMSE inf); out[0] is
+// n_valid rounded to float, so above 2^24 the backward inverts the rounded count (at most 1 ulp in the gradient's scale);
+// with n_valid == 0 the backward writes zeros, where the reference's loss is 0 / 0.
 #include "common.cuh"
 
 namespace cspn {
@@ -41,9 +45,10 @@ metrics_partial_kernel(const float* __restrict__ pred, const float* __restrict__
             for (int t = 0; t < 6; ++t) s[4 + t] += (ratio < thr[t]) ? 1.0 : 0.0;
         }
     }
-    // (torch.max propagates NaN, fmaxf drops it; either way `NaN < t` and `x < t` for the surviving operand: a NaN ratio
-    //  arises only from pred == 0 / 0-over-0 cases where the other quotient is inf or NaN as well -> the comparison is false
-    //  in both formulations.)
+    // (torch.max propagates NaN, fmaxf drops it.  The two agree here because g / p is NaN exactly when p / g is: a NaN
+    //  operand, or both infinite -- g == 0 is not valid.  Then both formulations compare NaN < t, false.  A ratio of -0 or
+    //  below, from p == -0, p < 0 or p == -inf, is counted under every threshold, as the reference counts it.
+    //  tests/golden/metrics/edges/ holds the reference's own results for each of these.)
 #pragma unroll
     for (int i = 0; i < kSums; ++i) {
         double v = s[i];

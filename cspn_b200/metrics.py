@@ -67,7 +67,17 @@ class _MaskedL1(torch.autograd.Function):
 
 class Wighted_L1_Loss(nn.Module):
     """Same name (typo included) and call as the reference's criterion (loss.py:12-23): mean |pred - label| over label > 1e-4.
-    Forward and backward are single CUDA passes; the returned loss is a 0-d CUDA tensor."""
+    Forward and backward are single CUDA passes; the returned loss is a 0-d CUDA tensor.  fp32 CUDA tensors of one shape,
+    any rank and layout; usable on any stream and inside a CUDA graph.
+
+    The gradient with respect to pred is sign(pred - label) * fl(fl(1 / n_valid) * grad_loss) where label > 1e-4 (0 where
+    pred == label or the difference is NaN) and 0 elsewhere; label gets none, and a second derivative is refused.  The
+    count reaches the backward as a float: above 2^24 valid pixels it is rounded to even first, which moves the scale by
+    at most one ulp.
+
+    With no valid pixel the loss is 0 and its gradient all zeros.  The reference returns 0 / 0 = NaN there (the sum of an
+    empty selection over a count of zero, loss.py:22); a frame without ground truth would then poison every weight of a
+    training run, so this deviation is deliberate (DESIGN.md section 4.7)."""
 
     def forward(self, pred, label):
         return _MaskedL1.apply(pred, label)
