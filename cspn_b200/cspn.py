@@ -10,6 +10,7 @@ device memory, the current stream and autograd plumbing.  There is no CPU / eage
 import torch
 import torch.nn as nn
 
+import operator
 import os
 
 from . import _lib, torch_op
@@ -925,3 +926,103 @@ class Simple_Gudi_UpConv_Block_Last_Layer(nn.Module):
 
     def extra_repr(self):
         return f'oheight={self.oheight}, owidth={self.owidth}'
+
+
+# ---- trilinear resampling: the Paddle module's resize_trilinear (fluid.layers.resize_trilinear) -----------------------
+def resize_output_size(in_shape, out_shape=None, scale=None):
+    """The output's (D, H, W): out_shape as given, or int(n * scale) per axis; exactly one of the two, every size >= 1."""
+    if (out_shape is None) == (scale is None):
+        raise ValueError('give exactly one of out_shape and scale')
+    if out_shape is not None:
+        try:
+            sizes = tuple(operator.index(n) for n in out_shape if not isinstance(n, bool))
+        except TypeError:
+            sizes = ()
+        if len(sizes) != 3 or len(tuple(out_shape)) != 3:
+            raise ValueError(f'out_shape must be three ints, got {out_shape!r}')
+    else:
+        if isinstance(scale, bool) or not isinstance(scale, (int, float)) or not scale > 0:
+            raise ValueError(f'scale must be a number > 0, got {scale!r}')
+        sizes = tuple(int(n * scale) for n in in_shape)
+    if min(sizes) < 1:
+        raise ValueError(f'every output size must be >= 1, got {sizes}')
+    return sizes
+
+
+def _check_resize_sizes(in_shape, out_size):
+    """The C ABI takes int sizes and < 2^31 elements per (B*C) slice: refuse what it cannot take before anything is allocated
+    or narrowed to int."""
+    B, C, d, h, w = in_shape
+    if max(B, C) > 2 ** 31 - 1 or d * h * w >= 2 ** 31 or out_size[0] * out_size[1] * out_size[2] >= 2 ** 31:
+        raise _lib.CspnError(f'resize_trilinear takes B, C < 2^31 and < 2^31 elements per (B*C) slice, got input '
+                             f'{tuple(in_shape)} and output size {tuple(out_size)}')
+
+
+def _resize_fwd(x, D, H, W, align_corners, align_mode):
+    """Forward only (no autograd) through cspn_resize_trilinear_fwd_f32, enqueued on the current stream."""
+    xc = x.contiguous()
+    out = xc.new_empty((*xc.shape[:2], D, H, W))
+    if out.numel():
+        with torch.cuda.device(xc.device):
+            rc = _lib.lib().cspn_resize_trilinear_fwd_f32(_ptr(xc), _ptr(out), *xc.shape, D, H, W, int(align_corners),
+                                                          align_mode, _stream(xc.device))
+        _lib.check(rc, 'cspn_resize_trilinear_fwd_f32')
+    return out
+
+
+def _resize_bwd(grad_out, in_size, align_corners, align_mode):
+    go = grad_out.contiguous()
+    gx = go.new_empty((*go.shape[:2], *in_size))
+    if gx.numel():
+        L = _lib.lib()
+        with torch.cuda.device(go.device):
+            ws_bytes = L.cspn_resize_trilinear_bwd_workspace_bytes(*in_size, *go.shape[2:])
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=go.device)
+            rc = L.cspn_resize_trilinear_bwd_f32(_ptr(go), _ptr(gx), *go.shape[:2], *in_size, *go.shape[2:], int(align_corners),
+                                                 align_mode, _ptr(ws), ws_bytes, _stream(go.device))
+        _lib.check(rc, 'cspn_resize_trilinear_bwd_f32')
+    return gx
+
+
+class _ResizeTrilinearFn(torch.autograd.Function):
+    """autograd seam of resize_trilinear without the torch-op shim: native forward + native gather backward.  The
+    backward needs the input's size only, so no tensor is saved."""
+
+    @staticmethod
+    def forward(ctx, x, D, H, W, align_corners, align_mode):
+        ctx.cfg = (tuple(x.shape[2:]), align_corners, align_mode)
+        return _resize_fwd(x, D, H, W, align_corners, align_mode)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        return _resize_bwd(grad_out, *ctx.cfg), None, None, None, None, None
+
+
+def resize_trilinear(input, out_shape=None, scale=None, align_corners=True, align_mode=1):
+    """fluid.layers.resize_trilinear on (B, C, D, H, W) fp32 CUDA tensors, forward and a deterministic backward.
+    Per axis n_in -> n_out, in fp32: r = (n_in-1)/(n_out-1) with align_corners, else n_in/n_out (0 when n_out == 1);
+    source s(o) = max(r*(o+0.5) - 0.5, 0) with align_corners=False and align_mode=0, else r*o; then the trilinear blend of
+    the 8 voxels around s.  Give exactly one of out_shape (three ints) or scale (n_out = int(n_in * scale)).
+    align_corners=True is F.interpolate(..., align_corners=True), align_corners=False with align_mode=0 is
+    F.interpolate(..., align_corners=False) (for n_out > 1); align_mode=1 has no PyTorch twin.  DESIGN.md section 4.14."""
+    if input.dim() != 5:
+        raise ValueError(f'input must be (B,C,D,H,W), got {tuple(input.shape)}')
+    if align_mode not in (0, 1) or isinstance(align_mode, bool):
+        raise ValueError(f'align_mode must be 0 or 1, got {align_mode!r}')
+    if min(input.shape[2:]) < 1:
+        raise ValueError(f'the input volume must not be empty, got {tuple(input.shape)}')
+    D, H, W = resize_output_size(input.shape[2:], out_shape, scale)
+    _check_resize_sizes(input.shape, (D, H, W))
+    align_corners = bool(align_corners)
+    if input.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if not input.is_cuda:
+        raise _lib.CspnError('resize_trilinear takes CUDA tensors only (there is no host-buffer entry point for it)')
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.resize_trilinear(input, D, H, W, align_corners, align_mode)
+    if torch.is_grad_enabled() and input.requires_grad:
+        return _ResizeTrilinearFn.apply(input, D, H, W, align_corners, align_mode)
+    return _resize_fwd(input, D, H, W, align_corners, align_mode)

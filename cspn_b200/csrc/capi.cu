@@ -661,6 +661,82 @@ int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, const float
     });
 }
 
+// ---- trilinear resampling (the Paddle module's resize_trilinear) --------------------------------------------------------
+// Bytes of a (B*C) x n fp32 tensor, saturated at the top of the address space
+static uintptr_t span_bytes(int B, int C, long long n) {
+    const unsigned long long lim = ~0ull / 4 / (unsigned long long)n;
+    const unsigned long long bc = (unsigned long long)B * C;
+    return bc > lim ? ~(uintptr_t)0 : (uintptr_t)(bc * n * 4);
+}
+
+static bool overlap(const void* a, uintptr_t na, const void* b, uintptr_t nb) {
+    const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+    const uintptr_t ea = na > ~pa ? ~(uintptr_t)0 : pa + na, eb = nb > ~pb ? ~(uintptr_t)0 : pb + nb;
+    return pa < eb && pb < ea;
+}
+
+// src is read and dst written: x and out in the forward, grad_out and grad_x in the backward
+static int check_resize(const void* src, const void* dst, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                        int align_corners, int align_mode, bool backward) {
+    if (!src || !dst) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!positive(B, C, D, H, W, Do, Ho, Wo)) {
+        set_error("non-positive size B=%d C=%d D=%d H=%d W=%d Do=%d Ho=%d Wo=%d", B, C, D, H, W, Do, Ho, Wo);
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (align_corners != 0 && align_corners != 1) { set_error("align_corners must be 0 or 1, got %d", align_corners); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (align_mode != 0 && align_mode != 1) { set_error("align_mode must be 0 or 1, got %d", align_mode); return CSPN_ERR_INVALID_ARGUMENT; }
+    if ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 3) {
+        set_error("tensor pointers must be 4-byte aligned");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    const char* why = "";
+    if (!resize_trilinear_launchable(D, H, W, Do, Ho, Wo, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    const long long vin = (long long)D * H * W, vout = (long long)Do * Ho * Wo;
+    if (overlap(src, span_bytes(B, C, backward ? vout : vin), dst, span_bytes(B, C, backward ? vin : vout))) {
+        set_error("%s overlaps %s", backward ? "grad_x" : "out", backward ? "grad_out" : "x");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    return CSPN_OK;
+}
+
+int cspn_resize_trilinear_fwd_f32(const float* x, float* out, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                                  int align_corners, int align_mode, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_resize(x, out, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode, false);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(x, "x", [&](int* launches) {
+        return resize_trilinear_forward(x, out, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners, align_mode,
+                                        (cudaStream_t)stream, launches);
+    });
+}
+
+size_t cspn_resize_trilinear_bwd_workspace_bytes(int D, int H, int W, int Do, int Ho, int Wo) {
+    if (!positive(D, H, W, Do, Ho, Wo)) return 0;
+    return resize_trilinear_bwd_workspace_bytes(D, H, W, Do, Ho, Wo);
+}
+
+int cspn_resize_trilinear_bwd_f32(const float* grad_out, float* grad_x, int B, int C, int D, int H, int W, int Do, int Ho,
+                                  int Wo, int align_corners, int align_mode, void* workspace, size_t workspace_bytes,
+                                  cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_resize(grad_out, grad_x, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode, true);
+    if (rc != CSPN_OK) return rc;
+    const size_t need = resize_trilinear_bwd_workspace_bytes(D, H, W, Do, Ho, Wo);
+    if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 7)) {
+        set_error("the backward needs %zu bytes of 8-byte aligned workspace (got %zu)", need, workspace_bytes);
+        return CSPN_ERR_WORKSPACE;
+    }
+    const long long vin = (long long)D * H * W, vout = (long long)Do * Ho * Wo;
+    if (overlap(workspace, need, grad_x, span_bytes(B, C, vin)) || overlap(workspace, need, grad_out, span_bytes(B, C, vout))) {
+        set_error("the workspace overlaps %s", overlap(workspace, need, grad_x, span_bytes(B, C, vin)) ? "grad_x" : "grad_out");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    return on_device_of(grad_out, "grad_out", [&](int* launches) {
+        return resize_trilinear_backward(grad_out, grad_x, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners, align_mode,
+                                         workspace, (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

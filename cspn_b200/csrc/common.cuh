@@ -171,4 +171,13 @@ int unpool_conv_forward(const float* x, const float* w, float* out, int B, int C
 int unpool_conv_backward(const float* x, const float* w, const float* g, float* gx, float* gw, int B, int Cin, int h, int wd,
                          int Cout, int H, int W, void* ws, cudaStream_t st, int* launches);
 
+// Trilinear resampling, the Paddle module's resize_trilinear (resize_trilinear.cu); arguments checked by the caller.
+// slices = B*C; (D, H, W) the input's size and (Do, Ho, Wo) the output's
+int resize_trilinear_launchable(int D, int H, int W, int Do, int Ho, int Wo, const char** why);
+size_t resize_trilinear_bwd_workspace_bytes(int D, int H, int W, int Do, int Ho, int Wo);
+int resize_trilinear_forward(const float* x, float* out, long long slices, int D, int H, int W, int Do, int Ho, int Wo,
+                             int align_corners, int align_mode, cudaStream_t st, int* launches);
+int resize_trilinear_backward(const float* grad_out, float* grad_x, long long slices, int D, int H, int W, int Do, int Ho,
+                              int Wo, int align_corners, int align_mode, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

@@ -40,6 +40,10 @@
 //       (the guidance / depth head: Unpool, crop to H x W, 3x3 convolution; x (B, Cin, h, w), weight (Cout, Cin, 3, 3))
 //   unpool_conv3x3_backward(Tensor x, Tensor weight, Tensor grad_out, int H, int W, bool need_x, bool need_weight)
 //       -> (Tensor, Tensor)
+//   resize_trilinear(Tensor input, int D, int H, int W, bool align_corners, int align_mode) -> Tensor
+//       (fluid.layers.resize_trilinear: input (B, C, d, h, w) resampled to (B, C, D, H, W))
+//   resize_trilinear_backward(Tensor grad_out, int in_D, int in_H, int in_W, bool align_corners, int align_mode) -> Tensor
+//       (grad_input (B, C, in_D, in_H, in_W) from grad_out alone: the backward needs the input's size only)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -487,6 +491,54 @@ std::tuple<at::Tensor, at::Tensor> unpool_conv3x3_backward_cuda(const at::Tensor
     return {grad_or_empty(gx, xc), grad_or_empty(gw, wc)};
 }
 
+// a * b * c < 2^31 for non-negative sizes, without overflowing int64
+bool volume_fits_int(int64_t a, int64_t b, int64_t c) {
+    constexpr int64_t kLimit = (int64_t)1 << 31;
+    return a < kLimit && b < kLimit && c < kLimit && a * b < kLimit && a * b * c < kLimit;
+}
+
+// Trilinear resampling (the Paddle module's resize_trilinear): (B, C, d, h, w) <-> (B, C, D, H, W)
+void check_resize(const at::Tensor& t, int64_t D, int64_t H, int64_t W, int64_t align_mode, const char* name) {
+    TORCH_CHECK_VALUE(t.dim() == 5, name, " must be (B,C,D,H,W), got ", t.sizes());
+    TORCH_CHECK_VALUE(D >= 1 && H >= 1 && W >= 1, "sizes must be >= 1, got ", D, "x", H, "x", W);
+    TORCH_CHECK_VALUE(align_mode == 0 || align_mode == 1, "align_mode must be 0 or 1, got ", align_mode);
+    TORCH_CHECK(t.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    // the C ABI takes int sizes and < 2^31 elements per (B*C) slice: refuse the rest before allocating or narrowing to int
+    TORCH_CHECK(t.size(0) < ((int64_t)1 << 31) && t.size(1) < ((int64_t)1 << 31) && volume_fits_int(t.size(2), t.size(3), t.size(4)) &&
+                    volume_fits_int(D, H, W),
+                "resize_trilinear takes B, C < 2^31 and < 2^31 elements per (B*C) slice, got ", name, " ", t.sizes(), " and ",
+                D, "x", H, "x", W);
+}
+
+at::Tensor resize_trilinear_cuda(const at::Tensor& x, int64_t D, int64_t H, int64_t W, bool align_corners, int64_t align_mode) {
+    check_resize(x, D, H, W, align_mode, "input");
+    const c10::cuda::CUDAGuard guard(x.device());
+    const at::Tensor xc = x.contiguous();
+    at::Tensor out = at::empty({xc.size(0), xc.size(1), D, H, W}, xc.options());
+    if (out.numel())
+        check_rc(cspn_resize_trilinear_fwd_f32(fptr(xc), mptr(out), (int)xc.size(0), (int)xc.size(1), (int)xc.size(2),
+                                               (int)xc.size(3), (int)xc.size(4), (int)D, (int)H, (int)W, align_corners,
+                                               (int)align_mode, current_stream()),
+                 "cspn_resize_trilinear_fwd_f32");
+    return out;
+}
+
+at::Tensor resize_trilinear_backward_cuda(const at::Tensor& grad_out, int64_t D, int64_t H, int64_t W, bool align_corners,
+                                          int64_t align_mode) {
+    check_resize(grad_out, D, H, W, align_mode, "grad_out");
+    const c10::cuda::CUDAGuard guard(grad_out.device());
+    const at::Tensor go = grad_out.contiguous();
+    at::Tensor gx = at::empty({go.size(0), go.size(1), D, H, W}, go.options());
+    const int Do = (int)go.size(2), Ho = (int)go.size(3), Wo = (int)go.size(4);
+    if (gx.numel()) {
+        const Workspace ws(cspn_resize_trilinear_bwd_workspace_bytes((int)D, (int)H, (int)W, Do, Ho, Wo), go);
+        check_rc(cspn_resize_trilinear_bwd_f32(fptr(go), mptr(gx), (int)go.size(0), (int)go.size(1), (int)D, (int)H, (int)W, Do,
+                                               Ho, Wo, align_corners, (int)align_mode, ws.ptr(), ws.bytes, current_stream()),
+                 "cspn_resize_trilinear_bwd_f32");
+    }
+    return gx;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -519,6 +571,8 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("unpool_conv3x3(Tensor x, Tensor weight, int H, int W) -> Tensor");
     m.def("unpool_conv3x3_backward(Tensor x, Tensor weight, Tensor grad_out, int H, int W, bool need_x, bool need_weight) "
           "-> (Tensor, Tensor)");
+    m.def("resize_trilinear(Tensor input, int D, int H, int W, bool align_corners, int align_mode) -> Tensor");
+    m.def("resize_trilinear_backward(Tensor grad_out, int in_D, int in_H, int in_W, bool align_corners, int align_mode) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -540,4 +594,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("affinity_propagate3d_backward", &affinity_propagate3d_backward_cuda);
     m.impl("unpool_conv3x3", &unpool_conv3x3_cuda);
     m.impl("unpool_conv3x3_backward", &unpool_conv3x3_backward_cuda);
+    m.impl("resize_trilinear", &resize_trilinear_cuda);
+    m.impl("resize_trilinear_backward", &resize_trilinear_backward_cuda);
 }

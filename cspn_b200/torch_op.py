@@ -245,6 +245,26 @@ def _register():
 
     lib.register_autograd('cspn_b200::unpool_conv3x3', backward_unpool, setup_context=setup_unpool)
 
+    @lib.register_fake('cspn_b200::resize_trilinear')
+    def _(x, D, H, W, align_corners, align_mode):
+        torch._check(x.dim() == 5, lambda: 'input must be (B,C,D,H,W)')
+        torch._check(D >= 1 and H >= 1 and W >= 1 and align_mode in (0, 1), lambda: 'sizes >= 1 and align_mode 0 or 1')
+        return x.new_empty((x.shape[0], x.shape[1], D, H, W))
+
+    @lib.register_fake('cspn_b200::resize_trilinear_backward')
+    def _(grad_out, D, H, W, align_corners, align_mode):
+        torch._check(grad_out.dim() == 5, lambda: 'grad_out must be (B,C,D,H,W)')
+        return grad_out.new_empty((grad_out.shape[0], grad_out.shape[1], D, H, W))
+
+    def setup_resize(ctx, inputs, output):        # the backward needs the input's size only: no tensor is saved
+        x, D, H, W, align_corners, align_mode = inputs
+        ctx.cfg = (*x.shape[2:], align_corners, align_mode)
+
+    def backward_resize(ctx, grad_out):
+        return torch.ops.cspn_b200.resize_trilinear_backward(grad_out.contiguous(), *ctx.cfg), None, None, None, None, None
+
+    lib.register_autograd('cspn_b200::resize_trilinear', backward_resize, setup_context=setup_resize)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

@@ -372,6 +372,32 @@ CSPN_API int cspn_unpool_conv3x3_bwd_f32(const float* x, const float* weight, co
                                 float* grad_weight, int B, int Cin, int h, int w, int Cout, int H, int W,
                                 void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- trilinear resampling: the Paddle module's resize_trilinear ---------------------------------------------------
+ * fluid.layers.resize_trilinear (one of the Paddle wheel's two custom ops, cspn_paddle/README.md:24): x [B][C][D][H][W] -> out
+ * [B][C][Do][Ho][Wo].  Per axis n_in -> n_out, in fp32, every operation rounded on its own:
+ *   r = (n_in-1)/(n_out-1) if align_corners, else n_in/n_out; r = 0 when n_out == 1
+ *   s(o) = max(r*(o+0.5) - 0.5, 0) if !align_corners && align_mode == 0, else r*o
+ *   i0 = (int)s, i1 = i0 + (i0 < n_in-1), l1 = s - i0, l0 = 1 - l1
+ *   out = l0d*(l0h*(l0w*x[d0,h0,w0] + l1w*x[d0,h0,w1]) + l1h*(...h1...)) + l1d*(...d1...), every product computed.
+ * The backward is a gather (no atomics): grad_x[d,h,w] = sum_od (sum_oh (sum_ow g*ww) * wh) * wd over the outputs that read
+ * the voxel, each sum from 0 in ascending o; the weight of (o, i) is l0 if i0(o) == i, else l1, and where i1 == i0 == i
+ * both products are added (l0 first).  The bits depend on the arguments only (DESIGN.md section 4.14).
+ * align_corners and align_mode are 0 or 1 (align_mode matters only without align_corners).  Every pointer 4-byte aligned;
+ * out / grad_x must not overlap x / grad_out, nor the workspace either of them.  The forward launches one kernel and needs no workspace; the backward
+ * launches two and writes every grad_x element.  Its workspace, cspn_resize_trilinear_bwd_workspace_bytes() bytes,
+ * 8-byte aligned, depends on the six sizes alone (0 for a non-positive one).  No allocation, no synchronisation.
+ * CSPN_ERR_INVALID_ARGUMENT for a null pointer, a non-positive size, an align flag outside {0, 1}, a misaligned or an
+ * overlapping pointer (a workspace overlapping grad_x or grad_out included); CSPN_ERR_WORKSPACE for a missing, short or misaligned workspace; CSPN_ERR_UNSUPPORTED for an input
+ * or output with >= 2^31 elements per (B*C) slice.  Any B*C is taken. */
+CSPN_API int cspn_resize_trilinear_fwd_f32(const float* x, float* out, int B, int C, int D, int H, int W, int Do, int Ho,
+                                  int Wo, int align_corners, int align_mode, cspn_stream_t stream);
+
+CSPN_API size_t cspn_resize_trilinear_bwd_workspace_bytes(int D, int H, int W, int Do, int Ho, int Wo);
+
+CSPN_API int cspn_resize_trilinear_bwd_f32(const float* grad_out, float* grad_x, int B, int C, int D, int H, int W, int Do,
+                                  int Ho, int Wo, int align_corners, int align_mode, void* workspace,
+                                  size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
