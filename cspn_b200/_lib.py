@@ -68,6 +68,9 @@ SIGNATURES = {
     'cspn_resize_trilinear_fwd_f32': (_i, [_vp] * 2 + [_i] * 10 + [_vp]),
     'cspn_resize_trilinear_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn_resize_trilinear_bwd_f32': (_i, [_vp] * 2 + [_i] * 10 + [_vp, _sz, _vp]),
+    'cspn_disparity_regression_fwd_f32': (_i, [_vp] * 2 + [_i] * 10 + [_vp]),
+    'cspn_disparity_regression_bwd_workspace_bytes': (_sz, [_i] * 6),
+    'cspn_disparity_regression_bwd_f32': (_i, [_vp] * 3 + [_i] * 10 + [_vp, _sz, _vp]),
     'cspn_host_alloc': (_vp, [_sz]),
     'cspn_host_free': (None, [_vp]),
     'cspn_last_error': (_cp, []),

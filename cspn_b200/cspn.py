@@ -1026,3 +1026,76 @@ def resize_trilinear(input, out_shape=None, scale=None, align_corners=True, alig
     if torch.is_grad_enabled() and input.requires_grad:
         return _ResizeTrilinearFn.apply(input, D, H, W, align_corners, align_mode)
     return _resize_fwd(input, D, H, W, align_corners, align_mode)
+
+
+# ---- disparity regression from a low-resolution cost volume: resize_trilinear, softmax over d, expectation ------------
+def _disparity_fwd(cost, D, H, W, align_corners, align_mode):
+    """Forward only (no autograd) through cspn_disparity_regression_fwd_f32, enqueued on the current stream."""
+    cc = cost.contiguous()
+    out = cc.new_empty((*cc.shape[:2], H, W))
+    if out.numel():
+        with torch.cuda.device(cc.device):
+            rc = _lib.lib().cspn_disparity_regression_fwd_f32(_ptr(cc), _ptr(out), *cc.shape, D, H, W, int(align_corners),
+                                                              align_mode, _stream(cc.device))
+        _lib.check(rc, 'cspn_disparity_regression_fwd_f32')
+    return out
+
+
+def _disparity_bwd(cost, grad_out, D, H, W, align_corners, align_mode):
+    cc, go = cost.contiguous(), grad_out.contiguous()
+    gc = torch.empty_like(cc)
+    if gc.numel():
+        L = _lib.lib()
+        with torch.cuda.device(cc.device):
+            ws_bytes = L.cspn_disparity_regression_bwd_workspace_bytes(*cc.shape[2:], D, H, W)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=cc.device)
+            rc = L.cspn_disparity_regression_bwd_f32(_ptr(cc), _ptr(go), _ptr(gc), *cc.shape, D, H, W, int(align_corners),
+                                                     align_mode, _ptr(ws), ws_bytes, _stream(cc.device))
+        _lib.check(rc, 'cspn_disparity_regression_bwd_f32')
+    return gc
+
+
+class _DisparityRegressionFn(torch.autograd.Function):
+    """autograd seam of disparity_regression without the torch-op shim: native forward + native gather backward.  Only
+    cost is saved; the backward recomputes the softmax from it."""
+
+    @staticmethod
+    def forward(ctx, cost, D, H, W, align_corners, align_mode):
+        ctx.save_for_backward(cost)
+        ctx.cfg = (D, H, W, align_corners, align_mode)
+        return _disparity_fwd(cost, D, H, W, align_corners, align_mode)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        cost, = ctx.saved_tensors
+        return _disparity_bwd(cost, grad_out, *ctx.cfg), None, None, None, None, None
+
+
+def disparity_regression(cost, out_shape=None, scale=None, align_corners=True, align_mode=1):
+    """Disparity from a low-resolution cost volume (B, C, D, H, W), fp32 on CUDA, in one op:
+    U = resize_trilinear(cost, (Do, Ho, Wo), align_corners, align_mode), then y[b,c,h,w] = sum_o o * softmax_o(U[b,c,:,h,w])
+    over the upsampled disparities o = 0 .. Do-1 (the soft-argmin head of GC-Net / PSMNet).  (Do, Ho, Wo) follow
+    resize_trilinear's out_shape / scale rules; the result is (B, C, Ho, Wo).  The upsampled volume is never stored, and
+    autograd saves cost alone.  For softmin, negate cost; scale or shift the result for other disparity units.
+    DESIGN.md section 4.15."""
+    if cost.dim() != 5:
+        raise ValueError(f'cost must be (B,C,D,H,W), got {tuple(cost.shape)}')
+    if align_mode not in (0, 1) or isinstance(align_mode, bool):
+        raise ValueError(f'align_mode must be 0 or 1, got {align_mode!r}')
+    if min(cost.shape[2:]) < 1:
+        raise ValueError(f'the cost volume must not be empty, got {tuple(cost.shape)}')
+    D, H, W = resize_output_size(cost.shape[2:], out_shape, scale)
+    _check_resize_sizes(cost.shape, (D, H, W))
+    align_corners = bool(align_corners)
+    if cost.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if not cost.is_cuda:
+        raise _lib.CspnError('disparity_regression takes CUDA tensors only (there is no host-buffer entry point for it)')
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.disparity_regression(cost, D, H, W, align_corners, align_mode)
+    if torch.is_grad_enabled() and cost.requires_grad:
+        return _DisparityRegressionFn.apply(cost, D, H, W, align_corners, align_mode)
+    return _disparity_fwd(cost, D, H, W, align_corners, align_mode)

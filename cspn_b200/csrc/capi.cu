@@ -675,9 +675,9 @@ static bool overlap(const void* a, uintptr_t na, const void* b, uintptr_t nb) {
     return pa < eb && pb < ea;
 }
 
-// src is read and dst written: x and out in the forward, grad_out and grad_x in the backward
-static int check_resize(const void* src, const void* dst, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
-                        int align_corners, int align_mode, bool backward) {
+// The sizes, flags and pointers of a resampling entry: src is read and dst written
+static int check_resize_args(const void* src, const void* dst, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                             int align_corners, int align_mode) {
     if (!src || !dst) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
     if (!positive(B, C, D, H, W, Do, Ho, Wo)) {
         set_error("non-positive size B=%d C=%d D=%d H=%d W=%d Do=%d Ho=%d Wo=%d", B, C, D, H, W, Do, Ho, Wo);
@@ -691,6 +691,14 @@ static int check_resize(const void* src, const void* dst, int B, int C, int D, i
     }
     const char* why = "";
     if (!resize_trilinear_launchable(D, H, W, Do, Ho, Wo, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+// src is read and dst written: x and out in the forward, grad_out and grad_x in the backward
+static int check_resize(const void* src, const void* dst, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                        int align_corners, int align_mode, bool backward) {
+    const int rc = check_resize_args(src, dst, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode);
+    if (rc != CSPN_OK) return rc;
     const long long vin = (long long)D * H * W, vout = (long long)Do * Ho * Wo;
     if (overlap(src, span_bytes(B, C, backward ? vout : vin), dst, span_bytes(B, C, backward ? vin : vout))) {
         set_error("%s overlaps %s", backward ? "grad_x" : "out", backward ? "grad_out" : "x");
@@ -734,6 +742,68 @@ int cspn_resize_trilinear_bwd_f32(const float* grad_out, float* grad_x, int B, i
     return on_device_of(grad_out, "grad_out", [&](int* launches) {
         return resize_trilinear_backward(grad_out, grad_x, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners, align_mode,
                                          workspace, (cudaStream_t)stream, launches);
+    });
+}
+
+// ---- disparity regression from a low-resolution cost volume (resize_trilinear, softmax over d, expectation) ---------------
+// resize's argument check, then the tile rule: cost is read and dst (out, or grad_cost) written
+static int check_disparity(const float* cost, const float* dst, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                           int align_corners, int align_mode) {
+    int rc = check_resize_args(cost, dst, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode);
+    if (rc != CSPN_OK) return rc;
+    const char* why = "";
+    if (!disparity_regression_launchable(D, H, W, Do, Ho, Wo, align_corners, align_mode, &why)) {
+        set_error("unsupported shape: %s", why);
+        return CSPN_ERR_UNSUPPORTED;
+    }
+    return CSPN_OK;
+}
+
+int cspn_disparity_regression_fwd_f32(const float* cost, float* out, int B, int C, int D, int H, int W, int Do, int Ho, int Wo,
+                                      int align_corners, int align_mode, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_disparity(cost, out, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode);
+    if (rc != CSPN_OK) return rc;
+    if (overlap(cost, span_bytes(B, C, (long long)D * H * W), out, span_bytes(B, C, (long long)Ho * Wo))) {
+        set_error("out overlaps cost");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    return on_device_of(cost, "cost", [&](int* launches) {
+        return disparity_regression_forward(cost, out, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners, align_mode,
+                                            (cudaStream_t)stream, launches);
+    });
+}
+
+size_t cspn_disparity_regression_bwd_workspace_bytes(int D, int H, int W, int Do, int Ho, int Wo) {
+    return cspn_resize_trilinear_bwd_workspace_bytes(D, H, W, Do, Ho, Wo);
+}
+
+int cspn_disparity_regression_bwd_f32(const float* cost, const float* grad_out, float* grad_cost, int B, int C, int D, int H,
+                                      int W, int Do, int Ho, int Wo, int align_corners, int align_mode, void* workspace,
+                                      size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    const int rc = check_disparity(cost, grad_cost, B, C, D, H, W, Do, Ho, Wo, align_corners, align_mode);
+    if (rc != CSPN_OK) return rc;
+    if (!grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (reinterpret_cast<uintptr_t>(grad_out) & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const uintptr_t n_cost = span_bytes(B, C, (long long)D * H * W), n_g = span_bytes(B, C, (long long)Ho * Wo);
+    if (overlap(grad_cost, n_cost, cost, n_cost) || overlap(grad_cost, n_cost, grad_out, n_g)) {
+        set_error("grad_cost overlaps %s", overlap(grad_cost, n_cost, cost, n_cost) ? "cost" : "grad_out");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    const size_t need = resize_trilinear_bwd_workspace_bytes(D, H, W, Do, Ho, Wo);
+    if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 7)) {
+        set_error("the backward needs %zu bytes of 8-byte aligned workspace (got %zu)", need, workspace_bytes);
+        return CSPN_ERR_WORKSPACE;
+    }
+    const char* hit = overlap(workspace, need, grad_cost, n_cost) ? "grad_cost"
+                      : overlap(workspace, need, cost, n_cost)    ? "cost"
+                      : overlap(workspace, need, grad_out, n_g)   ? "grad_out"
+                                                                  : nullptr;
+    if (hit) { set_error("the workspace overlaps %s", hit); return CSPN_ERR_INVALID_ARGUMENT; }
+    return on_device_of(cost, "cost", [&](int* launches) {
+        return disparity_regression_backward(cost, grad_out, grad_cost, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners,
+                                             align_mode, workspace, (cudaStream_t)stream, launches);
     });
 }
 

@@ -180,4 +180,15 @@ int resize_trilinear_forward(const float* x, float* out, long long slices, int D
 int resize_trilinear_backward(const float* grad_out, float* grad_x, long long slices, int D, int H, int W, int Do, int Ho,
                               int Wo, int align_corners, int align_mode, void* ws, cudaStream_t st, int* launches);
 
+// Disparity regression from a low-resolution cost volume (disparity_regression.cu): resize_trilinear to (Do, Ho, Wo), softmax
+// over Do and the expectation; arguments checked by the caller (resize's checks, then launchable).  The backward's workspace
+// is resize's tables, resize_trilinear_bwd_workspace_bytes()
+int disparity_regression_launchable(int D, int H, int W, int Do, int Ho, int Wo, int align_corners, int align_mode,
+                                    const char** why);
+int disparity_regression_forward(const float* cost, float* out, long long slices, int D, int H, int W, int Do, int Ho, int Wo,
+                                 int align_corners, int align_mode, cudaStream_t st, int* launches);
+int disparity_regression_backward(const float* cost, const float* grad_out, float* grad_cost, long long slices, int D, int H,
+                                  int W, int Do, int Ho, int Wo, int align_corners, int align_mode, void* ws, cudaStream_t st,
+                                  int* launches);
+
 }  // namespace cspn

@@ -44,6 +44,10 @@
 //       (fluid.layers.resize_trilinear: input (B, C, d, h, w) resampled to (B, C, D, H, W))
 //   resize_trilinear_backward(Tensor grad_out, int in_D, int in_H, int in_W, bool align_corners, int align_mode) -> Tensor
 //       (grad_input (B, C, in_D, in_H, in_W) from grad_out alone: the backward needs the input's size only)
+//   disparity_regression(Tensor cost, int D, int H, int W, bool align_corners, int align_mode) -> Tensor
+//       (cost (B, C, d, h, w) resized to (D, H, W), softmax over D, expectation of the index: (B, C, H, W))
+//   disparity_regression_backward(Tensor cost, Tensor grad_out, int D, int H, int W, bool align_corners, int align_mode)
+//       -> Tensor   (grad_cost (B, C, d, h, w); the softmax is recomputed from cost)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -539,6 +543,44 @@ at::Tensor resize_trilinear_backward_cuda(const at::Tensor& grad_out, int64_t D,
     return gx;
 }
 
+// Disparity regression (resize_trilinear, softmax over D, expectation): cost (B, C, d, h, w) -> (B, C, H, W)
+at::Tensor disparity_regression_cuda(const at::Tensor& cost, int64_t D, int64_t H, int64_t W, bool align_corners,
+                                     int64_t align_mode) {
+    check_resize(cost, D, H, W, align_mode, "cost");
+    const c10::cuda::CUDAGuard guard(cost.device());
+    const at::Tensor cc = cost.contiguous();
+    at::Tensor out = at::empty({cc.size(0), cc.size(1), H, W}, cc.options());
+    if (out.numel())
+        check_rc(cspn_disparity_regression_fwd_f32(fptr(cc), mptr(out), (int)cc.size(0), (int)cc.size(1), (int)cc.size(2),
+                                                   (int)cc.size(3), (int)cc.size(4), (int)D, (int)H, (int)W, align_corners,
+                                                   (int)align_mode, current_stream()),
+                 "cspn_disparity_regression_fwd_f32");
+    return out;
+}
+
+at::Tensor disparity_regression_backward_cuda(const at::Tensor& cost, const at::Tensor& grad_out, int64_t D, int64_t H,
+                                              int64_t W, bool align_corners, int64_t align_mode) {
+    check_resize(cost, D, H, W, align_mode, "cost");
+    TORCH_CHECK_VALUE(grad_out.dim() == 4 && grad_out.size(0) == cost.size(0) && grad_out.size(1) == cost.size(1) &&
+                          grad_out.size(2) == H && grad_out.size(3) == W,
+                      "grad_out must be (B, C, H, W) = (", cost.size(0), ", ", cost.size(1), ", ", H, ", ", W, "), got ",
+                      grad_out.sizes());
+    TORCH_CHECK(grad_out.scalar_type() == at::kFloat && grad_out.device() == cost.device(),
+                "grad_out must be fp32 on cost's device");
+    const c10::cuda::CUDAGuard guard(cost.device());
+    const at::Tensor cc = cost.contiguous(), go = grad_out.contiguous();
+    at::Tensor gc = at::empty_like(cc);
+    if (gc.numel()) {
+        const int d = (int)cc.size(2), h = (int)cc.size(3), w = (int)cc.size(4);
+        const Workspace ws(cspn_disparity_regression_bwd_workspace_bytes(d, h, w, (int)D, (int)H, (int)W), cc);
+        check_rc(cspn_disparity_regression_bwd_f32(fptr(cc), fptr(go), mptr(gc), (int)cc.size(0), (int)cc.size(1), d, h, w,
+                                                   (int)D, (int)H, (int)W, align_corners, (int)align_mode, ws.ptr(), ws.bytes,
+                                                   current_stream()),
+                 "cspn_disparity_regression_bwd_f32");
+    }
+    return gc;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -573,6 +615,9 @@ TORCH_LIBRARY(cspn_b200, m) {
           "-> (Tensor, Tensor)");
     m.def("resize_trilinear(Tensor input, int D, int H, int W, bool align_corners, int align_mode) -> Tensor");
     m.def("resize_trilinear_backward(Tensor grad_out, int in_D, int in_H, int in_W, bool align_corners, int align_mode) -> Tensor");
+    m.def("disparity_regression(Tensor cost, int D, int H, int W, bool align_corners, int align_mode) -> Tensor");
+    m.def("disparity_regression_backward(Tensor cost, Tensor grad_out, int D, int H, int W, bool align_corners, int align_mode) "
+          "-> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -596,4 +641,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("unpool_conv3x3_backward", &unpool_conv3x3_backward_cuda);
     m.impl("resize_trilinear", &resize_trilinear_cuda);
     m.impl("resize_trilinear_backward", &resize_trilinear_backward_cuda);
+    m.impl("disparity_regression", &disparity_regression_cuda);
+    m.impl("disparity_regression_backward", &disparity_regression_backward_cuda);
 }

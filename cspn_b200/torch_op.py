@@ -265,6 +265,29 @@ def _register():
 
     lib.register_autograd('cspn_b200::resize_trilinear', backward_resize, setup_context=setup_resize)
 
+    @lib.register_fake('cspn_b200::disparity_regression')
+    def _(cost, D, H, W, align_corners, align_mode):
+        torch._check(cost.dim() == 5, lambda: 'cost must be (B,C,D,H,W)')
+        torch._check(D >= 1 and H >= 1 and W >= 1 and align_mode in (0, 1), lambda: 'sizes >= 1 and align_mode 0 or 1')
+        return cost.new_empty((cost.shape[0], cost.shape[1], H, W))
+
+    @lib.register_fake('cspn_b200::disparity_regression_backward')
+    def _(cost, grad_out, D, H, W, align_corners, align_mode):
+        torch._check(cost.dim() == 5 and grad_out.dim() == 4, lambda: 'cost must be (B,C,D,H,W) and grad_out (B,C,H,W)')
+        return cost.new_empty(cost.shape)
+
+    def setup_disparity(ctx, inputs, output):     # the backward recomputes the softmax: cost is the one saved tensor
+        cost, D, H, W, align_corners, align_mode = inputs
+        ctx.save_for_backward(cost)
+        ctx.cfg = (D, H, W, align_corners, align_mode)
+
+    def backward_disparity(ctx, grad_out):
+        cost, = ctx.saved_tensors
+        return (torch.ops.cspn_b200.disparity_regression_backward(cost, grad_out.contiguous(), *ctx.cfg),
+                None, None, None, None, None)
+
+    lib.register_autograd('cspn_b200::disparity_regression', backward_disparity, setup_context=setup_disparity)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

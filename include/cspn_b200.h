@@ -398,6 +398,30 @@ CSPN_API int cspn_resize_trilinear_bwd_f32(const float* grad_out, float* grad_x,
                                   int Ho, int Wo, int align_corners, int align_mode, void* workspace,
                                   size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- disparity regression from a low-resolution cost volume ---------------------------------------------------------
+ * The soft-argmin head of GC-Net / PSMNet-style stereo networks on a cost volume cost [B][C][D][H][W], in one op:
+ *   U = resize_trilinear(cost, (Do, Ho, Wo), align_corners, align_mode)     (the bits of cspn_resize_trilinear_fwd_f32)
+ *   out[b][c][h][w] = sum_{o=0}^{Do-1} o * softmax_o(U[b][c][:][h][w])      out is [B][C][Ho][Wo]
+ * The softmax subtracts the column maximum, uses expf, and sums S = sum e and N = sum o*e in ascending o; out = N / S.  A NaN
+ * or +inf in the upsampled column, or a column all -inf, gives NaN.  The upsampled volume is never stored.
+ * The backward recomputes the softmax from cost: gU_o = ((e_o * (g / S)) * (o - out)), then resize's adjoint as a gather
+ * (along d per pixel, then sum_oh (sum_ow gv * w_w) * w_h per voxel, ascending, zero-weight taps included): no atomics,
+ * every grad_cost element written once, the bits depend on the arguments only (DESIGN.md section 4.15).
+ * Arguments and errors are cspn_resize_trilinear_*'s: align flags 0 or 1, every pointer 4-byte aligned, out / grad_cost
+ * must not overlap cost (nor grad_out), and the workspace, cspn_disparity_regression_bwd_workspace_bytes() bytes (resize's
+ * tables, 8*(Do+Ho+Wo+D+H+W)), 8-byte aligned, must overlap none of the three.  The forward launches one kernel, the
+ * backward two.  No allocation, no synchronisation.  CSPN_ERR_UNSUPPORTED also for Do > 2^24 and for a shape whose 1x1 tile
+ * of cost columns does not fit in shared memory: with Do = D, D above about 2150 without upsampling in H and W, above about
+ * 520 at 4x (about 370 with align_corners = 0, align_mode = 0). */
+CSPN_API int cspn_disparity_regression_fwd_f32(const float* cost, float* out, int B, int C, int D, int H, int W, int Do,
+                                  int Ho, int Wo, int align_corners, int align_mode, cspn_stream_t stream);
+
+CSPN_API size_t cspn_disparity_regression_bwd_workspace_bytes(int D, int H, int W, int Do, int Ho, int Wo);
+
+CSPN_API int cspn_disparity_regression_bwd_f32(const float* cost, const float* grad_out, float* grad_cost, int B, int C,
+                                  int D, int H, int W, int Do, int Ho, int Wo, int align_corners, int align_mode,
+                                  void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
