@@ -494,28 +494,11 @@ int cspn3d_fwd_gather_f32(const float* guidance, const float* feat, float* out, 
     return fwd3d(guidance, feat, out, &gather, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes, stream);
 }
 
-size_t cspn3d_bwd_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
-    if (!positive(B, C, D, H, W, iters)) return 0;
-    return bwd3d_workspace_bytes(C, D, H, W, iters);
-}
-
-int cspn3d_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
-                   int B, int C, int D, int H, int W, int iters, int norm_type, void* workspace, size_t workspace_bytes,
-                   cspn_stream_t stream) {
-    begin_call();
-    const int rc = check_prop(3, guidance, feat, grad_out, B, C, D, H, W, 3, 0, iters, norm_type);
-    if (rc != CSPN_OK) return rc;
-    return on_device_of(feat, "feat", [&](int* launches) {
-        return bwd3d(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace, workspace_bytes,
-                     (cudaStream_t)stream, launches);
-    });
-}
-
-// ---- K x K x K kernels (K = 3 is the 3D operator above, K = 5 runs in cspn3d_wide.cu) and caller-supplied gates (K in
-// {3, 5}, both in cspn3d_wide.cu).  The gates entries have no norm_type and pass 0 -------------------------------------
+// ---- K x K x K kernels (the K = 3 forward is the 3D operator above, everything else runs in cspn3d_wide.cu, the 3x3x3
+// backward included) and caller-supplied gates (K in {3, 5}).  The gates entries have no norm_type and pass 0 ----------
 static size_t wide3d_workspace_bytes(Family family, bool bwd, int B, int C, int D, int H, int W, int K, int iters) {
     if (!positive(B, C, D, H, W, iters) || !kernel_size_ok(3, K)) return 0;
-    if (K == 3 && family != Family::Gates) return bwd ? cspn3d_bwd_workspace_bytes(B, C, D, H, W, iters) : cspn3d_workspace_bytes(B, C, D, H, W, iters);
+    if (K == 3 && family != Family::Gates && !bwd) return cspn3d_workspace_bytes(B, C, D, H, W, iters);
     return bwd ? widek3d_bwd_workspace_bytes(C, D, H, W, K, iters, family) : widek3d_workspace_bytes(B, C, D, H, W, K, iters, family);
 }
 
@@ -540,9 +523,6 @@ static int wide3d_bwd(Family family, const float* guidance, const float* feat, c
     begin_call();
     const int rc = check_prop(3, guidance, feat, grad_out, B, C, D, H, W, K, 0, iters, norm_type);
     if (rc != CSPN_OK) return rc;
-    if (K == 3 && family != Family::Gates)
-        return cspn3d_bwd_f32(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, iters, norm_type, workspace,
-                              workspace_bytes, stream);
     return on_device_of(feat, "feat", [&](int* launches) {
         return widek3d_backward(guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, K, iters, family, norm_type,
                                 workspace, workspace_bytes, (cudaStream_t)stream, launches);
@@ -569,6 +549,17 @@ int cspn3d_k_fwd_gather_f32(const float* guidance, const float* feat, float* out
 
 size_t cspn3d_k_bwd_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters) {
     return wide3d_workspace_bytes(Family::Normalised, true, B, C, D, H, W, K, iters);
+}
+
+size_t cspn3d_bwd_workspace_bytes(int B, int C, int D, int H, int W, int iters) {
+    return wide3d_workspace_bytes(Family::Normalised, true, B, C, D, H, W, 3, iters);
+}
+
+int cspn3d_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,
+                   int B, int C, int D, int H, int W, int iters, int norm_type, void* workspace, size_t workspace_bytes,
+                   cspn_stream_t stream) {
+    return wide3d_bwd(Family::Normalised, guidance, feat, grad_out, grad_guidance, grad_feat, B, C, D, H, W, 3, iters, norm_type,
+                      workspace, workspace_bytes, stream);
 }
 
 int cspn3d_k_bwd_f32(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat,

@@ -127,6 +127,7 @@ __device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float v) {
 // The operator families of the wide kernels (cspn2d_wide.cu, cspn3d_wide.cu)
 enum class Family {
     Normalised,   // weights gathered from the neighbours' guidance and normalised; 2D K in {5, 7}, 3D K = 5 with `mode`
+                  // (3D backward: K in {3, 5})
     Paddle,       // 2D 'paddle' own-location norm, K in {3, 5, 7} (in 3D it is mode 2 of Normalised)
     Gates,        // caller-supplied gates used as given; 2D K in {3, 5, 7}, 3D K in {3, 5}
 };
@@ -148,12 +149,8 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
                       int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,
                       const Fan* fan = nullptr);
 
-size_t bwd3d_workspace_bytes(int C, int D, int H, int W, int iters);
-int bwd3d(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat, int B, int C,
-          int D, int H, int W, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches);
-
 // 3D, Normalised (guidance [B][K^3-1][D][H][W], mode 0 signed / 1 abs / 2 'paddle') or Gates (gates of that shape, mode
-// unused).  fan non-null: the fused gather
+// unused).  fan non-null: the fused gather.  The normalised forward is K = 5 only (K = 3: generic3d_forward)
 size_t widek3d_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters, Family family);
 int widek3d_forward(const float* guidance, const float* feat, float* out, int B, int C, int D, int H, int W, int K, int iters,
                     Family family, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches,

@@ -1,4 +1,5 @@
-// 3D CSPN (26 neighbours): prep (normalisation) + one 27-point stencil launch per iteration.
+// 3D CSPN (26 neighbours), forward: prep (normalisation) + one 27-point stencil launch per iteration.  The 3x3x3
+// backward runs on cspn3d_wide.cu's K x K x K kernels at R = 1.
 //
 // Reference: call sites only -- /root/reference/cspn_paddle/demo.py:20-54; the Paddle op's
 // source is not in the tree, so the arithmetic is the definition of SURVEY.md Appendix A.3
@@ -434,158 +435,6 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
             cur = dst;
             dst = (dst == o) ? tmp : o;
         }
-    }
-    CSPN_CUDA_TRY(cudaGetLastError());
-    return CSPN_OK;
-}
-
-// ---- 3D backward (adjoint), one volume at a time; same scheme as cspn2d_bwd.cu with 26 taps ----------------------
-// mode 0/1 ('26sum', '26sum_abs'): w_k = a_k / S with gathered a_k, kappa = 1 - sum w_k, c' = kappa d0:
-//     Gkappa = sum_c Gc_c d0_c,  H_k = Gw_k - Gkappa,  T = sum_k H_k w_k,  dL/da_j = (H_j - sign(a_j) T) / S,
-//     grad_g_j(p + off_j) = dL/da_j(p) [* sign(g_j) in abs mode],  grad_feat_c = kappa Gc_c + lambda_{0,c}.
-// mode 2 ('paddle'): w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the voxel's own location, no centre term:
-//     H_k = Gw_k,  grad_g_j(p) = (H_j - T) / S * sign(g_j(p)),  grad_feat_c = lambda_{0,c}.
-namespace {
-
-__global__ void __launch_bounds__(256)
-bwd3d_step_kernel(const float* __restrict__ wk, const float* __restrict__ d_t, const float* __restrict__ lam_in,
-                  float* __restrict__ lam_out, float* __restrict__ Gw, float* __restrict__ Gc, int C, int D, int H, int W,
-                  int first) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    const int z = blockIdx.z;
-    if (x >= W || y >= H) return;
-    const size_t HW = (size_t)H * W, V = (size_t)D * HW;
-    const size_t p = (size_t)z * HW + (size_t)y * W + x;
-    for (int c = 0; c < C; ++c) {
-        const float* li = lam_in + (size_t)c * V;
-        const float* dt = d_t + (size_t)c * V;
-        const float lp = __ldg(li + p);
-        float acc = 0.f;
-#pragma unroll
-        for (int k = 0; k < 26; ++k) {
-            const int zs = z - off3_dz(k), ys = y - off3_dy(k), xs = x - off3_dx(k);   // the voxel that reads me with tap k
-            if (zs >= 0 && zs < D && ys >= 0 && ys < H && xs >= 0 && xs < W) {
-                const size_t ps = (size_t)zs * HW + (size_t)ys * W + xs;
-                acc = fmaf(__ldg(wk + k * V + ps), __ldg(li + ps), acc);
-            }
-            const int zn = z + off3_dz(k), yn = y + off3_dy(k), xn = x + off3_dx(k);
-            float g = (first && c == 0) ? 0.f : Gw[k * V + p];
-            if (zn >= 0 && zn < D && yn >= 0 && yn < H && xn >= 0 && xn < W)
-                g = fmaf(lp, __ldg(dt + (size_t)zn * HW + (size_t)yn * W + xn), g);
-            Gw[k * V + p] = g;
-        }
-        lam_out[(size_t)c * V + p] = acc;
-        Gc[(size_t)c * V + p] = (first ? 0.f : Gc[(size_t)c * V + p]) + lp;
-    }
-}
-
-__global__ void __launch_bounds__(256)
-bwd3d_finalize_kernel(const float* __restrict__ g, const float* __restrict__ feat, const float* __restrict__ wk,
-                      const float* __restrict__ Gw, const float* __restrict__ Gc, const float* __restrict__ lam0,
-                      float* __restrict__ grad_g, float* __restrict__ grad_feat, int C, int D, int H, int W, int mode) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    const int z = blockIdx.z;
-    if (x >= W || y >= H) return;
-    const size_t HW = (size_t)H * W, V = (size_t)D * HW;
-    const size_t p = (size_t)z * HW + (size_t)y * W + x;
-    const float kappa = __ldg(wk + 26 * V + p);
-    float gkappa = 0.f;
-    for (int c = 0; c < C; ++c) {
-        const float gc = __ldg(Gc + (size_t)c * V + p);
-        gkappa = fmaf(gc, __ldg(feat + (size_t)c * V + p), gkappa);
-        if (grad_feat) grad_feat[(size_t)c * V + p] = fmaf(kappa, gc, __ldg(lam0 + (size_t)c * V + p));
-    }
-    if (!grad_g) return;
-    if (mode == 2) gkappa = 0.f;   // no centre term
-    float a[26], sg[26], S = 0.f;
-#pragma unroll
-    for (int k = 0; k < 26; ++k) {
-        float v = 0.f;
-        sg[k] = 1.f;
-        if (mode == 2) {
-            v = __ldg(g + k * V + p);
-            sg[k] = signf(v);
-            v = fabsf(v);
-        } else {
-            const int zz = z + off3_dz(k), yy = y + off3_dy(k), xx = x + off3_dx(k);
-            if (zz >= 0 && zz < D && yy >= 0 && yy < H && xx >= 0 && xx < W) {
-                v = __ldg(g + k * V + (size_t)zz * HW + (size_t)yy * W + xx);
-                if (mode == 1) { sg[k] = signf(v); v = fabsf(v); }
-            }
-        }
-        a[k] = v;
-        S += fabsf(v);
-    }
-    float T = 0.f;
-#pragma unroll
-    for (int k = 0; k < 26; ++k) T = fmaf(__ldg(Gw + k * V + p) - gkappa, __fdiv_rn(a[k], S), T);
-#pragma unroll
-    for (int k = 0; k < 26; ++k) {
-        const float ga = __fdiv_rn((__ldg(Gw + k * V + p) - gkappa) - signf(a[k]) * T, S) * sg[k];
-        if (mode == 2) {
-            grad_g[k * V + p] = ga;
-        } else {
-            const int zz = z + off3_dz(k), yy = y + off3_dy(k), xx = x + off3_dx(k);
-            if (zz >= 0 && zz < D && yy >= 0 && yy < H && xx >= 0 && xx < W)
-                grad_g[k * V + (size_t)zz * HW + (size_t)yy * W + xx] = ga;
-        }
-    }
-}
-
-}  // namespace
-
-size_t bwd3d_workspace_bytes(int C, int D, int H, int W, int iters) {
-    if (iters <= 0) return 0;
-    const size_t V = (size_t)D * H * W, n = (size_t)C * V;
-    // per volume: wk (27 planes) + d_1..d_{N-1} + lambda ping-pong + Gw (26 planes) + Gc
-    return sizeof(float) * (27 * V + (size_t)(iters - 1) * n + 2 * n + 26 * V + n);
-}
-
-int bwd3d(const float* guidance, const float* feat, const float* grad_out, float* grad_guidance, float* grad_feat, int B, int C,
-          int D, int H, int W, int iters, int mode, void* ws, size_t ws_bytes, cudaStream_t stream, int* launches) {
-    const size_t V = (size_t)D * H * W, n = (size_t)C * V;
-    if (grad_guidance) CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)B * 26 * V * sizeof(float), stream));
-    if (iters == 0) {
-        if (grad_feat) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_feat, grad_out, (size_t)B * n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = bwd3d_workspace_bytes(C, D, H, W, iters);
-    if (!ws || ws_bytes < need) {
-        set_error("3D backward needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if ((size_t)D * C > 65535) { set_error("3D backward: D*C exceeds gridDim.z"); return CSPN_ERR_UNSUPPORTED; }
-    float* wk = static_cast<float*>(ws);
-    float* Dt = wk + 27 * V;                                    // d_1 .. d_{N-1}
-    float* lam[2] = {Dt + (size_t)(iters - 1) * n, Dt + (size_t)(iters - 1) * n + n};
-    float* Gw = lam[1] + n;
-    float* Gc = Gw + 26 * V;
-    const dim3 block(32, 8);
-    const dim3 g2((W + 31) / 32, (H + 7) / 8);
-    for (int b = 0; b < B; ++b) {
-        const float* gb = guidance + (size_t)b * 26 * V;
-        const float* d0 = feat + (size_t)b * n;
-        prep3d_kernel<<<dim3(g2.x, g2.y, D), block, 0, stream>>>(gb, wk, D, H, W, mode);
-        ++*launches;
-        for (int t = 0; t + 1 < iters; ++t) {
-            step3d_kernel<<<dim3(g2.x, g2.y, D * C), block, 0, stream>>>(wk, d0, t == 0 ? d0 : Dt + (size_t)(t - 1) * n,
-                                                                         Dt + (size_t)t * n, C, D, H, W, Fan{});
-            ++*launches;
-        }
-        const float* lam_in = grad_out + (size_t)b * n;
-        for (int t = iters - 1; t >= 0; --t) {
-            float* lam_out = lam[t & 1];
-            bwd3d_step_kernel<<<dim3(g2.x, g2.y, D), block, 0, stream>>>(wk, t == 0 ? d0 : Dt + (size_t)(t - 1) * n, lam_in, lam_out,
-                                                                         Gw, Gc, C, D, H, W, t == iters - 1);
-            ++*launches;
-            lam_in = lam_out;
-        }
-        bwd3d_finalize_kernel<<<dim3(g2.x, g2.y, D), block, 0, stream>>>(gb, d0, wk, Gw, Gc, lam_in,
-                                                                         grad_guidance ? grad_guidance + (size_t)b * 26 * V : nullptr,
-                                                                         grad_feat ? grad_feat + (size_t)b * n : nullptr, C, D, H, W, mode);
-        ++*launches;
     }
     CSPN_CUDA_TRY(cudaGetLastError());
     return CSPN_OK;

@@ -1,34 +1,34 @@
-// 3D CSPN with a K x K x K affinity kernel, K = 2R+1 = 5 (K^3-1 = 124 neighbours), forward and backward.  The 3x3x3
-// operator keeps its own kernels (cspn3d.cu); K = 3 is delegated to them by the C ABI.
+// 3D CSPN with a K x K x K affinity kernel, K = 2R+1 = 5 (K^3-1 = 124 neighbours), forward and backward, and the 3x3x3
+// backward (R = 1).  The 3x3x3 forward keeps its own kernels (cspn3d.cu); the C ABI delegates it to them.
 //
-// Arithmetic: cspn3d.cu with K^3-1 taps.  Tap k enumerates (f, t, l) over [0,K)^3 in raster order without the centre
-// (R, R, R) and reads the source at (dz, dy, dx) = (R-f, R-t, R-l) (oracle/cspn_numpy_3d_k.py::offsets_3d):
+// Arithmetic: cspn3d.cu with K^3-1 taps (at K = 3 its taps in its order: Taps3<1> is off3_*).  Tap k enumerates (f, t, l)
+// over [0,K)^3 in raster order without the centre (R, R, R) and reads the source at (dz, dy, dx) = (R-f, R-t, R-l)
+// (oracle/cspn_numpy_3d_k.py::offsets_3d):
 //   gathered (mode 0 signed, 1 abs): a_k(p) = ghat_k(p + off_k) (0 outside),  w_k = a_k / sum_j |a_j|,  kappa = 1 - sum_k w_k,
 //                                    d_{t+1} = kappa d0 + sum_k w_k d_t(p + off_k);
 //   'paddle' (mode 2):               w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the voxel's own location, no centre term.
 //
-// Why not cspn3d.cu's design: its step keeps 9 rows x 6 floats of the current volume and 26 weights in registers.  124
-// weights per voxel and 25 rows x 8 floats do not fit, so
+// Why not cspn3d.cu's design at K = 5: its step keeps 9 rows x 6 floats of the current volume and 26 weights in registers.
+// 124 weights per voxel and 25 rows x 8 floats do not fit, so
 //   'paddle'  each step reads the 124 raw guidance planes at the voxel's own location (streamed in chunks of one z-slab of
 //             the window, 25 loads in flight per thread), sums |g| and divides once per voxel.  No prep, no weight planes;
 //   gathered  one prep launch per volume group writes w_k and kappa (K^3 = 125 planes per volume); each step streams them.
 // Both steps stage the CTA's tile of d_t plus an R-voxel halo in z, y and x in shared memory (zeros outside the volume).
 // W % 4 == 0 with 16-byte aligned pointers: 4 consecutive voxels per thread, every plane read as LDG.128; otherwise one
-// voxel per thread.  Volume groups are those of cspn3d.cu (group3d with K^3 planes per volume).
+// voxel per thread.  Volume groups: group3d with K^3 planes per volume.
 // Backward, in the staged form of cspn2d_wide.cu, one volume at a time: prep (for 'paddle' too), N-1 forward steps that keep
 // d_1..d_{N-1}, N adjoint steps lambda_t(q) = sum_k w_k(q - off_k) lambda_{t+1}(q - off_k) that keep every lambda_t
 // (lambda_{t+1} tile + halo in shared memory), K gather launches -- one per z-slab of the window, 25 register accumulators
 // Gw_k(p) = sum_c sum_t lambda_{t+1}(p) d_t(p + off_k) each, written over the then dead weight planes -- and one finalize
-// with the chain rule of cspn3d.cu's bwd3d_finalize_kernel over 124 taps.
+// with the chain rule (fin3k_kernel).
 //
 // Caller-supplied gates (fluid.layers.affinity_propagate itself, DESIGN.md section 4.11), K in {3, 5}:
 //   d_{t+1}(p) = sum_k g_k(p) d_t(p + off_k)   with the gates used as given (no |.|, no division, no centre term).
 // The step kernels' RAW mode reads the caller's gates [vol][NT][V] as the weight planes: no prep, no cold-sum branch.  The
 // backward runs the staged form above on the gates themselves: the adjoint reads the volume's gates, the last adjoint writes
 // lambda_0 straight into grad_feat, and the K gather launches write Gw_k straight into grad_gates (no prep, no finalize).
-// K = 3 runs here on R = 1 instantiations; cspn3d.cu keeps the 3x3x3 operator.
 //
-// Fused gather (cspn3d_{k,gates}_fwd_gather_f32, DESIGN.md section 4.6): the FAN flag of the two step kernels, as in
+// Fused gather (cspn3d_{,k_,gates_}fwd_gather_f32, DESIGN.md section 4.6): the FAN flag of the two step kernels, as in
 // cspn3d.cu: only the last step of a launch group stores to the other GPUs' gather buffers.
 #include <cstdlib>
 
@@ -68,7 +68,8 @@ __device__ __forceinline__ float4 ld_stream4(const float* p) {
 __device__ __forceinline__ bool cold_sum(float S) { return !(S >= 1.17549435e-38f && S <= 3.40282347e38f); }
 
 // ---- prep: w_k and kappa of every voxel.  grid z = volume of the group * D + z ------------------------------------
-// The guidance is read twice (sum, then quotients) instead of holding 124 values per thread.
+// At R = 2 the guidance is read twice (sum, then quotients) instead of holding 124 values per thread; the 26 of R = 1 stay
+// in registers and are read once.
 template <int R>
 __device__ __forceinline__ float prep_tap(const float* __restrict__ g, int k, int z, int y, int x, int D, int H, int W,
                                           size_t V, size_t p, int mode) {
@@ -91,13 +92,22 @@ prep3k_kernel(const float* __restrict__ g, float* __restrict__ wk, int D, int H,
     const size_t V = (size_t)D * H * W, p = ((size_t)z * H + y) * W + x;
     g += (size_t)vol * T::NT * V;
     wk += (size_t)vol * T::NP * V;
+    constexpr int U = R == 1 ? T::NT : 4;   // unroll: R = 1 fully, so that a[] is registers
+    float a[R == 1 ? T::NT : 1];
     float S = 0.f;
-#pragma unroll 4
-    for (int k = 0; k < T::NT; ++k) S += fabsf(prep_tap<R>(g, k, z, y, x, D, H, W, V, p, mode));
-    float s = 0.f;
-#pragma unroll 4
+#pragma unroll U
     for (int k = 0; k < T::NT; ++k) {
-        const float w = __fdiv_rn(prep_tap<R>(g, k, z, y, x, D, H, W, V, p, mode), S);   // IEEE: 0/0 NaN, x/inf 0
+        const float v = prep_tap<R>(g, k, z, y, x, D, H, W, V, p, mode);
+        if constexpr (R == 1) a[k] = v;
+        S += fabsf(v);
+    }
+    float s = 0.f;
+#pragma unroll U
+    for (int k = 0; k < T::NT; ++k) {
+        float v;
+        if constexpr (R == 1) v = a[k];
+        else v = prep_tap<R>(g, k, z, y, x, D, H, W, V, p, mode);
+        const float w = __fdiv_rn(v, S);   // IEEE: 0/0 NaN, x/inf 0
         s += w;
         wk[k * V + p] = w;
     }
@@ -176,6 +186,8 @@ step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, con
         for (int j = 0; j < 4; ++j) {
             if (cold_sum(S[j])) {   // cold: form the quotients one by one, as the weight planes hold them
                 float a = 0.f;
+                // by 4, as ptxas unrolls it at R = 2: unrolled 26 times at R = 1, the division calls cost a spill
+#pragma unroll 4
                 for (int k = 0; k < T::NT; ++k) {
                     const float* tr = reinterpret_cast<const float*>(tile[R + T::dz(k)][ty + R + T::dy(k)] + tx);
                     a = fmaf(__fdiv_rn(fabsf(__ldg(wp + k * V + j)), S[j]), tr[4 + j + T::dx(k)], a);
@@ -333,9 +345,10 @@ gather3k_kernel(const float* __restrict__ feat, const float* __restrict__ steps,
         }
 }
 
-// The chain rule of cspn3d.cu's bwd3d_finalize_kernel with NT taps.  wk holds Gw_0..Gw_{NT-1} and kappa; Gc_c = sum_t
-// lambda_{t+1,c} is summed here.  Gathered: grad_g_j lands at p + off_j (each g_j(q) feeds one voxel: no atomics),
-// grad_feat = kappa Gc + lambda_0.  'paddle': grad_g_j lands at p, grad_feat = lambda_0.  One volume: grid z = z.
+// The chain rule.  Gathered (mode 0/1): w_k = a_k / S with S = sum_j |a_j|, kappa = 1 - sum_k w_k, so with
+// Gkappa = sum_c Gc_c d0_c, H_k = Gw_k - Gkappa and T = sum_k H_k w_k:  dL/da_j = (H_j - sign(a_j) T) / S.  'paddle'
+// (mode 2): no centre term, H_k = Gw_k.  wk holds Gw_0..Gw_{NT-1} and kappa; Gc_c = sum_t lambda_{t+1,c} is summed here.
+// Gathered: grad_g_j lands at p + off_j (each g_j(q) feeds one voxel: no atomics), grad_feat = kappa Gc + lambda_0.  'paddle': grad_g_j lands at p, grad_feat = lambda_0.  One volume: grid z = z.
 template <int R>
 __global__ void __launch_bounds__(256)
 fin3k_kernel(const float* __restrict__ g, const float* __restrict__ feat, const float* __restrict__ wk,
@@ -565,7 +578,7 @@ int backward_gates_3k(const float* gates, const float* feat, const float* grad_o
     return CSPN_OK;
 }
 
-// K = 3 -> R = 1, K = 5 -> R = 2: f(R) as an integral constant (the gates kernels; the normalised ones exist for R = 2 only)
+// K = 3 -> R = 1, K = 5 -> R = 2: f(R) as an integral constant (the normalised forward exists for R = 2 only)
 template <class F>
 int with_radius(int K, F&& f) {
     return K == 3 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
@@ -638,9 +651,9 @@ int widek3d_backward(const float* guidance, const float* feat, const float* grad
     }
     const int rc = check_launch(C, D, H, K, family, "backward", widek3d_bwd_workspace_bytes(C, D, H, W, K, iters, family), ws, ws_bytes);
     if (rc != CSPN_OK) return rc;
-    if (!gates) return backward_3k<2>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, mode, ws, stream, launches);
-    if (!grad_g && !grad_feat) return CSPN_OK;
+    if (gates && !grad_g && !grad_feat) return CSPN_OK;
     return with_radius(K, [&](auto R) {
+        if (!gates) return backward_3k<R()>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, mode, ws, stream, launches);
         return backward_gates_3k<R()>(guidance, feat, grad_out, grad_g, grad_feat, B, C, D, H, W, iters, ws, stream, launches);
     });
 }

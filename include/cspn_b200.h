@@ -251,7 +251,8 @@ CSPN_API int cspn3d_fwd_f32_host(const float* guidance, const float* feat, float
                         int B, int C, int D, int H, int W, int iters, int norm_type, int device);
 
 /* ---- 3D backward (the Paddle op trains too: cspn_paddle/demo.py:72-75 minimises a loss through it).
- * grad_guidance [B][26][D][H][W], grad_feat [B][C][D][H][W]; either may be NULL. */
+ * grad_guidance [B][26][D][H][W], grad_feat [B][C][D][H][W]; either may be NULL.  Workspace (27 + (2*iters-1)*C)*D*H*W
+ * floats, 0 for iters == 0 (one volume at a time; independent of B and of the device). */
 CSPN_API size_t cspn3d_bwd_workspace_bytes(int B, int C, int D, int H, int W, int iters);
 
 CSPN_API int cspn3d_bwd_f32(const float* guidance, const float* feat, const float* grad_out,
@@ -264,10 +265,10 @@ CSPN_API int cspn3d_bwd_f32(const float* guidance, const float* feat, const floa
  * (dz, dy, dx) = ((K-1)/2 - f, (K-1)/2 - t, (K-1)/2 - l) (DESIGN.md section 4.9).
  * guidance [B][K^3-1][D][H][W] (one gate shared by the C channels of feat), feat / out / grad_* [B][C][D][H][W];
  * norm_type is a cspn_norm3d (0 gathered signed, 1 gathered abs, 2 own-location 'paddle').
- * K = 3 IS the 3D operator: the calls delegate to cspn3d_fwd_f32 / cspn3d_bwd_f32 and the workspace queries return theirs.
- * K = 5: forward workspace G*(125 + (iters > 1 ? C : 0))*D*H*W floats, with G the volumes per launch group (all B unless
- * that exceeds 4 GiB or gridDim.z); backward (125 + (2*iters-1)*C)*D*H*W floats; 0 for iters == 0; neither depends on the
- * device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5}, an unknown norm, iters < 0, a non-positive shape or a null
+ * K = 3 is the 3D operator above: cspn3d_fwd_f32 / cspn3d_bwd_f32 are these calls at K = 3, with the same results and
+ * workspace queries.  Forward workspace G*(K^3 + (iters > 1 ? C : 0))*D*H*W floats, with G the volumes per launch group
+ * (all B unless that exceeds 4 GiB or gridDim.z); backward (K^3 + (2*iters-1)*C)*D*H*W floats; 0 for iters == 0; neither
+ * depends on the device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5}, an unknown norm, iters < 0, a non-positive shape or a null
  * guidance / feat / out (grad_out in the backward; grad_guidance and grad_feat may be NULL).  CSPN_ERR_UNSUPPORTED for a
  * shape the launch grid cannot take (D*C > 65535). */
 CSPN_API size_t cspn3d_k_workspace_bytes(int B, int C, int D, int H, int W, int K, int iters);

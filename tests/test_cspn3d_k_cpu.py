@@ -134,6 +134,9 @@ def test_workspace_formulas():
     for n in (0, 1, 12):      # K = 3 is the 3D operator: its queries are theirs
         assert L.cspn3d_k_workspace_bytes(B, C, D, H, W, 3, n) == L.cspn3d_workspace_bytes(B, C, D, H, W, n)
         assert L.cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, 3, n) == L.cspn3d_bwd_workspace_bytes(B, C, D, H, W, n)
+    for n in (1, 2, 12, 24):  # the 3x3x3 backward: (27 + (2N-1)*C)*V floats
+        assert L.cspn3d_bwd_workspace_bytes(B, C, D, H, W, n) == 4 * (27 * V + (2 * n - 1) * C * V)
+    assert L.cspn3d_bwd_workspace_bytes(B, C, D, H, W, 0) == 0
     for K in (4, 7):
         assert L.cspn3d_k_workspace_bytes(B, C, D, H, W, K, 3) == 0 and L.cspn3d_k_bwd_workspace_bytes(B, C, D, H, W, K, 3) == 0
     # the demo.py volume (3 x 1 x 48 x 64 x 128, N = 24) runs as one group: 3 * 126 planes

@@ -7,6 +7,9 @@ is not timed on a shared card):
   - the torch port's eager op sequence (oracle/cspn_torch_port_3d_k.py::cspn3d_torch_k) at the demo shape as the baseline;
   - the bytes a step moves, computed from shapes, and the rate that gives.
 
+At K = 3 the demo volume's forward (W % 4 == 0) runs cspn3d.cu's raw-guidance step and its backward the K x K x K kernels at
+R = 1; at K = 5 both run the K x K x K kernels.
+
     python tools/time_3d_k.py [--reps 10] [--baseline-reps 3] [--json out.jsonl]
 
 The card's name and power limit are read in the same run and printed with the numbers.
@@ -56,8 +59,8 @@ def median_ms(fn, reps, warmup=2):
 
 def step_bytes(B, C, V, K, norm):
     """HBM bytes of one forward step: 'paddle' reads K^3-1 guidance planes, d_t and writes d_{t+1}; the gathered norms read
-    K^3 weight planes, d_0, d_t and write d_{t+1}.  K = 3 runs cspn3d.cu's direct kernels (26 guidance planes for every
-    norm, plus d_0 for the gathered ones)."""
+    K^3 weight planes, d_0, d_t and write d_{t+1}.  K = 3 at W % 4 == 0 runs cspn3d.cu's raw-guidance kernels (26 guidance
+    planes for every norm, plus d_0 for the gathered ones)."""
     nt = K ** 3 - 1
     if K == 3:
         return 4 * B * V * (nt + (2 if norm == 'paddle' else 3) * C)
