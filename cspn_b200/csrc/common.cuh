@@ -45,6 +45,13 @@ __host__ __device__ constexpr int off3_dx(int k) { return 1 - off3_idx(k) % 3; }
 
 __device__ __forceinline__ float signf(float v) { return (v > 0.f ? 1.f : 0.f) - (v < 0.f ? 1.f : 0.f); }
 
+// a sum of |gates| whose quotient form must be used: 0 (0/0 = NaN), subnormal (divided exactly), inf or NaN (weights 0 / NaN)
+__device__ __forceinline__ bool cold_sum(float S) { return !(S >= 1.17549435e-38f && S <= 3.40282347e38f); }
+// The own-location ('paddle') steps divide acc = sum_k |g_k| d(p + off_k) by S once.  That is the quotient form
+// sum_k (|g_k| / S) d(p + off_k) up to rounding only where S is normal and acc finite: an acc that overflowed (a large S
+// times |d| > 1) or met an inf / NaN of d must be formed from the quotients too, so that each term is w_k d as the weights have it
+__device__ __forceinline__ bool cold_paddle(float S, float acc) { return cold_sum(S) || !(fabsf(acc) <= 3.40282347e38f); }
+
 // ---- problem descriptors --------------------------------------------------------------------
 struct Problem2D {
     const float* guidance;  // [B][gch][H][W]

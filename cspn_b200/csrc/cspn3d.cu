@@ -60,7 +60,8 @@ prep3d_kernel(const float* __restrict__ g, float* __restrict__ wk, int D, int H,
 }
 
 // FAN (every step kernel below): the result also goes to fan's destinations (the last step of a fused gather); fan is
-// not read otherwise.
+// not read otherwise.  The two weight-plane steps add kappa d0 only where d0 is not null: 'paddle' has no centre term,
+// and its kappa of 0 would still turn an inf or NaN of d0 into 0 * inf = NaN.
 template <bool FAN = false>
 __global__ void __launch_bounds__(256)
 step3d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
@@ -73,7 +74,7 @@ step3d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const 
     const size_t p = (size_t)z * HW + (size_t)y * W + x;
     wk += (size_t)(c / C) * 27 * V;
     const float* cc = cur + (size_t)c * V;
-    float acc = __ldg(wk + 26 * V + p) * __ldg(d0 + (size_t)c * V + p);
+    float acc = d0 ? __ldg(wk + 26 * V + p) * __ldg(d0 + (size_t)c * V + p) : 0.f;
 #pragma unroll
     for (int k = 0; k < 26; ++k) {
         const int zz = z + off3_dz(k), yy = y + off3_dy(k), xx = x + off3_dx(k);
@@ -127,9 +128,12 @@ step3d_vec4_kernel(const float* __restrict__ wk, const float* __restrict__ d0, c
                 for (int i = 0; i < 6; ++i) r[i] = 0.f;
             }
         }
-    const float4 kap = __ldg(reinterpret_cast<const float4*>(wk + 26 * V + p));
-    const float4 dz0 = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)c * V + p));
-    float acc[4] = {kap.x * dz0.x, kap.y * dz0.y, kap.z * dz0.z, kap.w * dz0.w};
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    if (d0) {
+        const float4 kap = __ldg(reinterpret_cast<const float4*>(wk + 26 * V + p));
+        const float4 dz0 = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)c * V + p));
+        acc[0] = kap.x * dz0.x; acc[1] = kap.y * dz0.y; acc[2] = kap.z * dz0.z; acc[3] = kap.w * dz0.w;
+    }
 #pragma unroll
     for (int k = 0; k < 26; ++k) {
         const float4 w = __ldg(reinterpret_cast<const float4*>(wk + k * V + p));
@@ -149,7 +153,9 @@ step3d_vec4_kernel(const float* __restrict__ wk, const float* __restrict__ d0, c
 // 'paddle' normalisation straight from the RAW guidance (cspn_paddle/demo.py:24,47-52): the gate of tap k is
 // |g_k(p)| / sum_j |g_j(p)| at the voxel's own location, so one step is  out(p) = (sum_k |g_k(p)| cur(p + off_k)) / (sum_k |g_k(p)|):
 // ONE division per voxel instead of 26, no normalised-weight planes at all (no prep launch, no workspace for weights, 27
-// instead of 29 planes read per step).  0 / 0 = NaN as with explicit gates.  The 26 guidance float4 of a thread are
+// instead of 29 planes read per step).  Where S is 0, subnormal, inf or NaN, or the sum overflowed or met an inf / NaN of
+// cur (cold_paddle), a lane forms the 26 quotients |g_k| / S one by one instead: 0 / 0 = NaN, exact weights at a subnormal
+// S, weights of 0 where S overflowed, as the weight-plane path has them.  The 26 guidance float4 of a thread are
 // requested back to back before any arithmetic (CSPN3D_HOIST, default on): the kernel lives on loads in flight.
 #ifndef CSPN3D_HOIST
 #define CSPN3D_HOIST 1
@@ -162,6 +168,29 @@ __device__ __forceinline__ float4 ld_stream(const float* p) {
     v = __ldg(reinterpret_cast<const float4*>(p));
 #endif
     return v;
+}
+
+// The quotient form of one voxel (z, y, x), the cold path of the two raw-guidance steps below: (sum_k w_k cur(p + off_k),
+// sum_k w_k) with w_k = a_k / S formed one by one, as prep3d_kernel forms the weight planes (MODE 0 '26sum', 1 '26sum_abs':
+// a_k = g_k(p + off_k), zero outside; 2 'paddle': a_k = |g_k(p)|).  The gates and the neighbours are read again (L1 / L2
+// hits), and the function stays out of line, so that the hot loops of the callers keep nothing live for it.
+template <int MODE>
+__device__ __noinline__ float2 quotient_voxel(const float* __restrict__ g, const float* __restrict__ cc, float S, int z, int y,
+                                              int x, int D, int H, int W) {
+    const size_t HW = (size_t)H * W, V = (size_t)D * HW, p = (size_t)z * HW + (size_t)y * W + x;
+    float acc = 0.f, s = 0.f;
+#pragma unroll 1
+    for (int k = 0; k < 26; ++k) {
+        const int zz = z + off3_dz(k), yy = y + off3_dy(k), xx = x + off3_dx(k);
+        const bool in = zz >= 0 && zz < D && yy >= 0 && yy < H && xx >= 0 && xx < W;
+        const size_t q = (size_t)zz * HW + (size_t)yy * W + xx;
+        float a = MODE == 2 ? fabsf(__ldg(g + k * V + p)) : (in ? __ldg(g + k * V + q) : 0.f);
+        if (MODE == 1) a = fabsf(a);
+        const float w = __fdiv_rn(a, S);
+        s += w;
+        acc = fmaf(w, in ? __ldg(cc + q) : 0.f, acc);
+    }
+    return make_float2(acc, s);
 }
 
 #ifndef CSPN3D_PADDLE_BLOCKS
@@ -212,9 +241,11 @@ step3d_paddle_vec4_kernel(const float* __restrict__ g, const float* __restrict__
         acc[2] = fmaf(a2, r[o + 2], acc[2]);
         acc[3] = fmaf(a3, r[o + 3], acc[3]);
     }
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        acc[j] = cold_paddle(S[j], acc[j]) ? quotient_voxel<2>(g, cc, S[j], z, y, x + j, D, H, W).x : __fdiv_rn(acc[j], S[j]);
     const size_t o = (size_t)c * V + p;
-    const float4 v =
-        make_float4(__fdiv_rn(acc[0], S[0]), __fdiv_rn(acc[1], S[1]), __fdiv_rn(acc[2], S[2]), __fdiv_rn(acc[3], S[3]));
+    const float4 v = make_float4(acc[0], acc[1], acc[2], acc[3]);
     *reinterpret_cast<float4*>(dst + o) = v;
     if constexpr (FAN) fan_store(fan, o, v);
 }
@@ -222,7 +253,7 @@ step3d_paddle_vec4_kernel(const float* __restrict__ g, const float* __restrict__
 // '26sum' / '26sum_abs' (gathered affinities + centre term, the cspn.py-style generalisation) straight from the RAW guidance,
 // like the 'paddle' kernel above: a_k(p) = g_k(p + off_k) (zero outside the volume) is read where it lies -- an aligned float4
 // of the shifted row plus, for dx = +-1, one neighbouring scalar (an L1 hit: the next thread's quad) -- S = sum |a_k|,
-// w_k = a_k * (1 / S) (one division per voxel; where 1 / S overflows, i.e. S subnormal, the quotients are formed exactly),
+// w_k = a_k * (1 / S) (one division per voxel; where 1 / S overflows, i.e. S subnormal, or d0 is +-inf, quotient_voxel forms them),
 // kappa = 1 - sum_k w_k from the products as the weight-plane path forms it from its quotients, out = kappa d0 + sum_k w_k
 // cur(p + off_k).  No prep launch, no 27-plane workspace (1.65 GB for cfg4), 26 + 2 instead of 29 + 27/N planes per step.
 #ifndef CSPN3D_GATHER_BLOCKS
@@ -304,21 +335,16 @@ step3d_gather_vec4_kernel(const float* __restrict__ g, const float* __restrict__
         acc[2] = fmaf(w2, r[o + 2], acc[2]);
         acc[3] = fmaf(w3, r[o + 3], acc[3]);
     }
-    if (inv[0] > 8.0e37f || inv[1] > 8.0e37f || inv[2] > 8.0e37f || inv[3] > 8.0e37f) {   // cold: S subnormal, 1 / S overflowed
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            if (!(inv[j] > 8.0e37f)) continue;
-            acc[j] = 0.f; s[j] = 0.f;
-#pragma unroll
-            for (int k = 0; k < 26; ++k) {
-                const float av = j == 0 ? a[k].x : (j == 1 ? a[k].y : (j == 2 ? a[k].z : a[k].w));
-                const float w = __fdiv_rn(av, S[j]);
-                s[j] += w;
-                acc[j] = fmaf(w, rows[off3_dz(k) + 1][off3_dy(k) + 1][1 + off3_dx(k) + j], acc[j]);
-            }
-        }
-    }
+    // cold: S subnormal (1 / S overflowed), or d0 = +-inf, where kappa d0 is NaN or inf depending on whether kappa is exactly
+    // 0, so kappa must be 1 - sum_k a_k / S of the quotients (the products a_k * (1 / S) round differently)
     const float4 dz0 = __ldg(reinterpret_cast<const float4*>(d0 + (size_t)c * V + p));
+    const float d0v[4] = {dz0.x, dz0.y, dz0.z, dz0.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        if (inv[j] > 8.0e37f || fabsf(d0v[j]) == INFINITY) {
+            const float2 q = quotient_voxel<ABS ? 1 : 0>(g, cc, S[j], z, y, x + j, D, H, W);
+            acc[j] = q.x; s[j] = q.y;
+        }
     const size_t o = (size_t)c * V + p;
     const float4 v = make_float4(fmaf(1.f - s[0], dz0.x, acc[0]), fmaf(1.f - s[1], dz0.y, acc[1]),
                                  fmaf(1.f - s[2], dz0.z, acc[2]), fmaf(1.f - s[3], dz0.w, acc[3]));
@@ -421,6 +447,7 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
     for (int b0 = 0; b0 < B; b0 += G) {
         const int n = (B - b0 < G) ? B - b0 : G;  // volumes in this group
         const float* d0 = feat + (size_t)b0 * C * V;
+        const float* centre = mode == 2 ? nullptr : d0;   // 'paddle': no kappa d0 term in the steps
         float* o = out + (size_t)b0 * C * V;
         prep3d_kernel<<<dim3(g2.x, g2.y, D * n), block, 0, stream>>>(guidance + (size_t)b0 * 26 * V, wk, D, H, W, mode);
         ++*launches;
@@ -428,9 +455,9 @@ int generic3d_forward(const float* guidance, const float* feat, float* out, int 
         float* dst = (iters & 1) ? o : tmp;
         for (int it = 0; it < iters; ++it) {
             if (fan && it == iters - 1)
-                launch_plane_step<true>(vec4, wk, d0, cur, dst, n, C, D, H, W, stream, offset_fan(*fan, (size_t)b0 * C * V));
+                launch_plane_step<true>(vec4, wk, centre, cur, dst, n, C, D, H, W, stream, offset_fan(*fan, (size_t)b0 * C * V));
             else
-                launch_plane_step<false>(vec4, wk, d0, cur, dst, n, C, D, H, W, stream, Fan{});
+                launch_plane_step<false>(vec4, wk, centre, cur, dst, n, C, D, H, W, stream, Fan{});
             ++*launches;
             cur = dst;
             dst = (dst == o) ? tmp : o;

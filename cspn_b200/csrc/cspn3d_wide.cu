@@ -64,9 +64,6 @@ __device__ __forceinline__ float4 ld_stream4(const float* p) {
     return v;
 }
 
-// a sum of |gates| whose quotient form must be used: 0 (0/0 = NaN), subnormal (divided exactly), inf or NaN (weights 0 / NaN)
-__device__ __forceinline__ bool cold_sum(float S) { return !(S >= 1.17549435e-38f && S <= 3.40282347e38f); }
-
 // ---- prep: w_k and kappa of every voxel.  grid z = volume of the group * D + z ------------------------------------
 // At R = 2 the guidance is read twice (sum, then quotients) instead of holding 124 values per thread; the 26 of R = 1 stay
 // in registers and are read once.
@@ -184,7 +181,7 @@ step3k_vec_kernel(const float* __restrict__ w, const float* __restrict__ d0, con
     if (PADDLE) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            if (cold_sum(S[j])) {   // cold: form the quotients one by one, as the weight planes hold them
+            if (cold_paddle(S[j], acc[j])) {   // cold: form the quotients one by one, as the weight planes hold them
                 float a = 0.f;
                 // by 4, as ptxas unrolls it at R = 2: unrolled 26 times at R = 1, the division calls cost a spill
 #pragma unroll 4
@@ -248,7 +245,7 @@ step3k_scalar_kernel(const float* __restrict__ w, const float* __restrict__ d0, 
         }
     }
     if (PADDLE) {
-        if (cold_sum(S)) {
+        if (cold_paddle(S, acc)) {
             acc = 0.f;
             for (int k = 0; k < T::NT; ++k)
                 acc = fmaf(__fdiv_rn(fabsf(__ldg(wp + k * V)), S), tile[R + T::dz(k)][ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
