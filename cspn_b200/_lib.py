@@ -71,6 +71,10 @@ SIGNATURES = {
     'cspn_disparity_regression_fwd_f32': (_i, [_vp] * 2 + [_i] * 10 + [_vp]),
     'cspn_disparity_regression_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn_disparity_regression_bwd_f32': (_i, [_vp] * 3 + [_i] * 10 + [_vp, _sz, _vp]),
+    'cspn_concat_volume_fwd_f32': (_i, [_vp] * 3 + [_i] * 5 + [_vp]),
+    'cspn_concat_volume_bwd_f32': (_i, [_vp] * 3 + [_i] * 5 + [_vp]),
+    'cspn_gwc_volume_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp]),
+    'cspn_gwc_volume_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp]),
     'cspn_host_alloc': (_vp, [_sz]),
     'cspn_host_free': (None, [_vp]),
     'cspn_last_error': (_cp, []),

@@ -1099,3 +1099,131 @@ def disparity_regression(cost, out_shape=None, scale=None, align_corners=True, a
     if torch.is_grad_enabled() and cost.requires_grad:
         return _DisparityRegressionFn.apply(cost, D, H, W, align_corners, align_mode)
     return _disparity_fwd(cost, D, H, W, align_corners, align_mode)
+
+
+# ---- stereo cost volumes: PSMNet's concatenation volume and GwcNet's group-wise correlation volume ----------------------
+def _check_cost_volume(left, right, max_disp, num_groups=None):
+    """The checks of both volume fronts; every refusal comes before anything is allocated or narrowed to int."""
+    if left.dim() != 4 or right.shape != left.shape:
+        raise ValueError(f'left and right must be (B,F,H,W) of one shape, got {tuple(left.shape)} and {tuple(right.shape)}')
+    if isinstance(max_disp, bool) or not isinstance(max_disp, int) or max_disp < 1:
+        raise ValueError(f'max_disp must be an int >= 1, got {max_disp!r}')
+    B, F, H, W = left.shape
+    if min(B, F, H, W) < 1:
+        raise ValueError(f'the feature maps must not be empty, got {tuple(left.shape)}')
+    if num_groups is not None:
+        if isinstance(num_groups, bool) or not isinstance(num_groups, int) or num_groups < 1 or F % num_groups:
+            raise ValueError(f'num_groups must be an int >= 1 that divides F={F}, got {num_groups!r}')
+    if left.dtype != torch.float32 or right.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if left.device != right.device:
+        raise RuntimeError('left and right are on different devices')
+    if B > 2 ** 31 - 1 or 2 * F > 2 ** 31 - 1 or max_disp * H * W >= 2 ** 31:
+        raise _lib.CspnError(f'the cost volumes take B, 2F < 2^31 and < 2^31 elements per (B, channel) slice, got features '
+                             f'{tuple(left.shape)} and max_disp {max_disp}')
+    if not left.is_cuda:
+        raise _lib.CspnError('the cost volumes take CUDA tensors only (there is no host-buffer entry point for them)')
+
+
+def _concat_fwd(left, right, D):
+    """Forward only (no autograd) through cspn_concat_volume_fwd_f32, enqueued on the current stream."""
+    lc, rc_ = left.contiguous(), right.contiguous()
+    B, F, H, W = lc.shape
+    out = lc.new_empty((B, 2 * F, D, H, W))
+    with torch.cuda.device(lc.device):
+        rc = _lib.lib().cspn_concat_volume_fwd_f32(_ptr(lc), _ptr(rc_), _ptr(out), B, F, H, W, D, _stream(lc.device))
+    _lib.check(rc, 'cspn_concat_volume_fwd_f32')
+    return out
+
+
+def _concat_bwd(grad_out):
+    go = grad_out.contiguous()
+    B, F2, D, H, W = go.shape
+    gl, gr = go.new_empty((B, F2 // 2, H, W)), go.new_empty((B, F2 // 2, H, W))
+    with torch.cuda.device(go.device):
+        rc = _lib.lib().cspn_concat_volume_bwd_f32(_ptr(go), _ptr(gl), _ptr(gr), B, F2 // 2, H, W, D, _stream(go.device))
+    _lib.check(rc, 'cspn_concat_volume_bwd_f32')
+    return gl, gr
+
+
+def _gwc_fwd(left, right, D, G):
+    """Forward only (no autograd) through cspn_gwc_volume_fwd_f32, enqueued on the current stream."""
+    lc, rc_ = left.contiguous(), right.contiguous()
+    B, F, H, W = lc.shape
+    out = lc.new_empty((B, G, D, H, W))
+    with torch.cuda.device(lc.device):
+        rc = _lib.lib().cspn_gwc_volume_fwd_f32(_ptr(lc), _ptr(rc_), _ptr(out), B, F, H, W, D, G, _stream(lc.device))
+    _lib.check(rc, 'cspn_gwc_volume_fwd_f32')
+    return out
+
+
+def _gwc_bwd(left, right, grad_out):
+    lc, rc_, go = left.contiguous(), right.contiguous(), grad_out.contiguous()
+    B, F, H, W = lc.shape
+    gl, gr = torch.empty_like(lc), torch.empty_like(lc)
+    with torch.cuda.device(lc.device):
+        rc = _lib.lib().cspn_gwc_volume_bwd_f32(_ptr(lc), _ptr(rc_), _ptr(go), _ptr(gl), _ptr(gr), B, F, H, W, go.shape[2],
+                                                go.shape[1], _stream(lc.device))
+    _lib.check(rc, 'cspn_gwc_volume_bwd_f32')
+    return gl, gr
+
+
+class _ConcatVolumeFn(torch.autograd.Function):
+    """autograd seam of build_concat_volume without the torch-op shim.  The backward reads grad_out alone: no tensor is
+    saved."""
+
+    @staticmethod
+    def forward(ctx, left, right, D):
+        return _concat_fwd(left, right, D)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        gl, gr = _concat_bwd(grad_out)
+        return gl, gr, None
+
+
+class _GwcVolumeFn(torch.autograd.Function):
+    """autograd seam of build_gwc_volume without the torch-op shim: left and right are saved."""
+
+    @staticmethod
+    def forward(ctx, left, right, D, G):
+        ctx.save_for_backward(left, right)
+        return _gwc_fwd(left, right, D, G)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        left, right = ctx.saved_tensors
+        gl, gr = _gwc_bwd(left, right, grad_out)
+        return gl, gr, None, None
+
+
+def build_concat_volume(left, right, max_disp):
+    """PSMNet's concatenation cost volume in one kernel: left and right (B, F, H, W) fp32 CUDA features give
+    (B, 2F, max_disp, H, W) with out[:, c, d, y, x] = left[:, c, y, x] and out[:, F + c, d, y, x] = right[:, c, y, x - d] for
+    x >= d, +0.0 for x < d.  The values are copies (every bit kept); differentiable in both inputs, and left may be right.
+    DESIGN.md section 4.16."""
+    _check_cost_volume(left, right, max_disp)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.concat_volume(left, right, max_disp)
+    if torch.is_grad_enabled() and (left.requires_grad or right.requires_grad):
+        return _ConcatVolumeFn.apply(left, right, max_disp)
+    return _concat_fwd(left, right, max_disp)
+
+
+def build_gwc_volume(left, right, max_disp, num_groups):
+    """GwcNet's group-wise correlation cost volume in one kernel: left and right (B, F, H, W) fp32 CUDA features give
+    (B, G, max_disp, H, W) with out[:, g, d, y, x] = mean over the n = F / G channels c of group g of
+    left[:, c, y, x] * right[:, c, y, x - d] for x >= d, +0.0 for x < d (products summed in ascending c, then / n).
+    F % G != 0 is refused.  Differentiable in both inputs, and left may be right.  DESIGN.md section 4.16."""
+    _check_cost_volume(left, right, max_disp, num_groups)
+    if torch.compiler.is_compiling() or _use_torch_op():
+        return torch.ops.cspn_b200.gwc_volume(left, right, max_disp, num_groups)
+    if torch.is_grad_enabled() and (left.requires_grad or right.requires_grad):
+        return _GwcVolumeFn.apply(left, right, max_disp, num_groups)
+    return _gwc_fwd(left, right, max_disp, num_groups)

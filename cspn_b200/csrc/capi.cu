@@ -1,6 +1,7 @@
 // extern "C" surface of libcspn_b200.so (include/cspn_b200.h): argument checking, algorithm
 // dispatch, and the chunked host-buffer pipeline behind the *_host entry points.
 #include <cstdlib>
+#include <initializer_list>
 #include <mutex>
 #include <vector>
 
@@ -795,6 +796,103 @@ int cspn_disparity_regression_bwd_f32(const float* cost, const float* grad_out, 
     return on_device_of(cost, "cost", [&](int* launches) {
         return disparity_regression_backward(cost, grad_out, grad_cost, (long long)B * C, D, H, W, Do, Ho, Wo, align_corners,
                                              align_mode, workspace, (cudaStream_t)stream, launches);
+    });
+}
+
+// ---- stereo cost volumes (concatenation and group-wise correlation) -------------------------------------------------------
+// The sizes and F % G of an entry (G == 0: the concatenation volume); checked before any byte count is formed
+static int check_cost_volume_sizes(int B, int F, int H, int W, int D, int G, bool gwc) {
+    if (!positive(B, F, H, W, D) || (gwc && G < 1)) {
+        set_error("non-positive size B=%d F=%d H=%d W=%d D=%d%s", B, F, H, W, D, gwc && G < 1 ? " or G < 1" : "");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (gwc && F % G != 0) { set_error("num_groups=%d must divide F=%d", G, F); return CSPN_ERR_INVALID_ARGUMENT; }
+    return CSPN_OK;
+}
+
+struct Buf {
+    const void* p;
+    uintptr_t bytes;
+    const char* name;
+};
+
+// The pointers of an entry, the tile rule, then the overlaps: `in` are read and `outs` written.  An output may overlap neither an input
+// nor another output; inputs may alias one another (left may be right).
+static int check_cost_volume(int F, int H, int W, int D, int G, std::initializer_list<Buf> in, std::initializer_list<Buf> outs) {
+    uintptr_t bits = 0;
+    for (const auto* set : {&in, &outs})
+        for (const Buf& b : *set) {
+            if (!b.p) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+            bits |= reinterpret_cast<uintptr_t>(b.p);
+        }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (2ll * F >= (1ll << 31)) { set_error("unsupported shape: 2F >= 2^31 channels"); return CSPN_ERR_UNSUPPORTED; }
+    const char* why = "";
+    if (!cost_volume_launchable(F, H, W, D, G, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    for (const Buf& o : outs) {
+        for (const Buf& i : in)
+            if (overlap(o.p, o.bytes, i.p, i.bytes)) { set_error("%s overlaps %s", o.name, i.name); return CSPN_ERR_INVALID_ARGUMENT; }
+        for (const Buf& o2 : outs)
+            if (&o2 < &o && overlap(o.p, o.bytes, o2.p, o2.bytes)) {
+                set_error("%s overlaps %s", o.name, o2.name);
+                return CSPN_ERR_INVALID_ARGUMENT;
+            }
+    }
+    return CSPN_OK;
+}
+
+int cspn_concat_volume_fwd_f32(const float* left, const float* right, float* out, int B, int F, int H, int W, int D,
+                               cspn_stream_t stream) {
+    begin_call();
+    int rc = check_cost_volume_sizes(B, F, H, W, D, 0, false);
+    if (rc != CSPN_OK) return rc;
+    const uintptr_t n_in = span_bytes(B, F, (long long)H * W), n_out = span_bytes(B, F, 2ll * D * H * W);
+    rc = check_cost_volume(F, H, W, D, 0, {{left, n_in, "left"}, {right, n_in, "right"}}, {{out, n_out, "out"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(left, "left", [&](int* launches) {
+        return concat_volume_forward(left, right, out, B, F, H, W, D, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn_concat_volume_bwd_f32(const float* grad_out, float* grad_left, float* grad_right, int B, int F, int H, int W, int D,
+                               cspn_stream_t stream) {
+    begin_call();
+    int rc = check_cost_volume_sizes(B, F, H, W, D, 0, false);
+    if (rc != CSPN_OK) return rc;
+    const uintptr_t n_in = span_bytes(B, F, (long long)H * W), n_g = span_bytes(B, F, 2ll * D * H * W);
+    rc = check_cost_volume(F, H, W, D, 0, {{grad_out, n_g, "grad_out"}},
+                           {{grad_left, n_in, "grad_left"}, {grad_right, n_in, "grad_right"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(grad_out, "grad_out", [&](int* launches) {
+        return concat_volume_backward(grad_out, grad_left, grad_right, B, F, H, W, D, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn_gwc_volume_fwd_f32(const float* left, const float* right, float* out, int B, int F, int H, int W, int D, int G,
+                            cspn_stream_t stream) {
+    begin_call();
+    int rc = check_cost_volume_sizes(B, F, H, W, D, G, true);
+    if (rc != CSPN_OK) return rc;
+    const uintptr_t n_in = span_bytes(B, F, (long long)H * W), n_out = span_bytes(B, G, (long long)D * H * W);
+    rc = check_cost_volume(F, H, W, D, G, {{left, n_in, "left"}, {right, n_in, "right"}}, {{out, n_out, "out"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(left, "left", [&](int* launches) {
+        return gwc_volume_forward(left, right, out, B, F, H, W, D, G, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn_gwc_volume_bwd_f32(const float* left, const float* right, const float* grad_out, float* grad_left, float* grad_right,
+                            int B, int F, int H, int W, int D, int G, cspn_stream_t stream) {
+    begin_call();
+    int rc = check_cost_volume_sizes(B, F, H, W, D, G, true);
+    if (rc != CSPN_OK) return rc;
+    const uintptr_t n_in = span_bytes(B, F, (long long)H * W), n_g = span_bytes(B, G, (long long)D * H * W);
+    rc = check_cost_volume(F, H, W, D, G, {{left, n_in, "left"}, {right, n_in, "right"}, {grad_out, n_g, "grad_out"}},
+                           {{grad_left, n_in, "grad_left"}, {grad_right, n_in, "grad_right"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(left, "left", [&](int* launches) {
+        return gwc_volume_backward(left, right, grad_out, grad_left, grad_right, B, F, H, W, D, G, (cudaStream_t)stream,
+                                   launches);
     });
 }
 

@@ -195,4 +195,16 @@ int disparity_regression_backward(const float* cost, const float* grad_out, floa
                                   int W, int Do, int Ho, int Wo, int align_corners, int align_mode, void* ws, cudaStream_t st,
                                   int* launches);
 
+// Stereo cost volumes from left and right feature maps (cost_volume.cu): the concatenation volume (G == 0) and the
+// group-wise correlation volume; arguments checked by the caller (sizes, F % G, pointers, then launchable)
+int cost_volume_launchable(int F, int H, int W, int D, int G, const char** why);
+int concat_volume_forward(const float* left, const float* right, float* out, int B, int F, int H, int W, int D,
+                          cudaStream_t st, int* launches);
+int concat_volume_backward(const float* grad_out, float* grad_left, float* grad_right, int B, int F, int H, int W, int D,
+                           cudaStream_t st, int* launches);
+int gwc_volume_forward(const float* left, const float* right, float* out, int B, int F, int H, int W, int D, int G,
+                       cudaStream_t st, int* launches);
+int gwc_volume_backward(const float* left, const float* right, const float* grad_out, float* grad_left, float* grad_right,
+                        int B, int F, int H, int W, int D, int G, cudaStream_t st, int* launches);
+
 }  // namespace cspn

@@ -48,6 +48,12 @@
 //       (cost (B, C, d, h, w) resized to (D, H, W), softmax over D, expectation of the index: (B, C, H, W))
 //   disparity_regression_backward(Tensor cost, Tensor grad_out, int D, int H, int W, bool align_corners, int align_mode)
 //       -> Tensor   (grad_cost (B, C, d, h, w); the softmax is recomputed from cost)
+//   concat_volume(Tensor left, Tensor right, int max_disp) -> Tensor
+//       (PSMNet's concatenation volume: left, right (B, F, H, W) -> (B, 2F, max_disp, H, W))
+//   concat_volume_backward(Tensor grad_out) -> (Tensor, Tensor)      (grad_left, grad_right from grad_out alone)
+//   gwc_volume(Tensor left, Tensor right, int max_disp, int num_groups) -> Tensor
+//       (GwcNet's group-wise correlation volume: (B, F, H, W) -> (B, num_groups, max_disp, H, W))
+//   gwc_volume_backward(Tensor left, Tensor right, Tensor grad_out) -> (Tensor, Tensor)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -581,6 +587,79 @@ at::Tensor disparity_regression_backward_cuda(const at::Tensor& cost, const at::
     return gc;
 }
 
+// Stereo cost volumes: left, right (B, F, H, W) -> (B, 2F, D, H, W) (concatenation) or (B, G, D, H, W) (group-wise
+// correlation).  The C ABI takes int sizes and < 2^31 elements per (B, channel) slice: refuse the rest before allocating
+void check_cost_volume(const at::Tensor& left, const at::Tensor& right, int64_t D, int64_t G) {
+    TORCH_CHECK_VALUE(left.dim() == 4 && left.sizes() == right.sizes(), "left and right must be (B,F,H,W) of one shape, got ",
+                      left.sizes(), " and ", right.sizes());
+    TORCH_CHECK_VALUE(D >= 1, "max_disp must be >= 1, got ", D);
+    TORCH_CHECK_VALUE(G >= 1 && left.size(1) % G == 0, "num_groups must be >= 1 and divide F=", left.size(1), ", got ", G);
+    TORCH_CHECK(left.scalar_type() == at::kFloat && right.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(left.device() == right.device(), "left and right are on different devices");
+    TORCH_CHECK(left.size(0) < ((int64_t)1 << 31) && 2 * left.size(1) < ((int64_t)1 << 31) &&
+                    volume_fits_int(D, left.size(2), left.size(3)),
+                "the cost volumes take B, 2F < 2^31 and < 2^31 elements per (B, channel) slice, got features ", left.sizes(),
+                " and max_disp ", D);
+}
+
+at::Tensor concat_volume_cuda(const at::Tensor& left, const at::Tensor& right, int64_t D) {
+    check_cost_volume(left, right, D, 1);
+    const c10::cuda::CUDAGuard guard(left.device());
+    const at::Tensor l = left.contiguous(), r = right.contiguous();
+    at::Tensor out = at::empty({l.size(0), 2 * l.size(1), D, l.size(2), l.size(3)}, l.options());
+    if (out.numel())
+        check_rc(cspn_concat_volume_fwd_f32(fptr(l), fptr(r), mptr(out), (int)l.size(0), (int)l.size(1), (int)l.size(2),
+                                            (int)l.size(3), (int)D, current_stream()),
+                 "cspn_concat_volume_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> concat_volume_backward_cuda(const at::Tensor& grad_out) {
+    TORCH_CHECK_VALUE(grad_out.dim() == 5 && grad_out.size(1) % 2 == 0, "grad_out must be (B,2F,D,H,W), got ", grad_out.sizes());
+    TORCH_CHECK(grad_out.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(grad_out.size(0) < ((int64_t)1 << 31) && grad_out.size(1) < ((int64_t)1 << 31) &&
+                    volume_fits_int(grad_out.size(2), grad_out.size(3), grad_out.size(4)),
+                "the cost volumes take B, 2F < 2^31 and < 2^31 elements per (B, channel) slice, got grad_out ", grad_out.sizes());
+    const c10::cuda::CUDAGuard guard(grad_out.device());
+    const at::Tensor go = grad_out.contiguous();
+    const int64_t B = go.size(0), F = go.size(1) / 2, H = go.size(3), W = go.size(4);
+    at::Tensor gl = at::empty({B, F, H, W}, go.options()), gr = at::empty({B, F, H, W}, go.options());
+    if (gl.numel() && go.size(2))
+        check_rc(cspn_concat_volume_bwd_f32(fptr(go), mptr(gl), mptr(gr), (int)B, (int)F, (int)H, (int)W, (int)go.size(2),
+                                            current_stream()),
+                 "cspn_concat_volume_bwd_f32");
+    return {gl, gr};
+}
+
+at::Tensor gwc_volume_cuda(const at::Tensor& left, const at::Tensor& right, int64_t D, int64_t G) {
+    check_cost_volume(left, right, D, G);
+    const c10::cuda::CUDAGuard guard(left.device());
+    const at::Tensor l = left.contiguous(), r = right.contiguous();
+    at::Tensor out = at::empty({l.size(0), G, D, l.size(2), l.size(3)}, l.options());
+    if (out.numel())
+        check_rc(cspn_gwc_volume_fwd_f32(fptr(l), fptr(r), mptr(out), (int)l.size(0), (int)l.size(1), (int)l.size(2),
+                                         (int)l.size(3), (int)D, (int)G, current_stream()),
+                 "cspn_gwc_volume_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> gwc_volume_backward_cuda(const at::Tensor& left, const at::Tensor& right,
+                                                            const at::Tensor& grad_out) {
+    TORCH_CHECK_VALUE(grad_out.dim() == 5 && left.dim() == 4 && grad_out.size(0) == left.size(0) &&
+                          grad_out.size(3) == left.size(2) && grad_out.size(4) == left.size(3),
+                      "grad_out must be (B,G,D,H,W) of left ", left.sizes(), ", got ", grad_out.sizes());
+    check_cost_volume(left, right, grad_out.size(2), grad_out.size(1));
+    TORCH_CHECK(grad_out.scalar_type() == at::kFloat && grad_out.device() == left.device(), "grad_out must be fp32 on left's device");
+    const c10::cuda::CUDAGuard guard(left.device());
+    const at::Tensor l = left.contiguous(), r = right.contiguous(), go = grad_out.contiguous();
+    at::Tensor gl = at::empty_like(l), gr = at::empty_like(l);
+    if (gl.numel())
+        check_rc(cspn_gwc_volume_bwd_f32(fptr(l), fptr(r), fptr(go), mptr(gl), mptr(gr), (int)l.size(0), (int)l.size(1),
+                                         (int)l.size(2), (int)l.size(3), (int)go.size(2), (int)go.size(1), current_stream()),
+                 "cspn_gwc_volume_bwd_f32");
+    return {gl, gr};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -618,6 +697,10 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("disparity_regression(Tensor cost, int D, int H, int W, bool align_corners, int align_mode) -> Tensor");
     m.def("disparity_regression_backward(Tensor cost, Tensor grad_out, int D, int H, int W, bool align_corners, int align_mode) "
           "-> Tensor");
+    m.def("concat_volume(Tensor left, Tensor right, int max_disp) -> Tensor");
+    m.def("concat_volume_backward(Tensor grad_out) -> (Tensor, Tensor)");
+    m.def("gwc_volume(Tensor left, Tensor right, int max_disp, int num_groups) -> Tensor");
+    m.def("gwc_volume_backward(Tensor left, Tensor right, Tensor grad_out) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -643,4 +726,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("resize_trilinear_backward", &resize_trilinear_backward_cuda);
     m.impl("disparity_regression", &disparity_regression_cuda);
     m.impl("disparity_regression_backward", &disparity_regression_backward_cuda);
+    m.impl("concat_volume", &concat_volume_cuda);
+    m.impl("concat_volume_backward", &concat_volume_backward_cuda);
+    m.impl("gwc_volume", &gwc_volume_cuda);
+    m.impl("gwc_volume_backward", &gwc_volume_backward_cuda);
 }

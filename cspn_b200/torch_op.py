@@ -288,6 +288,52 @@ def _register():
 
     lib.register_autograd('cspn_b200::disparity_regression', backward_disparity, setup_context=setup_disparity)
 
+    @lib.register_fake('cspn_b200::concat_volume')
+    def _(left, right, max_disp):
+        torch._check(left.dim() == 4 and left.shape == right.shape, lambda: 'left and right must be (B,F,H,W) of one shape')
+        torch._check(max_disp >= 1, lambda: 'max_disp must be >= 1')
+        B, F, H, W = left.shape
+        return left.new_empty((B, 2 * F, max_disp, H, W))
+
+    @lib.register_fake('cspn_b200::concat_volume_backward')
+    def _(grad_out):
+        torch._check(grad_out.dim() == 5 and grad_out.shape[1] % 2 == 0, lambda: 'grad_out must be (B,2F,D,H,W)')
+        B, F2, D, H, W = grad_out.shape
+        return grad_out.new_empty((B, F2 // 2, H, W)), grad_out.new_empty((B, F2 // 2, H, W))
+
+    def setup_concat(ctx, inputs, output):        # the backward reads grad_out alone: no tensor is saved
+        pass
+
+    def backward_concat(ctx, grad_out):
+        gl, gr = torch.ops.cspn_b200.concat_volume_backward(grad_out.contiguous())
+        return gl, gr, None
+
+    lib.register_autograd('cspn_b200::concat_volume', backward_concat, setup_context=setup_concat)
+
+    @lib.register_fake('cspn_b200::gwc_volume')
+    def _(left, right, max_disp, num_groups):
+        torch._check(left.dim() == 4 and left.shape == right.shape, lambda: 'left and right must be (B,F,H,W) of one shape')
+        torch._check(max_disp >= 1 and num_groups >= 1 and left.shape[1] % num_groups == 0,
+                     lambda: 'max_disp >= 1 and num_groups >= 1 dividing F')
+        B, F, H, W = left.shape
+        return left.new_empty((B, num_groups, max_disp, H, W))
+
+    @lib.register_fake('cspn_b200::gwc_volume_backward')
+    def _(left, right, grad_out):
+        torch._check(left.dim() == 4 and grad_out.dim() == 5, lambda: 'left must be (B,F,H,W) and grad_out (B,G,D,H,W)')
+        return left.new_empty(left.shape), left.new_empty(left.shape)
+
+    def setup_gwc(ctx, inputs, output):
+        left, right, max_disp, num_groups = inputs
+        ctx.save_for_backward(left, right)
+
+    def backward_gwc(ctx, grad_out):
+        left, right = ctx.saved_tensors
+        gl, gr = torch.ops.cspn_b200.gwc_volume_backward(left, right, grad_out.contiguous())
+        return gl, gr, None, None
+
+    lib.register_autograd('cspn_b200::gwc_volume', backward_gwc, setup_context=setup_gwc)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

@@ -423,6 +423,33 @@ CSPN_API int cspn_disparity_regression_bwd_f32(const float* cost, const float* g
                                   int D, int H, int W, int Do, int Ho, int Wo, int align_corners, int align_mode,
                                   void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- stereo cost volumes from left and right feature maps ----------------------------------------------------------
+ * left and right are [B][F][H][W] (the reference and the target image's features); D >= 1 disparities, the matched pixel
+ * of left[..., x] at disparity d is right[..., x - d].  Cells with x < d are +0.0 whatever the inputs hold; D > W is allowed.
+ *   concat (PSMNet):  out [B][2F][D][H][W]: out[b][c][d][y][x] = left[b][c][y][x], out[b][F+c][d][y][x] = right[b][c][y][x-d]
+ *                     (copies: every bit is kept)
+ *   gwc (GwcNet):     out [B][G][D][H][W], n = F / G: out[b][g][d][y][x] = (sum_{c in group g} left*right) / n, the products
+ *                     summed in ascending c from the first, every operation rounded on its own
+ * Backward, from grad_out (the volume's shape), both gradients [B][F][H][W], sums in ascending d from d = 0:
+ *   concat:  grad_left[c][y][x] = sum_{d<=min(x,D-1)} g[c][d][y][x], grad_right[c][y][x] = sum_{d<=min(W-1-x,D-1)} g[F+c][d][y][x+d]
+ *   gwc:     t = g / n;  grad_left = sum_d t[grp][d][y][x] * right[c][y][x-d],  grad_right = sum_d t[grp][d][y][x+d] * left[c][y][x+d]
+ * No atomics, no workspace, every output element written once; the bits depend on the arguments only (DESIGN.md section
+ * 4.16).  left may be right.  CSPN_ERR_INVALID_ARGUMENT for a null or not 4-byte aligned pointer, a size < 1, F % G != 0,
+ * or an output that overlaps an input or the other output.  CSPN_ERR_UNSUPPORTED for 2F >= 2^31, D*H*W >= 2^31, and a D
+ * whose 1-column tile does not fit in shared memory (concat: min(D, W) above about 14500; gwc: n * min(D, W) above about
+ * 58000, or D above about 3200).  One launch each.  No allocation, no synchronisation. */
+CSPN_API int cspn_concat_volume_fwd_f32(const float* left, const float* right, float* out, int B, int F, int H, int W, int D,
+                                  cspn_stream_t stream);
+
+CSPN_API int cspn_concat_volume_bwd_f32(const float* grad_out, float* grad_left, float* grad_right, int B, int F, int H,
+                                  int W, int D, cspn_stream_t stream);
+
+CSPN_API int cspn_gwc_volume_fwd_f32(const float* left, const float* right, float* out, int B, int F, int H, int W, int D,
+                                  int G, cspn_stream_t stream);
+
+CSPN_API int cspn_gwc_volume_bwd_f32(const float* left, const float* right, const float* grad_out, float* grad_left,
+                                  float* grad_right, int B, int F, int H, int W, int D, int G, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
