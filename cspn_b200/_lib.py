@@ -75,6 +75,8 @@ SIGNATURES = {
     'cspn_concat_volume_bwd_f32': (_i, [_vp] * 3 + [_i] * 5 + [_vp]),
     'cspn_gwc_volume_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp]),
     'cspn_gwc_volume_bwd_f32': (_i, [_vp] * 5 + [_i] * 6 + [_vp]),
+    'cspn_affinity_pool2d_fwd_f32': (_i, [_vp] * 3 + [_i] * 5 + [_vp] * 2),
+    'cspn_affinity_pool2d_bwd_f32': (_i, [_vp] * 6 + [_i] * 5 + [_vp] * 2),
     'cspn_host_alloc': (_vp, [_sz]),
     'cspn_host_free': (None, [_vp]),
     'cspn_last_error': (_cp, []),

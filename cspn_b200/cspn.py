@@ -10,6 +10,7 @@ device memory, the current stream and autograd plumbing.  There is no CPU / eage
 import torch
 import torch.nn as nn
 
+import ctypes
 import operator
 import os
 
@@ -1227,3 +1228,100 @@ def build_gwc_volume(left, right, max_disp, num_groups):
     if torch.is_grad_enabled() and (left.requires_grad or right.requires_grad):
         return _GwcVolumeFn.apply(left, right, max_disp, num_groups)
     return _gwc_fwd(left, right, max_disp, num_groups)
+
+
+# ---- affinity pooling: the CSPN stereo network's convolutional spatial pyramid pooling --------------------------------------
+def _check_affinity_pool(feat, gate, kernel_sizes):
+    """The checks of affinity_pool2d; every refusal comes before anything is allocated or narrowed to int.  Returns the
+    kernel sizes as a tuple of ints."""
+    if feat.dim() != 4 or gate.dim() != 4:
+        raise ValueError(f'feat must be (B,C,H,W) and gate (B,L,H,W), got {tuple(feat.shape)} and {tuple(gate.shape)}')
+    B, C, H, W = feat.shape
+    if min(B, C, H, W) < 1:
+        raise ValueError(f'feat must not be empty, got {tuple(feat.shape)}')
+    if (isinstance(kernel_sizes, (str, bytes)) or not hasattr(kernel_sizes, '__len__')
+            or any(isinstance(p, bool) or not isinstance(p, int) for p in kernel_sizes)):
+        raise ValueError(f'kernel_sizes must be a sequence of ints, got {kernel_sizes!r}')
+    ks = tuple(kernel_sizes)
+    if not 1 <= len(ks) <= 8:
+        raise ValueError(f'kernel_sizes must hold 1 to 8 sizes, got {len(ks)}')
+    if any(not 1 <= p <= min(H, W) for p in ks):
+        raise ValueError(f'kernel sizes must be in [1, min(H, W) = {min(H, W)}], got {ks}')
+    if tuple(gate.shape) != (B, len(ks), H, W):
+        raise ValueError(f'gate must be (B, L, H, W) = {(B, len(ks), H, W)}, got {tuple(gate.shape)}')
+    if feat.dtype != torch.float32 or gate.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if feat.device != gate.device:
+        raise RuntimeError('feat and gate are on different devices')
+    if B > 2 ** 31 - 1 or C > 2 ** 31 - 1 or H * W >= 2 ** 31:
+        raise _lib.CspnError(f'affinity_pool2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got feat '
+                             f'{tuple(feat.shape)}')
+    if not feat.is_cuda:
+        raise _lib.CspnError('affinity_pool2d takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return ks
+
+
+def _c_sizes(ks):
+    return (ctypes.c_int * len(ks))(*ks)
+
+
+def _pool_fwd(feat, gate, ks):
+    """Forward only (no autograd) through cspn_affinity_pool2d_fwd_f32: the packed levels, on the current stream."""
+    f, g = feat.contiguous(), gate.contiguous()
+    B, C, H, W = f.shape
+    out = f.new_empty((B * C * sum((H // p) * (W // p) for p in ks),))
+    with torch.cuda.device(f.device):
+        rc = _lib.lib().cspn_affinity_pool2d_fwd_f32(_ptr(f), _ptr(g), _ptr(out), B, C, H, W, len(ks), _c_sizes(ks),
+                                                      _stream(f.device))
+    _lib.check(rc, 'cspn_affinity_pool2d_fwd_f32')
+    return out
+
+
+def _pool_bwd(feat, gate, out, grad_out, ks):
+    f, g, o, go = feat.contiguous(), gate.contiguous(), out.contiguous(), grad_out.contiguous()
+    B, C, H, W = f.shape
+    gf, gg = torch.empty_like(f), torch.empty_like(g)
+    with torch.cuda.device(f.device):
+        rc = _lib.lib().cspn_affinity_pool2d_bwd_f32(_ptr(f), _ptr(g), _ptr(o), _ptr(go), _ptr(gf), _ptr(gg), B, C, H, W, len(ks),
+                                                      _c_sizes(ks), _stream(f.device))
+    _lib.check(rc, 'cspn_affinity_pool2d_bwd_f32')
+    return gf, gg
+
+
+class _AffinityPoolFn(torch.autograd.Function):
+    """autograd seam of affinity_pool2d without the torch-op shim: feat, gate and the packed output are saved."""
+
+    @staticmethod
+    def forward(ctx, feat, gate, ks):
+        out = _pool_fwd(feat, gate, ks)
+        ctx.ks = ks
+        ctx.save_for_backward(feat, gate, out)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        feat, gate, out = ctx.saved_tensors
+        gf, gg = _pool_bwd(feat, gate, out, grad_out, ctx.ks)
+        return gf, gg, None
+
+
+def affinity_pool2d(feat, gate, kernel_sizes):
+    """The CSPN stereo network's convolutional spatial pyramid pooling, every level in one launch: feat (B, C, H, W) and
+    gate (B, L, H, W) fp32 CUDA tensors and L kernel sizes p_l (1 <= L <= 8, 1 <= p_l <= min(H, W), any order, repeats
+    allowed) give a tuple of L tensors (B, C, H // p_l, W // p_l).  Level l pools the windows of F.avg_pool2d(x, p_l)
+    (stride p_l, no padding, floor mode) with the weights w = |g_l| / sum_window |g_l| of gate channel l, shared by all
+    channels: out_l[:, c, i, j] = sum_window w * feat[:, c].  A constant gate gives avg_pool2d; an all-zero window gives NaN.
+    Differentiable in feat and gate, with a deterministic backward.  DESIGN.md section 4.17."""
+    ks = _check_affinity_pool(feat, gate, kernel_sizes)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        flat = torch.ops.cspn_b200.affinity_pool2d(feat, gate, list(ks))
+    elif torch.is_grad_enabled() and (feat.requires_grad or gate.requires_grad):
+        flat = _AffinityPoolFn.apply(feat, gate, ks)
+    else:
+        flat = _pool_fwd(feat, gate, ks)
+    B, C, H, W = feat.shape
+    shapes = [(B, C, H // p, W // p) for p in ks]
+    return tuple(v.view(s) for v, s in zip(flat.split([B * C * h * w for _, _, h, w in shapes]), shapes))

@@ -896,6 +896,82 @@ int cspn_gwc_volume_bwd_f32(const float* left, const float* right, const float* 
     });
 }
 
+// ---- affinity pooling (the CSPN stereo network's spatial pyramid pooling) ---------------------------------------------------
+// The sizes, the levels, the pointers, the launch limits, then the overlaps, in that order: `in` are read and `outs` written.
+// *n_out is the packed output's element count per (B, channel), sum_l (H / p_l) * (W / p_l).
+static int check_affinity_pool(int B, int C, int H, int W, int L, const int* ks, long long* n_out,
+                               std::initializer_list<Buf> in, std::initializer_list<Buf> outs) {
+    if (!positive(B, C, H, W)) { set_error("non-positive size B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (L < 1 || L > kAffinityPoolMaxLevels) { set_error("the number of levels L=%d must be 1..8", L); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!ks) { set_error("null kernel_sizes"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const int lim = H < W ? H : W;
+    *n_out = 0;
+    for (int l = 0; l < L; ++l) {
+        if (ks[l] < 1 || ks[l] > lim) {
+            set_error("kernel_sizes[%d]=%d must be in [1, min(H, W)=%d]", l, ks[l], lim);
+            return CSPN_ERR_INVALID_ARGUMENT;
+        }
+        *n_out += (long long)(H / ks[l]) * (W / ks[l]);
+    }
+    uintptr_t bits = 0;
+    for (const auto* set : {&in, &outs})
+        for (const Buf& b : *set) {
+            if (!b.p) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+            bits |= reinterpret_cast<uintptr_t>(b.p);
+        }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!affinity_pool_launchable(B, C, H, W, L, ks, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+// An output may overlap neither an input nor another output; inputs may alias one another
+static int check_disjoint(std::initializer_list<Buf> in, std::initializer_list<Buf> outs) {
+    for (const Buf& o : outs) {
+        for (const Buf& i : in)
+            if (overlap(o.p, o.bytes, i.p, i.bytes)) { set_error("%s overlaps %s", o.name, i.name); return CSPN_ERR_INVALID_ARGUMENT; }
+        for (const Buf& o2 : outs)
+            if (&o2 < &o && overlap(o.p, o.bytes, o2.p, o2.bytes)) {
+                set_error("%s overlaps %s", o.name, o2.name);
+                return CSPN_ERR_INVALID_ARGUMENT;
+            }
+    }
+    return CSPN_OK;
+}
+
+int cspn_affinity_pool2d_fwd_f32(const float* feat, const float* gate, float* out, int B, int C, int H, int W, int L,
+                                 const int* kernel_sizes, cspn_stream_t stream) {
+    begin_call();
+    long long n;
+    int rc = check_affinity_pool(B, C, H, W, L, kernel_sizes, &n, {{feat, 0, "feat"}, {gate, 0, "gate"}}, {{out, 0, "out"}});
+    if (rc != CSPN_OK) return rc;
+    rc = check_disjoint({{feat, span_bytes(B, C, (long long)H * W), "feat"}, {gate, span_bytes(B, L, (long long)H * W), "gate"}},
+                        {{out, span_bytes(B, C, n), "out"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return affinity_pool_forward(feat, gate, out, B, C, H, W, L, kernel_sizes, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn_affinity_pool2d_bwd_f32(const float* feat, const float* gate, const float* out, const float* grad_out,
+                                 float* grad_feat, float* grad_gate, int B, int C, int H, int W, int L, const int* kernel_sizes,
+                                 cspn_stream_t stream) {
+    begin_call();
+    long long n;
+    int rc = check_affinity_pool(B, C, H, W, L, kernel_sizes, &n,
+                                 {{feat, 0, "feat"}, {gate, 0, "gate"}, {out, 0, "out"}, {grad_out, 0, "grad_out"}},
+                                 {{grad_feat, 0, "grad_feat"}, {grad_gate, 0, "grad_gate"}});
+    if (rc != CSPN_OK) return rc;
+    const uintptr_t n_f = span_bytes(B, C, (long long)H * W), n_g = span_bytes(B, L, (long long)H * W), n_o = span_bytes(B, C, n);
+    rc = check_disjoint({{feat, n_f, "feat"}, {gate, n_g, "gate"}, {out, n_o, "out"}, {grad_out, n_o, "grad_out"}},
+                        {{grad_feat, n_f, "grad_feat"}, {grad_gate, n_g, "grad_gate"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return affinity_pool_backward(feat, gate, out, grad_out, grad_feat, grad_gate, B, C, H, W, L, kernel_sizes,
+                                      (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

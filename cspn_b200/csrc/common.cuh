@@ -207,4 +207,15 @@ int gwc_volume_forward(const float* left, const float* right, float* out, int B,
 int gwc_volume_backward(const float* left, const float* right, const float* grad_out, float* grad_left, float* grad_right,
                         int B, int F, int H, int W, int D, int G, cudaStream_t st, int* launches);
 
+// Affinity pooling, the CSPN stereo network's spatial pyramid pooling (affinity_pool.cu): L <= 8 levels of feat (B, C, H, W)
+// pooled with the gates (B, L, H, W) into one level-major buffer; arguments checked by the caller (sizes, kernel sizes,
+// pointers, then launchable)
+constexpr int kAffinityPoolMaxLevels = 8;
+int affinity_pool_launchable(int B, int C, int H, int W, int L, const int* kernel_sizes, const char** why);
+int affinity_pool_forward(const float* feat, const float* gate, float* out, int B, int C, int H, int W, int L,
+                          const int* kernel_sizes, cudaStream_t st, int* launches);
+int affinity_pool_backward(const float* feat, const float* gate, const float* out, const float* grad_out, float* grad_feat,
+                           float* grad_gate, int B, int C, int H, int W, int L, const int* kernel_sizes, cudaStream_t st,
+                           int* launches);
+
 }  // namespace cspn

@@ -54,6 +54,11 @@
 //   gwc_volume(Tensor left, Tensor right, int max_disp, int num_groups) -> Tensor
 //       (GwcNet's group-wise correlation volume: (B, F, H, W) -> (B, num_groups, max_disp, H, W))
 //   gwc_volume_backward(Tensor left, Tensor right, Tensor grad_out) -> (Tensor, Tensor)
+//   affinity_pool2d(Tensor feat, Tensor gate, int[] kernel_sizes) -> Tensor
+//       (CSPN's spatial pyramid pooling: feat (B, C, H, W) and gate (B, L, H, W) -> the L levels (B, C, H/p, W/p) packed
+//       level-major in one flat tensor)
+//   affinity_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] kernel_sizes) -> (Tensor, Tensor)
+//       (grad_feat, grad_gate; out and grad_out packed as the forward's result)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -63,6 +68,7 @@
 #include <optional>
 #include <tuple>
 #include <utility>
+#include <vector>
 
 #include "../../include/cspn_b200.h"
 
@@ -660,6 +666,63 @@ std::tuple<at::Tensor, at::Tensor> gwc_volume_backward_cuda(const at::Tensor& le
     return {gl, gr};
 }
 
+// Affinity pooling: feat (B, C, H, W), gate (B, L, H, W), L kernel sizes -> one flat tensor, level l's (B, C, H/p, W/p)
+// after the levels before it.  The C ABI takes int sizes and < 2^31 elements per (B, channel) slice: refuse the rest before
+// allocating.  Returns the packed length per (B, channel).
+int64_t check_affinity_pool(const at::Tensor& feat, const at::Tensor& gate, at::IntArrayRef ks) {
+    TORCH_CHECK_VALUE(feat.dim() == 4 && gate.dim() == 4 && gate.size(0) == feat.size(0) && gate.size(2) == feat.size(2) &&
+                          gate.size(3) == feat.size(3),
+                      "feat must be (B,C,H,W) and gate (B,L,H,W), got ", feat.sizes(), " and ", gate.sizes());
+    TORCH_CHECK_VALUE(ks.size() >= 1 && ks.size() <= 8 && gate.size(1) == (int64_t)ks.size(),
+                      "kernel_sizes must hold 1..8 sizes, one per gate channel, got ", ks, " for gate ", gate.sizes());
+    TORCH_CHECK(feat.scalar_type() == at::kFloat && gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(feat.device() == gate.device(), "feat and gate are on different devices");
+    const int64_t H = feat.size(2), W = feat.size(3);
+    TORCH_CHECK_VALUE(feat.numel() > 0, "feat must not be empty, got ", feat.sizes());
+    int64_t n = 0;
+    for (int64_t p : ks) {
+        TORCH_CHECK_VALUE(p >= 1 && p <= std::min(H, W), "kernel sizes must be in [1, min(H, W)], got ", ks, " for ", H, "x", W);
+        n += (H / p) * (W / p);
+    }
+    TORCH_CHECK(feat.size(0) < ((int64_t)1 << 31) && feat.size(1) < ((int64_t)1 << 31) && volume_fits_int(1, H, W),
+                "affinity_pool2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got feat ", feat.sizes());
+    return n;
+}
+
+std::vector<int> int_sizes(at::IntArrayRef ks) { return std::vector<int>(ks.begin(), ks.end()); }
+
+at::Tensor affinity_pool2d_cuda(const at::Tensor& feat, const at::Tensor& gate, at::IntArrayRef ks) {
+    const int64_t n = check_affinity_pool(feat, gate, ks);
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), g = gate.contiguous();
+    at::Tensor out = at::empty({f.size(0) * f.size(1) * n}, f.options());
+    const std::vector<int> k = int_sizes(ks);
+    check_rc(cspn_affinity_pool2d_fwd_f32(fptr(f), fptr(g), mptr(out), (int)f.size(0), (int)f.size(1), (int)f.size(2),
+                                          (int)f.size(3), (int)k.size(), k.data(), current_stream()),
+             "cspn_affinity_pool2d_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> affinity_pool2d_backward_cuda(const at::Tensor& feat, const at::Tensor& gate,
+                                                                 const at::Tensor& out, const at::Tensor& grad_out,
+                                                                 at::IntArrayRef ks) {
+    const int64_t n = check_affinity_pool(feat, gate, ks);
+    const int64_t len = feat.size(0) * feat.size(1) * n;
+    TORCH_CHECK_VALUE(out.dim() == 1 && out.size(0) == len && grad_out.dim() == 1 && grad_out.size(0) == len,
+                      "out and grad_out must be the packed levels (", len, "), got ", out.sizes(), " and ", grad_out.sizes());
+    TORCH_CHECK(out.scalar_type() == at::kFloat && grad_out.scalar_type() == at::kFloat && out.device() == feat.device() &&
+                    grad_out.device() == feat.device(),
+                "out and grad_out must be fp32 on feat's device");
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), g = gate.contiguous(), o = out.contiguous(), go = grad_out.contiguous();
+    at::Tensor gf = at::empty_like(f), gg = at::empty_like(g);
+    const std::vector<int> k = int_sizes(ks);
+    check_rc(cspn_affinity_pool2d_bwd_f32(fptr(f), fptr(g), fptr(o), fptr(go), mptr(gf), mptr(gg), (int)f.size(0), (int)f.size(1),
+                                          (int)f.size(2), (int)f.size(3), (int)k.size(), k.data(), current_stream()),
+             "cspn_affinity_pool2d_bwd_f32");
+    return {gf, gg};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -701,6 +764,8 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("concat_volume_backward(Tensor grad_out) -> (Tensor, Tensor)");
     m.def("gwc_volume(Tensor left, Tensor right, int max_disp, int num_groups) -> Tensor");
     m.def("gwc_volume_backward(Tensor left, Tensor right, Tensor grad_out) -> (Tensor, Tensor)");
+    m.def("affinity_pool2d(Tensor feat, Tensor gate, int[] kernel_sizes) -> Tensor");
+    m.def("affinity_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] kernel_sizes) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -730,4 +795,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("concat_volume_backward", &concat_volume_backward_cuda);
     m.impl("gwc_volume", &gwc_volume_cuda);
     m.impl("gwc_volume_backward", &gwc_volume_backward_cuda);
+    m.impl("affinity_pool2d", &affinity_pool2d_cuda);
+    m.impl("affinity_pool2d_backward", &affinity_pool2d_backward_cuda);
 }

@@ -334,6 +334,32 @@ def _register():
 
     lib.register_autograd('cspn_b200::gwc_volume', backward_gwc, setup_context=setup_gwc)
 
+    @lib.register_fake('cspn_b200::affinity_pool2d')
+    def _(feat, gate, kernel_sizes):
+        torch._check(feat.dim() == 4 and gate.dim() == 4 and 1 <= len(kernel_sizes) <= 8 and gate.shape[1] == len(kernel_sizes),
+                     lambda: 'feat must be (B,C,H,W), gate (B,L,H,W) and kernel_sizes L <= 8 ints')
+        B, C, H, W = feat.shape
+        torch._check(all(1 <= p <= min(H, W) for p in kernel_sizes), lambda: 'kernel sizes must be in [1, min(H, W)]')
+        return feat.new_empty((B * C * sum((H // p) * (W // p) for p in kernel_sizes),))
+
+    @lib.register_fake('cspn_b200::affinity_pool2d_backward')
+    def _(feat, gate, out, grad_out, kernel_sizes):
+        torch._check(feat.dim() == 4 and gate.dim() == 4 and out.dim() == 1 and grad_out.shape == out.shape,
+                     lambda: 'feat and gate must be 4D, out and grad_out the packed levels')
+        return feat.new_empty(feat.shape), gate.new_empty(gate.shape)
+
+    def setup_pool(ctx, inputs, output):
+        feat, gate, kernel_sizes = inputs
+        ctx.kernel_sizes = kernel_sizes
+        ctx.save_for_backward(feat, gate, output)
+
+    def backward_pool(ctx, grad_out):
+        feat, gate, out = ctx.saved_tensors
+        gf, gg = torch.ops.cspn_b200.affinity_pool2d_backward(feat, gate, out, grad_out.contiguous(), ctx.kernel_sizes)
+        return gf, gg, None
+
+    lib.register_autograd('cspn_b200::affinity_pool2d', backward_pool, setup_context=setup_pool)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

@@ -450,6 +450,29 @@ CSPN_API int cspn_gwc_volume_fwd_f32(const float* left, const float* right, floa
 CSPN_API int cspn_gwc_volume_bwd_f32(const float* left, const float* right, const float* grad_out, float* grad_left,
                                   float* grad_right, int B, int F, int H, int W, int D, int G, cspn_stream_t stream);
 
+/* ---- affinity pooling: the CSPN stereo network's convolutional spatial pyramid pooling --------------------------------
+ * feat [B][C][H][W]; gate [B][L][H][W], channel l the raw affinity of level l, shared by all C channels; kernel_sizes a HOST
+ * array of L ints, 1 <= L <= 8, each 1 <= p_l <= min(H, W), in any order, repeats allowed.  Level l pools the windows of
+ * avg_pool2d(x, p_l) (stride p_l, no padding, floor mode) into [B][C][H/p_l][W/p_l]:
+ *   a = |gate_l|,  S = sum_window a,  w = a / S,  out_l[b][c][i][j] = sum_window w * feat[b][c]
+ * out and grad_out are one buffer, level-major: level l starts at B*C*sum_{l'<l} (H/p_l')*(W/p_l').  The order: each window
+ * row summed in ascending x, then the row sums in ascending y (S and out alike); backward
+ *   grad_feat[c][q] = sum over the levels that cover q, ascending l, of w_l(q) * grad_out_l[c][cell], +0.0 if none covers q
+ *   grad_gate_l[q]  = ((sum_c grad_out_l[c][cell] * (feat[c][q] - out_l[c][cell]), ascending c) / S) * sgn(gate_l[q]),
+ *                     +0.0 outside level l's windows
+ * every operation rounded on its own, every sum from its first term (DESIGN.md section 4.17).  An all-zero window gives
+ * NaN (0/0) in every channel of its cell.  No atomics, no workspace, every output element written once; the bits depend on
+ * the arguments only.  CSPN_ERR_INVALID_ARGUMENT for a null or not 4-byte aligned pointer, a size < 1, L outside [1, 8],
+ * a null kernel_sizes or a p_l outside [1, min(H, W)], and an output that overlaps an input or the other output.
+ * CSPN_ERR_UNSUPPORTED for H*W >= 2^31 and a grid past 2^31 - 1 blocks.  One launch each.  No allocation, no
+ * synchronisation. */
+CSPN_API int cspn_affinity_pool2d_fwd_f32(const float* feat, const float* gate, float* out, int B, int C, int H, int W,
+                                  int L, const int* kernel_sizes, cspn_stream_t stream);
+
+CSPN_API int cspn_affinity_pool2d_bwd_f32(const float* feat, const float* gate, const float* out, const float* grad_out,
+                                  float* grad_feat, float* grad_gate, int B, int C, int H, int W, int L,
+                                  const int* kernel_sizes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
