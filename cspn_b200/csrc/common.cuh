@@ -80,18 +80,14 @@ int cluster2d_plan_json(int H, int W, int iters, int chained, char* buf, int len
 int cluster2d_forward_steps(const Problem2D& p, float* steps, cudaStream_t stream, int* launches);
 int cluster2d_adjoint_steps(const Problem2D& p, const float* grad_out, float* lam, cudaStream_t stream, int* launches);
 
-void launch_prep2d(const float* guidance, const float* sparse, float* wk, int B, int H, int W, int gch, int norm_abs,
-                   cudaStream_t stream);
-void launch_step2d(const float* wk, const float* d0, const float* cur, float* dst, int B, int C, int H, int W,
-                   cudaStream_t stream);
-
 // Keep-sparse prep of the K x K and 3x3 launch-per-step paths (cspn2d_wide.cu): the K*K planes of prep2d_kernel /
 // prepk_kernel with m = 1[sparse > 0] (w'_k, kappa), and d0 [B][C][H][W] = (1-m) blur + m sparse, the value the constant
 // term kappa * d0 of the unchanged step kernels multiplies
 void launch_prep_keep(int K, const float* guidance, const float* sparse, const float* blur, float* wk, float* d0, int B, int C,
                       int H, int W, int gch, int norm_abs, cudaStream_t stream);
 
-// keep: as for generic2d_workspace_bytes.  grad_sparse: [B][1][H][W], written in keep mode only (may be null)
+// The 3x3 backward: the cluster formulation, else the K x K one at K = 3 (cspn2d_bwd.cu).  keep: as for
+// generic2d_workspace_bytes.  grad_sparse: [B][1][H][W], written in keep mode only (may be null)
 size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep = false);
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws,
           size_t ws_bytes, cudaStream_t stream, int* launches, float* grad_sparse = nullptr);
@@ -134,7 +130,7 @@ __device__ __forceinline__ void fan_store(const Fan& fan, size_t o, float v) {
 // The operator families of the wide kernels (cspn2d_wide.cu, cspn3d_wide.cu)
 enum class Family {
     Normalised,   // weights gathered from the neighbours' guidance and normalised; 2D K in {5, 7}, 3D K = 5 with `mode`
-                  // (3D backward: K in {3, 5})
+                  // (2D and 3D backward: K = 3 too)
     Paddle,       // 2D 'paddle' own-location norm, K in {3, 5, 7} (in 3D it is mode 2 of Normalised)
     Gates,        // caller-supplied gates used as given; 2D K in {3, 5, 7}, 3D K in {3, 5}
 };

@@ -19,8 +19,8 @@
 //    mode runs the transposed stencil register-resident and writes every lambda_t, and one gather kernel forms
 //    Gw_k(p) = sum_t lambda_{t+1}(p) d_t(p + off_k), Gc = sum_t lambda_{t+1} straight into the finalize arithmetic:
 //    no Gw planes in memory, 2 N planes of workspace.
-//  * launch-per-step (W % 4 != 0, misaligned tensors, or CSPN_B200_BWD=steps): generic prep + N-1 forward steps, N adjoint
-//    steps that also read-modify-write the 8 planes of Gw, finalize.
+//  * launch-per-step (W % 4 != 0, misaligned tensors, or CSPN_B200_BWD=steps): the K x K backward of cspn2d_wide.cu at
+//    K = 3 -- prep, N-1 forward steps, N adjoint steps, and its gather kernel, which forms Gw / Gc as above.
 #include <cstdlib>
 #include <cstring>
 
@@ -30,124 +30,10 @@ namespace cspn {
 
 namespace {
 
-// one backward step: reads lambda_{t+1} (lam_in), d_t; writes lambda_t (lam_out); accumulates Gw, Gc
-__global__ void __launch_bounds__(256)
-bwd_step_kernel(const float* __restrict__ wk, const float* __restrict__ d_t, const float* __restrict__ lam_in,
-                float* __restrict__ lam_out, float* __restrict__ Gw, float* __restrict__ Gc, int C, int H, int W,
-                int first) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    const int b = blockIdx.z;
-    if (x >= W || y >= H) return;
-    const size_t HW = (size_t)H * W, p = (size_t)y * W + x;
-    const float* w = wk + (size_t)b * 9 * HW;
-    float gw[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) gw[k] = first ? 0.f : Gw[((size_t)b * 8 + k) * HW + p];
-    for (int c = 0; c < C; ++c) {
-        const size_t plane = ((size_t)b * C + c) * HW;
-        const float* li = lam_in + plane;
-        const float* dt = d_t + plane;
-        const float lp = __ldg(li + p);
-        float acc = 0.f;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            // destination pixel (y - dy, x - dx) reads this pixel with tap k
-            const int ys = y - off2_dy(k), xs = x - off2_dx(k);
-            if (ys >= 0 && ys < H && xs >= 0 && xs < W) {
-                const size_t ps = (size_t)ys * W + xs;
-                acc = fmaf(__ldg(w + k * HW + ps), __ldg(li + ps), acc);
-            }
-            const int yn = y + off2_dy(k), xn = x + off2_dx(k);
-            if (yn >= 0 && yn < H && xn >= 0 && xn < W) gw[k] = fmaf(lp, __ldg(dt + (size_t)yn * W + xn), gw[k]);
-        }
-        lam_out[plane + p] = acc;
-        Gc[plane + p] = (first ? 0.f : Gc[plane + p]) + lp;
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) Gw[((size_t)b * 8 + k) * HW + p] = gw[k];
-}
-
-// KEEP (keep-sparse mode, sparse non-null): m = 1[sparse > 0], grad_blur's coefficient is (1-m)(1-s) = kappa - m, and
-// grad_sparse (may be null) receives m * sum_c Gc_c, the channels summed in order
-template <bool KEEP>
-__device__ __forceinline__ void bwd_finalize_body(const float* __restrict__ guidance, const float* __restrict__ blur,
-                                                  const float* __restrict__ sparse, const float* __restrict__ wk,
-                                                  const float* __restrict__ Gw, const float* __restrict__ Gc,
-                                                  const float* __restrict__ lam0, float* __restrict__ grad_guidance,
-                                                  float* __restrict__ grad_blur, float* __restrict__ grad_sparse, int C, int H, int W,
-                                                  int gch, int norm_abs) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y;
-    const int b = blockIdx.z;
-    if (x >= W || y >= H) return;
-    const size_t HW = (size_t)H * W, p = (size_t)y * W + x;
-    const float kappa = __ldg(wk + ((size_t)b * 9 + 8) * HW + p);
-    [[maybe_unused]] float m_keep = 0.f, gsum = 0.f;
-    if constexpr (KEEP) m_keep = __ldg(sparse + (size_t)b * HW + p) > 0.f ? 1.f : 0.f;
-    const float cblur = KEEP ? kappa - m_keep : kappa;
-    float gkappa = 0.f;
-    for (int c = 0; c < C; ++c) {
-        const size_t plane = ((size_t)b * C + c) * HW;
-        const float gc = __ldg(Gc + plane + p);
-        gkappa = fmaf(gc, __ldg(blur + plane + p), gkappa);
-        if (grad_blur) grad_blur[plane + p] = fmaf(cblur, gc, __ldg(lam0 + plane + p));
-        if constexpr (KEEP) gsum += gc;
-    }
-    if constexpr (KEEP)
-        if (grad_sparse) grad_sparse[(size_t)b * HW + p] = m_keep * gsum;
-    if (!grad_guidance) return;
-    const float* g = guidance + (size_t)b * gch * HW;
-    float a[8], sg[8], S = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int yy = y + off2_dy(k), xx = x + off2_dx(k);
-        float v = 0.f;
-        sg[k] = 1.f;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-            v = __ldg(g + k * HW + (size_t)yy * W + xx);
-            if (norm_abs) { sg[k] = signf(v); v = fabsf(v); }   // d|g|/dg = sign(g) (0 at 0, like torch.abs)
-        }
-        a[k] = v;
-        S += fabsf(v);
-    }
-    const float m = KEEP ? m_keep : sparse ? signf(__ldg(sparse + (size_t)b * HW + p)) : 0.f;
-    const float om = 1.f - m;
-    float Hk[8], T = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        Hk[k] = om * (__ldg(Gw + ((size_t)b * 8 + k) * HW + p) - gkappa);
-        T = fmaf(Hk[k], __fdiv_rn(a[k], S), T);
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int yy = y + off2_dy(k), xx = x + off2_dx(k);
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-            const float ga = __fdiv_rn(Hk[k] - signf(a[k]) * T, S);
-            grad_guidance[((size_t)b * gch + k) * HW + (size_t)yy * W + xx] = ga * sg[k];
-        }
-    }
-}
-
-__global__ void __launch_bounds__(256)
-bwd_finalize_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
-                    const float* __restrict__ wk, const float* __restrict__ Gw, const float* __restrict__ Gc,
-                    const float* __restrict__ lam0, float* __restrict__ grad_guidance, float* __restrict__ grad_blur, int C,
-                    int H, int W, int gch, int norm_abs) {
-    bwd_finalize_body<false>(guidance, blur, sparse, wk, Gw, Gc, lam0, grad_guidance, grad_blur, nullptr, C, H, W, gch, norm_abs);
-}
-
-__global__ void __launch_bounds__(256)
-bwd_finalize_keep_kernel(const float* __restrict__ guidance, const float* __restrict__ blur, const float* __restrict__ sparse,
-                         const float* __restrict__ wk, const float* __restrict__ Gw, const float* __restrict__ Gc,
-                         const float* __restrict__ lam0, float* __restrict__ grad_guidance, float* __restrict__ grad_blur,
-                         float* __restrict__ grad_sparse, int C, int H, int W, int gch, int norm_abs) {
-    bwd_finalize_body<true>(guidance, blur, sparse, wk, Gw, Gc, lam0, grad_guidance, grad_blur, grad_sparse, C, H, W, gch, norm_abs);
-}
-
-// Staged cluster formulation, last stage: Gw / Gc gathered over all steps in registers, then the finalize arithmetic
-// of bwd_finalize_kernel.  steps[t] = d_{t+1}, lam[t] = lambda_t (planes of n = B*C*H*W floats), lambda_N = grad_out.
-// KEEP: as in bwd_finalize_body, with grad_blur's coefficient (1-m)(1 - sum_k w_k) formed from the quotients
+// Staged cluster formulation, last stage: Gw / Gc gathered over all steps in registers, then the chain rule of the file
+// header.  steps[t] = d_{t+1}, lam[t] = lambda_t (planes of n = B*C*H*W floats), lambda_N = grad_out.
+// KEEP (keep-sparse mode, sparse non-null): m = 1[sparse > 0], grad_blur's coefficient is (1-m)(1 - sum_k w_k), formed
+// from the quotients, and grad_sparse (may be null) receives m * sum_c Gc_c, the channels summed in order
 template <bool KEEP>
 __device__ __forceinline__ void bwd_gather_finalize_body(const float* __restrict__ guidance, const float* __restrict__ blur,
                                                          const float* __restrict__ sparse, const float* __restrict__ steps,
@@ -251,23 +137,21 @@ bool cluster_backward_enabled() {
 
 }  // namespace
 
+// The launch-per-step formulation's workspace, which covers the cluster's 2 N planes (d_1..d_N, lambda_0..lambda_{N-1})
 size_t bwd2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep) {
-    if (iters <= 0) return 0;
-    const size_t HW = (size_t)H * W, n = (size_t)B * C * HW;
-    // wk (9 planes/image) + d_1..d_{N-1} + lambda ping-pong + Gw + Gc (+ d0' in the keep-sparse mode)
-    const size_t per_step = sizeof(float) * ((size_t)B * 9 * HW + (size_t)(iters - 1) * n + 2 * n + (size_t)B * 8 * HW + n +
-                                             (keep ? n : 0));
-    const size_t cluster = cluster_backward_enabled() ? sizeof(float) * 2 * (size_t)iters * n : 0;   // d_1..d_N, lambda_0..lambda_{N-1}
-    return per_step > cluster ? per_step : cluster;
+    return widek_bwd_workspace_bytes(B, C, H, W, 3, iters, Family::Normalised, keep);
 }
 
-// Cluster formulation (see the file header).  Returns CSPN_ERR_UNSUPPORTED when the shape / alignment is not
-// the cluster kernel's; the caller then falls back to the launch-per-step path.
+// Cluster formulation (see the file header).  Returns CSPN_ERR_UNSUPPORTED, having enqueued nothing, when the shape /
+// alignment is not the cluster kernel's; the caller then falls back to the launch-per-step path.
 static int bwd2d_cluster(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, float* grad_sparse,
                          void* ws, cudaStream_t stream, int* launches) {
     char why[200] = "";
     if ((reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(ws)) & 15) return CSPN_ERR_UNSUPPORTED;
     if (!cluster2d_supported(p, why, sizeof(why))) return CSPN_ERR_UNSUPPORTED;
+    // the gather writes the guidance gradient of taps inside the image and channels < 8 only
+    if (grad_guidance)
+        CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * p.H * p.W * sizeof(float), stream));
     const long long n = (long long)p.B * p.C * p.H * p.W;
     float* steps = static_cast<float*>(ws);            // steps[t] = d_{t+1}
     float* lam = steps + (size_t)p.iters * n;          // lam[t]   = lambda_t
@@ -291,62 +175,14 @@ static int bwd2d_cluster(const Problem2D& p, const float* grad_out, float* grad_
 
 int bwd2d(const Problem2D& p, const float* grad_out, float* grad_guidance, float* grad_blur, void* ws, size_t ws_bytes,
           cudaStream_t stream, int* launches, float* grad_sparse) {
-    const size_t HW = (size_t)p.H * p.W, n = (size_t)p.B * p.C * HW;
-    if (grad_guidance)
-        CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * HW * sizeof(float), stream));
-    if (p.iters == 0) {
-        if (grad_blur) CSPN_CUDA_TRY(cudaMemcpyAsync(grad_blur, grad_out, n * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-        return CSPN_OK;
-    }
-    const size_t need = bwd2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters, p.keep);
-    if (!ws || ws_bytes < need) {
-        set_error("2D backward needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
-        return CSPN_ERR_WORKSPACE;
-    }
-    if (p.B > 65535 || (long)p.B * p.C > 65535) { set_error("backward: B*C exceeds gridDim.z"); return CSPN_ERR_UNSUPPORTED; }
-    if (cluster_backward_enabled()) {
+    // a workspace or grid the fallback would refuse is refused by it, with its message, on either route
+    if (p.iters > 0 && cluster_backward_enabled() && ws && ws_bytes >= bwd2d_workspace_bytes(p.B, p.C, p.H, p.W, p.iters, p.keep) &&
+        (long long)p.B * p.C <= 65535) {
         const int rc = bwd2d_cluster(p, grad_out, grad_guidance, grad_blur, grad_sparse, ws, stream, launches);
         if (rc != CSPN_ERR_UNSUPPORTED) return rc;
         clear_error();   // shape / alignment outside the cluster kernel's: the launch-per-step path below handles it
     }
-    float* wk = static_cast<float*>(ws);
-    float* D = wk + (size_t)p.B * 9 * HW;             // d_1 .. d_{N-1}
-    float* lam[2] = {D + (size_t)(p.iters - 1) * n, D + (size_t)(p.iters - 1) * n + n};
-    float* Gw = lam[1] + n;
-    float* Gc = Gw + (size_t)p.B * 8 * HW;
-
-    // keep-sparse mode: the constant term of the forward steps reads d0' = (1-m) blur + m sparse (after Gc)
-    const float* d0 = p.blur;
-    if (p.keep) {
-        launch_prep_keep(3, p.guidance, p.sparse, p.blur, wk, Gc + n, p.B, p.C, p.H, p.W, p.gch, p.norm_abs, stream);
-        d0 = Gc + n;
-    } else {
-        launch_prep2d(p.guidance, p.sparse, wk, p.B, p.H, p.W, p.gch, p.norm_abs, stream);
-    }
-    ++*launches;
-    for (int t = 0; t + 1 < p.iters; ++t) {           // d_{t+1} = step(d_t)
-        launch_step2d(wk, d0, t == 0 ? p.blur : D + (size_t)(t - 1) * n, D + (size_t)t * n, p.B, p.C, p.H, p.W, stream);
-        ++*launches;
-    }
-    const dim3 block(32, 8);
-    const dim3 grid((p.W + 31) / 32, (p.H + 7) / 8, p.B);
-    const float* lam_in = grad_out;
-    for (int t = p.iters - 1; t >= 0; --t) {
-        float* lam_out = lam[t & 1];
-        const float* d_t = (t == 0) ? p.blur : D + (size_t)(t - 1) * n;
-        bwd_step_kernel<<<grid, block, 0, stream>>>(wk, d_t, lam_in, lam_out, Gw, Gc, p.C, p.H, p.W, t == p.iters - 1);
-        ++*launches;
-        lam_in = lam_out;
-    }
-    if (p.keep)
-        bwd_finalize_keep_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, wk, Gw, Gc, lam_in, grad_guidance,
-                                                             grad_blur, grad_sparse, p.C, p.H, p.W, p.gch, p.norm_abs);
-    else
-        bwd_finalize_kernel<<<grid, block, 0, stream>>>(p.guidance, p.blur, p.sparse, wk, Gw, Gc, lam_in, grad_guidance, grad_blur,
-                                                        p.C, p.H, p.W, p.gch, p.norm_abs);
-    ++*launches;
-    CSPN_CUDA_TRY(cudaGetLastError());
-    return CSPN_OK;
+    return widek_backward(p, 3, Family::Normalised, grad_out, grad_guidance, grad_blur, ws, ws_bytes, stream, launches, grad_sparse);
 }
 
 }  // namespace cspn

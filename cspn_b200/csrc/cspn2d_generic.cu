@@ -1,7 +1,8 @@
-// Generic 2D CSPN path: one "prep" launch (affinity normalisation + mask folding) and one
+// Generic 2D CSPN forward: one "prep" launch (affinity normalisation + mask folding) and one
 // 9-point stencil launch per iteration.  Handles every shape (odd W, huge H, prop_time of any
-// size); it is the fallback of the cluster kernel (cspn2d_cluster.cu) and the simplest
-// statement of the arithmetic on the GPU.
+// size); it is the forward fallback of the cluster kernel (cspn2d_cluster.cu) and the simplest
+// statement of the arithmetic on the GPU.  The fallback backward is the K x K one of cspn2d_wide.cu
+// at K = 3 (cspn2d_bwd.cu): the 3x3 step there measured slower on odd widths (DESIGN.md section 4.8).
 //
 // Arithmetic (SURVEY.md Appendix A; reference /root/reference/cspn_pytorch/models/cspn.py):
 //   a_k(p) = g_k(p + off_k) (0 outside the image)             cspn.py:105-132
@@ -74,18 +75,6 @@ step2d_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const 
 }
 
 }  // namespace
-
-// launchers shared with the backward pass (cspn2d_bwd.cu)
-void launch_prep2d(const float* guidance, const float* sparse, float* wk, int B, int H, int W, int gch, int norm_abs,
-                   cudaStream_t stream) {
-    const dim3 block(32, 8);
-    prep2d_kernel<<<dim3((W + 31) / 32, (H + 7) / 8, B), block, 0, stream>>>(guidance, sparse, wk, H, W, gch, norm_abs);
-}
-void launch_step2d(const float* wk, const float* d0, const float* cur, float* dst, int B, int C, int H, int W,
-                   cudaStream_t stream) {
-    const dim3 block(32, 8);
-    step2d_kernel<<<dim3((W + 31) / 32, (H + 7) / 8, B * C), block, 0, stream>>>(wk, d0, cur, dst, C, H, W);
-}
 
 // keep: the d0' planes of the keep-sparse mode follow the ping-pong buffer
 size_t generic2d_workspace_bytes(int B, int C, int H, int W, int iters, bool keep) {

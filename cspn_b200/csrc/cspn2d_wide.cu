@@ -1,6 +1,6 @@
 // 2D CSPN with a K x K affinity kernel, K = 2R+1 in {5, 7} (K*K-1 = 24 / 48 neighbours), forward and backward.
-// The 3x3 operator keeps its own kernels (cspn2d_cluster.cu, cspn2d_generic.cu, cspn2d_bwd.cu); K = 3 is delegated to
-// them by the C ABI.
+// The 3x3 operator keeps its own forward kernels (cspn2d_cluster.cu, cspn2d_generic.cu) and its cluster backward
+// (cspn2d_bwd.cu); its fallback backward is the one here at K = 3, whose taps are off2_dy / off2_dx in the same order.
 //
 // Arithmetic: cspn2d_generic.cu with K*K-1 taps.  Tap k enumerates (t, l) over [0,K)^2 in raster order without the
 // centre (R, R) and reads the source at (dy, dx) = (R-t, R-l) (oracle/cspn_numpy_k.py::offsets_2d):
@@ -24,8 +24,8 @@
 //   w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location,   d_{t+1} = sum_k w_k d_t(p + off_k)
 // with no centre term and no sparse replacement.  Its prep (prepk_paddle_kernel) writes w_k and a zero kappa plane; the
 // step kernels' PADDLE flag drops the kappa d0 term and the d0 load; the adjoint step is shared as it is; the gather's
-// PADDLE flag applies the own-location chain rule (grad_g_j at p, grad_feat = lambda_0).  K = 3 runs here too: the
-// cluster kernel keeps the folded 3x3 form only.
+// PADDLE flag applies the own-location chain rule (grad_g_j at p, grad_feat = lambda_0).  K = 3 runs here on every
+// route: the cluster kernel keeps the folded 3x3 form only.
 //
 // Caller-supplied gates (fluid.layers.affinity_propagate itself, DESIGN.md section 4.11), K in {3, 5, 7}:
 //   d_{t+1}(p) = sum_k g_k(p) d_t(p + off_k)   with the gates used as given (no |.|, no normalisation, no centre term).
@@ -564,17 +564,16 @@ const FamilyTraits& traits(Family family) {
     return t[(int)family];
 }
 
-// f(R, PADDLE, RAW) as integral constants for the K x K kernels of `family`.  The normalised family has no R = 1 kernels:
-// its K = 3 is the 3x3 operator, which the C ABI never sends here.
+// f(R, PADDLE, RAW) as integral constants for the K x K kernels of `family`.  The normalised family's K = 3 is the 3x3
+// operator, whose backward falls back to these kernels (cspn2d_bwd.cu); its forward is never sent here.
 template <class F>
 int with_kernels(int K, Family family, F&& f) {
     using std::integral_constant;
     constexpr std::true_type yes{};
     constexpr std::false_type no{};
     const auto radius = [&](auto paddle, auto raw) {
-        if constexpr (paddle)
-            if (K == 3) return f(integral_constant<int, 1>{}, paddle, raw);
-        return K == 5 ? f(integral_constant<int, 2>{}, paddle, raw) : f(integral_constant<int, 3>{}, paddle, raw);
+        return K == 3 ? f(integral_constant<int, 1>{}, paddle, raw)
+             : K == 5 ? f(integral_constant<int, 2>{}, paddle, raw) : f(integral_constant<int, 3>{}, paddle, raw);
     };
     return family == Family::Normalised ? radius(no, no) : family == Family::Paddle ? radius(yes, no) : radius(yes, yes);
 }

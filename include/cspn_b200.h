@@ -109,7 +109,8 @@ CSPN_API int cspn2d_fwd_gather_f32(const float* guidance, const float* blur, con
 
 /* ---- 2D backward (adjoint of the above; reference: autograd through cspn.py:42-83, used by
  * train.py:198).  grad_guidance [B][guidance_channels][H][W] (channels >= 8 are zero-filled),
- * grad_blur [B][C][H][W].  Either may be NULL.  Needs the forward inputs again. */
+ * grad_blur [B][C][H][W].  Either may be NULL.  Needs the forward inputs again.  Workspace: 9*B*H*W + 2*iters*B*C*H*W
+ * floats (0 for iters == 0), on the cluster route and off it alike. */
 CSPN_API size_t cspn2d_bwd_workspace_bytes(int B, int C, int H, int W, int iters);
 
 CSPN_API int cspn2d_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* grad_out,
@@ -123,9 +124,9 @@ CSPN_API int cspn2d_bwd_f32(const float* guidance, const float* blur, const floa
  * guidance [B][guidance_channels >= K*K-1][H][W] (channels 0..K*K-2 used, shared across the C channels of blur);
  * blur / sparse / out / grad_* and norm_type (cspn_norm2d: 0 signed, 1 abs) as in the 3x3 calls above.
  * K = 3 IS the 3x3 operator: the calls delegate to cspn2d_fwd_f32 (CSPN_ALGO_AUTO) / cspn2d_bwd_f32 and the workspace
- * queries return theirs.  K = 5 / 7: forward workspace B*K*K*H*W + B*C*H*W floats, backward B*K*K*H*W + 2*iters*B*C*H*W
- * floats (0 for iters == 0); the size does not depend on the device.  CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5, 7},
- * guidance_channels < K*K-1, an unknown norm, iters < 0, a non-positive shape or a null guidance / blur / out
+ * queries return theirs.  Forward workspace B*K*K*H*W + B*C*H*W floats at K = 5 / 7, backward B*K*K*H*W +
+ * 2*iters*B*C*H*W floats at every K (0 for iters == 0); the size does not depend on the device.
+ * CSPN_ERR_INVALID_ARGUMENT for K not in {3, 5, 7}, guidance_channels < K*K-1, an unknown norm, iters < 0, a non-positive shape or a null guidance / blur / out
  * (grad_out in the backward; grad_guidance and grad_blur may be NULL). */
 CSPN_API size_t cspn2d_k_workspace_bytes(int B, int C, int H, int W, int K, int iters);
 
@@ -168,8 +169,8 @@ CSPN_API int cspn2d_k_fwd_gather_f32(const float* guidance, const float* blur, c
  * [B][1][H][W] is shared by the C channels of blur; a NULL sparse gives the default mode's bits (the K x K and 3x3 calls
  * above).  Arguments, shapes and status codes as in cspn2d_k_fwd_f32 / cspn2d_k_bwd_f32; `algo` (cspn_algo) chooses the
  * 3x3 path as in cspn2d_fwd_f32 and is ignored for K = 5 / 7, where the CSPN_B200_FORCE_* hooks do not apply either.
- * Workspace: K = 3 cluster plans as cspn2d_workspace_bytes; the launch-per-step paths (3x3 generic, K = 5 / 7) one
- * B*C*H*W plane more than the default mode's (d0' = (1 - m) blur + m sparse).  CSPN_ALGO_AUTO reports
+ * Workspace: K = 3 cluster plans as cspn2d_workspace_bytes; the launch-per-step paths (3x3 generic, K = 5 / 7) and every
+ * backward one B*C*H*W plane more than the default mode's (d0' = (1 - m) blur + m sparse).  CSPN_ALGO_AUTO reports
  * CSPN_ERR_WORKSPACE as cspn2d_fwd_f32 does when a problem it sized for the cluster kernel falls back to the generic path.
  * The gather entry takes peer_out / n_peer / multicast_out after `out` as cspn2d_k_fwd_gather_f32 does (K = 3 on the
  * cluster kernel's epilogue, CSPN_ERR_UNSUPPORTED for a shape it cannot take; K = 5 / 7 on the last step).

@@ -116,7 +116,7 @@ def test_c_abi_rejects_bad_arguments():
     assert b'null' in L.cspn_last_error()
 
 
-def test_workspace_formulas():
+def test_workspace_formulas(monkeypatch):
     L = _lib.lib()
     B, C, H, W = 3, 2, 10, 15
     HW = H * W
@@ -128,6 +128,12 @@ def test_workspace_formulas():
     for n in (0, 1, 24):      # K = 3 is the 3x3 operator: its queries are theirs
         assert L.cspn2d_k_workspace_bytes(B, C, H, W, 3, n) == L.cspn2d_workspace_bytes(B, C, H, W, n, _lib.ALGO_AUTO)
         assert L.cspn2d_k_bwd_workspace_bytes(B, C, H, W, 3, n) == L.cspn2d_bwd_workspace_bytes(B, C, H, W, n)
+    for n in (1, 2, 24):      # the 3x3 backward's fallback is the K x K one at K = 3, whose size covers the cluster route's
+        assert L.cspn2d_bwd_workspace_bytes(B, C, H, W, n) == 4 * (B * 9 * HW + 2 * n * B * C * HW)
+        assert L.cspn2d_keep_bwd_workspace_bytes(B, C, H, W, 3, n) == 4 * (B * 9 * HW + (2 * n + 1) * B * C * HW)
+        monkeypatch.setenv('CSPN_B200_BWD', 'steps')     # the 3x3 backward's size does not depend on its route
+        assert L.cspn2d_bwd_workspace_bytes(B, C, H, W, n) == 4 * (B * 9 * HW + 2 * n * B * C * HW)
+        monkeypatch.delenv('CSPN_B200_BWD')
     assert L.cspn2d_k_workspace_bytes(B, C, H, W, 4, 3) == 0 and L.cspn2d_k_bwd_workspace_bytes(B, C, H, W, 9, 3) == 0
 
 
