@@ -1325,3 +1325,115 @@ def affinity_pool2d(feat, gate, kernel_sizes):
     B, C, H, W = feat.shape
     shapes = [(B, C, H // p, W // p) for p in ks]
     return tuple(v.view(s) for v, s in zip(flat.split([B * C * h * w for _, _, h, w in shapes]), shapes))
+
+
+# ---- affinity fusion: the CSPN stereo network's spatial pyramid fusion ----------------------------------------------------------
+def _check_affinity_fuse(levels, gate, align_corners, align_mode):
+    """The checks of affinity_fuse2d; every refusal comes before anything is allocated or narrowed to int.  Returns the
+    levels as a tuple."""
+    if isinstance(levels, torch.Tensor) or not isinstance(levels, (list, tuple)):
+        raise ValueError(f'levels must be a list or tuple of tensors, got {type(levels).__name__}')
+    lv = tuple(levels)
+    if not 1 <= len(lv) <= 8:
+        raise ValueError(f'levels must hold 1 to 8 tensors, got {len(lv)}')
+    if not all(isinstance(x, torch.Tensor) for x in lv) or not isinstance(gate, torch.Tensor):
+        raise ValueError('levels and gate must be tensors')
+    if gate.dim() != 4 or any(x.dim() != 4 for x in lv):
+        raise ValueError(f'levels must be (B,C,h,w) and gate (B,L,H,W), got {[tuple(x.shape) for x in lv]} and '
+                         f'{tuple(gate.shape)}')
+    B, L, H, W = gate.shape
+    C = lv[0].shape[1]
+    if L != len(lv) or any(tuple(x.shape[:2]) != (B, C) for x in lv):
+        raise ValueError(f'gate (B, L, H, W) and the L levels (B, C, h, w) must agree, got gate {tuple(gate.shape)} and levels '
+                         f'{[tuple(x.shape) for x in lv]}')
+    if min(B, C, H, W) < 1 or any(min(x.shape[2:]) < 1 for x in lv):
+        raise ValueError(f'levels and gate must not be empty, got {[tuple(x.shape) for x in lv]} and {tuple(gate.shape)}')
+    if isinstance(align_mode, bool) or align_mode not in (0, 1):
+        raise ValueError(f'align_mode must be 0 or 1, got {align_mode!r}')
+    if gate.dtype != torch.float32 or any(x.dtype != torch.float32 for x in lv):
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if any(x.device != gate.device for x in lv):
+        raise RuntimeError('the levels and gate are on different devices')
+    if B > 2 ** 31 - 1 or C > 2 ** 31 - 1 or H * W >= 2 ** 31 or any(x.shape[2] * x.shape[3] >= 2 ** 31 for x in lv):
+        raise _lib.CspnError(f'affinity_fuse2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got levels '
+                             f'{[tuple(x.shape) for x in lv]} and gate {tuple(gate.shape)}')
+    if not gate.is_cuda:
+        raise _lib.CspnError('affinity_fuse2d takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return lv
+
+
+def _level_args(levels):
+    """The C ABI's host arrays: the level pointers and (h_0, w_0, h_1, w_1, ...)."""
+    hw = [n for x in levels for n in x.shape[2:]]
+    return (ctypes.c_void_p * len(levels))(*[x.data_ptr() for x in levels]), (ctypes.c_int * len(hw))(*hw)
+
+
+def _fuse_fwd(levels, gate, align_corners, align_mode):
+    """Forward only (no autograd) through cspn_affinity_fuse2d_fwd_f32, on the current stream."""
+    xs, g = [x.contiguous() for x in levels], gate.contiguous()
+    B, L, H, W = g.shape
+    out = g.new_empty((B, xs[0].shape[1], H, W))
+    ptrs, hw = _level_args(xs)
+    with torch.cuda.device(g.device):
+        rc = _lib.lib().cspn_affinity_fuse2d_fwd_f32(ptrs, hw, _ptr(g), _ptr(out), B, xs[0].shape[1], H, W, L, int(align_corners),
+                                                      align_mode, _stream(g.device))
+    _lib.check(rc, 'cspn_affinity_fuse2d_fwd_f32')
+    return out
+
+
+def _fuse_bwd(levels, gate, out, grad_out, align_corners, align_mode):
+    """grad_levels (a list, one per level), grad_gate through cspn_affinity_fuse2d_bwd_f32."""
+    xs, g, o, go = [x.contiguous() for x in levels], gate.contiguous(), out.contiguous(), grad_out.contiguous()
+    B, L, H, W = g.shape
+    C = xs[0].shape[1]
+    gl, gg = [torch.empty_like(x) for x in xs], torch.empty_like(g)
+    ptrs, hw = _level_args(xs)
+    gptrs, _ = _level_args(gl)
+    Lb = _lib.lib()
+    with torch.cuda.device(g.device):
+        ws_bytes = Lb.cspn_affinity_fuse2d_bwd_workspace_bytes(B, C, H, W, L, hw)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=g.device)
+        rc = Lb.cspn_affinity_fuse2d_bwd_f32(ptrs, hw, _ptr(g), _ptr(o), _ptr(go), gptrs, _ptr(gg), B, C, H, W, L,
+                                             int(align_corners), align_mode, _ptr(ws), ws_bytes, _stream(g.device))
+    _lib.check(rc, 'cspn_affinity_fuse2d_bwd_f32')
+    return gl, gg
+
+
+class _AffinityFuseFn(torch.autograd.Function):
+    """autograd seam of affinity_fuse2d without the torch-op shim: the levels, gate and out are saved.  A level passed twice
+    gets the sum of its gradients from autograd."""
+
+    @staticmethod
+    def forward(ctx, align_corners, align_mode, gate, *levels):
+        out = _fuse_fwd(levels, gate, align_corners, align_mode)
+        ctx.cfg = (align_corners, align_mode)
+        ctx.save_for_backward(gate, out, *levels)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        gate, out, *levels = ctx.saved_tensors
+        gl, gg = _fuse_bwd(levels, gate, out, grad_out, *ctx.cfg)
+        return None, None, gg, *gl
+
+
+def affinity_fuse2d(levels, gate, align_corners=True, align_mode=1):
+    """The CSPN stereo network's spatial pyramid fusion: one CSPN step across the levels of a feature pyramid, with the
+    upsampling, in one launch.  levels is a list or tuple of L fp32 CUDA tensors (B, C, h_l, w_l), 1 <= L <= 8, of any sizes
+    (a level may repeat, or be finer than the output); gate (B, L, H, W) holds level l's raw affinity in channel l, shared
+    by all C channels, and sets the output size.  At every pixel w_l = |g_l| / sum_l |g_l| and
+    out[:, c] = sum_l w_l * u_l[:, c], where u_l is level l resampled bilinearly to (H, W) with resize_trilinear's rule:
+    align_corners=False, align_mode=0 is F.interpolate(..., mode='bilinear', align_corners=False); align_corners=True is
+    F.interpolate(..., align_corners=True); the default is Paddle's align_corners=True, align_mode=1.  The upsampled levels
+    are never stored.  All-zero gates at a pixel give NaN there.  Returns (B, C, H, W); differentiable in the levels and
+    gate, with a deterministic backward.  DESIGN.md section 4.18."""
+    lv = _check_affinity_fuse(levels, gate, align_corners, align_mode)
+    align_corners = bool(align_corners)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.affinity_fuse2d(list(lv), gate, align_corners, align_mode)
+    if torch.is_grad_enabled() and (gate.requires_grad or any(x.requires_grad for x in lv)):
+        return _AffinityFuseFn.apply(align_corners, align_mode, gate, *lv)
+    return _fuse_fwd(lv, gate, align_corners, align_mode)

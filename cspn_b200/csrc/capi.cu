@@ -926,7 +926,7 @@ static int check_affinity_pool(int B, int C, int H, int W, int L, const int* ks,
 }
 
 // An output may overlap neither an input nor another output; inputs may alias one another
-static int check_disjoint(std::initializer_list<Buf> in, std::initializer_list<Buf> outs) {
+static int check_disjoint(const std::vector<Buf>& in, const std::vector<Buf>& outs) {
     for (const Buf& o : outs) {
         for (const Buf& i : in)
             if (overlap(o.p, o.bytes, i.p, i.bytes)) { set_error("%s overlaps %s", o.name, i.name); return CSPN_ERR_INVALID_ARGUMENT; }
@@ -969,6 +969,104 @@ int cspn_affinity_pool2d_bwd_f32(const float* feat, const float* gate, const flo
     return on_device_of(feat, "feat", [&](int* launches) {
         return affinity_pool_backward(feat, gate, out, grad_out, grad_feat, grad_gate, B, C, H, W, L, kernel_sizes,
                                       (cudaStream_t)stream, launches);
+    });
+}
+
+// ---- affinity fusion (the CSPN stereo network's spatial pyramid fusion) ----------------------------------------------------
+// The sizes, the levels, the flags, the pointers, then the launch limits: `in` are read and `outs` written, and the level
+// pointers join them (grad_levels only in the backward).  On success n_lvl[l] is level l's elements per (B, channel).
+static int check_affinity_fuse(int B, int C, int H, int W, int L, const int* level_hw, int align_corners, int align_mode,
+                               const float* const* levels, float* const* grad_levels, bool backward, long long* n_lvl,
+                               std::vector<Buf> in, std::vector<Buf> outs) {
+    if (!positive(B, C, H, W)) { set_error("non-positive size B=%d C=%d H=%d W=%d", B, C, H, W); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (L < 1 || L > kAffinityFuseMaxLevels) { set_error("the number of levels L=%d must be 1..8", L); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!level_hw) { set_error("null level_hw"); return CSPN_ERR_INVALID_ARGUMENT; }
+    for (int l = 0; l < L; ++l) {
+        if (!positive(level_hw[2 * l], level_hw[2 * l + 1])) {
+            set_error("non-positive size %dx%d of level %d", level_hw[2 * l], level_hw[2 * l + 1], l);
+            return CSPN_ERR_INVALID_ARGUMENT;
+        }
+        n_lvl[l] = (long long)level_hw[2 * l] * level_hw[2 * l + 1];
+    }
+    if (align_corners != 0 && align_corners != 1) { set_error("align_corners must be 0 or 1, got %d", align_corners); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (align_mode != 0 && align_mode != 1) { set_error("align_mode must be 0 or 1, got %d", align_mode); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!levels || (backward && !grad_levels)) { set_error("null level pointer array"); return CSPN_ERR_INVALID_ARGUMENT; }
+    for (int l = 0; l < L; ++l) {
+        in.push_back({levels[l], 0, "levels[]"});
+        if (backward) outs.push_back({grad_levels[l], 0, "grad_levels[]"});
+    }
+    uintptr_t bits = 0;
+    for (const auto* set : {&in, &outs})
+        for (const Buf& b : *set) {
+            if (!b.p) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+            bits |= reinterpret_cast<uintptr_t>(b.p);
+        }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!affinity_fuse_launchable(B, C, H, W, L, level_hw, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+// The level buffers as overlap operands, named levels[l] or grad_levels[l]
+using LevelNames = char[kAffinityFuseMaxLevels][24];
+static void add_levels(std::vector<Buf>& set, const float* const* p, int B, int C, int L, const long long* n_lvl, const char* what,
+                       LevelNames& names) {
+    for (int l = 0; l < L; ++l) {
+        snprintf(names[l], sizeof(names[l]), "%s[%d]", what, l);
+        set.push_back({p[l], span_bytes(B, C, n_lvl[l]), names[l]});
+    }
+}
+
+int cspn_affinity_fuse2d_fwd_f32(const float* const* levels, const int* level_hw, const float* gate, float* out, int B, int C,
+                                 int H, int W, int L, int align_corners, int align_mode, cspn_stream_t stream) {
+    begin_call();
+    long long n_lvl[kAffinityFuseMaxLevels];
+    int rc = check_affinity_fuse(B, C, H, W, L, level_hw, align_corners, align_mode, levels, nullptr, false, n_lvl,
+                                 {{gate, 0, "gate"}}, {{out, 0, "out"}});
+    if (rc != CSPN_OK) return rc;
+    LevelNames names;
+    std::vector<Buf> in{{gate, span_bytes(B, L, (long long)H * W), "gate"}};
+    add_levels(in, levels, B, C, L, n_lvl, "levels", names);
+    rc = check_disjoint(in, {{out, span_bytes(B, C, (long long)H * W), "out"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(gate, "gate", [&](int* launches) {
+        return affinity_fuse_forward(levels, level_hw, gate, out, B, C, H, W, L, align_corners, align_mode, (cudaStream_t)stream,
+                                     launches);
+    });
+}
+
+size_t cspn_affinity_fuse2d_bwd_workspace_bytes(int B, int C, int H, int W, int L, const int* level_hw) {
+    if (!positive(B, C, H, W) || L < 1 || L > kAffinityFuseMaxLevels || !level_hw) return 0;
+    for (int l = 0; l < 2 * L; ++l)
+        if (level_hw[l] < 1) return 0;
+    return affinity_fuse_bwd_workspace_bytes(B, C, H, W, L, level_hw);
+}
+
+int cspn_affinity_fuse2d_bwd_f32(const float* const* levels, const int* level_hw, const float* gate, const float* out,
+                                 const float* grad_out, float* const* grad_levels, float* grad_gate, int B, int C, int H, int W,
+                                 int L, int align_corners, int align_mode, void* workspace, size_t workspace_bytes,
+                                 cspn_stream_t stream) {
+    begin_call();
+    long long n_lvl[kAffinityFuseMaxLevels];
+    int rc = check_affinity_fuse(B, C, H, W, L, level_hw, align_corners, align_mode, levels, grad_levels, true, n_lvl,
+                                 {{gate, 0, "gate"}, {out, 0, "out"}, {grad_out, 0, "grad_out"}}, {{grad_gate, 0, "grad_gate"}});
+    if (rc != CSPN_OK) return rc;
+    const size_t need = affinity_fuse_bwd_workspace_bytes(B, C, H, W, L, level_hw);
+    if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 3)) {
+        set_error("the backward needs %zu bytes of 4-byte aligned workspace (got %zu)", need, workspace_bytes);
+        return CSPN_ERR_WORKSPACE;
+    }
+    const uintptr_t n_g = span_bytes(B, L, (long long)H * W), n_o = span_bytes(B, C, (long long)H * W);
+    LevelNames in_names, out_names;
+    std::vector<Buf> in{{gate, n_g, "gate"}, {out, n_o, "out"}, {grad_out, n_o, "grad_out"}};
+    std::vector<Buf> outs{{grad_gate, n_g, "grad_gate"}, {workspace, need, "the workspace"}};
+    add_levels(in, levels, B, C, L, n_lvl, "levels", in_names);
+    add_levels(outs, grad_levels, B, C, L, n_lvl, "grad_levels", out_names);
+    rc = check_disjoint(in, outs);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(gate, "gate", [&](int* launches) {
+        return affinity_fuse_backward(levels, level_hw, gate, out, grad_out, grad_levels, grad_gate, B, C, H, W, L, align_corners,
+                                      align_mode, workspace, (cudaStream_t)stream, launches);
     });
 }
 

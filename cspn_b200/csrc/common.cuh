@@ -214,4 +214,17 @@ int affinity_pool_backward(const float* feat, const float* gate, const float* ou
                            float* grad_gate, int B, int C, int H, int W, int L, const int* kernel_sizes, cudaStream_t st,
                            int* launches);
 
+// Affinity fusion, the CSPN stereo network's spatial pyramid fusion (affinity_fuse.cu): L <= 8 levels (B, C, h_l, w_l),
+// level_hw = (h_0, w_0, h_1, w_1, ...), resampled to (H, W) and combined with the normalised gates (B, L, H, W); arguments
+// checked by the caller (sizes, flags, pointers, then launchable).  The backward's workspace holds the weight planes and the
+// row pass, affinity_fuse_bwd_workspace_bytes() (0 when it would reach 2^62 bytes)
+constexpr int kAffinityFuseMaxLevels = 8;
+int affinity_fuse_launchable(int B, int C, int H, int W, int L, const int* level_hw, const char** why);
+size_t affinity_fuse_bwd_workspace_bytes(int B, int C, int H, int W, int L, const int* level_hw);
+int affinity_fuse_forward(const float* const* levels, const int* level_hw, const float* gate, float* out, int B, int C, int H,
+                          int W, int L, int align_corners, int align_mode, cudaStream_t st, int* launches);
+int affinity_fuse_backward(const float* const* levels, const int* level_hw, const float* gate, const float* out,
+                           const float* grad_out, float* const* grad_levels, float* grad_gate, int B, int C, int H, int W, int L,
+                           int align_corners, int align_mode, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

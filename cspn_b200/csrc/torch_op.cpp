@@ -59,6 +59,11 @@
 //       level-major in one flat tensor)
 //   affinity_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] kernel_sizes) -> (Tensor, Tensor)
 //       (grad_feat, grad_gate; out and grad_out packed as the forward's result)
+//   affinity_fuse2d(Tensor[] levels, Tensor gate, bool align_corners, int align_mode) -> Tensor
+//       (CSPN's spatial pyramid fusion: L levels (B, C, h_l, w_l) upsampled to gate (B, L, H, W)'s size and combined with
+//       its normalised affinities -> (B, C, H, W))
+//   affinity_fuse2d_backward(Tensor[] levels, Tensor gate, Tensor out, Tensor grad_out, bool align_corners, int align_mode)
+//       -> (Tensor[], Tensor)   (grad_levels, grad_gate)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -723,6 +728,88 @@ std::tuple<at::Tensor, at::Tensor> affinity_pool2d_backward_cuda(const at::Tenso
     return {gf, gg};
 }
 
+// Affinity fusion: L levels (B, C, h_l, w_l) and gate (B, L, H, W) -> (B, C, H, W).  The C ABI takes int sizes and < 2^31
+// elements per (B, channel) slice of every tensor: refuse the rest before allocating or narrowing to int.  Returns the
+// levels' (h_l, w_l), flattened.
+std::vector<int> check_affinity_fuse(at::TensorList levels, const at::Tensor& gate, int64_t align_mode) {
+    TORCH_CHECK_VALUE(levels.size() >= 1 && levels.size() <= 8, "levels must hold 1..8 tensors, got ", levels.size());
+    TORCH_CHECK_VALUE(gate.dim() == 4 && gate.size(1) == (int64_t)levels.size(),
+                      "gate must be (B, L, H, W) with L = ", levels.size(), " levels, got ", gate.sizes());
+    TORCH_CHECK_VALUE(align_mode == 0 || align_mode == 1, "align_mode must be 0 or 1, got ", align_mode);
+    TORCH_CHECK_VALUE(gate.numel() > 0, "gate must not be empty, got ", gate.sizes());
+    const at::Tensor& x0 = levels[0];
+    TORCH_CHECK(gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    std::vector<int> hw;
+    for (const at::Tensor& x : levels) {
+        TORCH_CHECK_VALUE(x.dim() == 4 && x.size(0) == gate.size(0) && x.size(1) == x0.size(1) && x.numel() > 0,
+                          "every level must be a non-empty (B, C, h, w) with gate's B and one C, got ", x.sizes(), " for gate ",
+                          gate.sizes());
+        TORCH_CHECK(x.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+        TORCH_CHECK(x.device() == gate.device(), "the levels and gate are on different devices");
+        TORCH_CHECK(volume_fits_int(1, x.size(2), x.size(3)), "affinity_fuse2d takes < 2^31 elements per (B, channel) slice, got ",
+                    x.sizes());
+        hw.push_back((int)x.size(2));
+        hw.push_back((int)x.size(3));
+    }
+    TORCH_CHECK(gate.size(0) < ((int64_t)1 << 31) && x0.size(1) < ((int64_t)1 << 31) && volume_fits_int(1, gate.size(2), gate.size(3)),
+                "affinity_fuse2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got gate ", gate.sizes());
+    return hw;
+}
+
+std::vector<const float*> level_ptrs(const std::vector<at::Tensor>& xs) {
+    std::vector<const float*> p;
+    for (const at::Tensor& x : xs) p.push_back(fptr(x));
+    return p;
+}
+
+std::vector<at::Tensor> contiguous_all(at::TensorList xs) {
+    std::vector<at::Tensor> c;
+    for (const at::Tensor& x : xs) c.push_back(x.contiguous());
+    return c;
+}
+
+at::Tensor affinity_fuse2d_cuda(at::TensorList levels, const at::Tensor& gate, bool align_corners, int64_t align_mode) {
+    const std::vector<int> hw = check_affinity_fuse(levels, gate, align_mode);
+    const c10::cuda::CUDAGuard guard(gate.device());
+    const std::vector<at::Tensor> xs = contiguous_all(levels);
+    const at::Tensor g = gate.contiguous();
+    at::Tensor out = at::empty({g.size(0), xs[0].size(1), g.size(2), g.size(3)}, g.options());
+    check_rc(cspn_affinity_fuse2d_fwd_f32(level_ptrs(xs).data(), hw.data(), fptr(g), mptr(out), (int)g.size(0), (int)xs[0].size(1),
+                                          (int)g.size(2), (int)g.size(3), (int)xs.size(), align_corners, (int)align_mode,
+                                          current_stream()),
+             "cspn_affinity_fuse2d_fwd_f32");
+    return out;
+}
+
+std::tuple<std::vector<at::Tensor>, at::Tensor> affinity_fuse2d_backward_cuda(at::TensorList levels, const at::Tensor& gate,
+                                                                              const at::Tensor& out, const at::Tensor& grad_out,
+                                                                              bool align_corners, int64_t align_mode) {
+    const std::vector<int> hw = check_affinity_fuse(levels, gate, align_mode);
+    const std::vector<int64_t> shape{gate.size(0), levels[0].size(1), gate.size(2), gate.size(3)};
+    TORCH_CHECK_VALUE(out.sizes() == at::IntArrayRef(shape) && grad_out.sizes() == at::IntArrayRef(shape),
+                      "out and grad_out must be (B, C, H, W) = ", at::IntArrayRef(shape), ", got ", out.sizes(), " and ",
+                      grad_out.sizes());
+    TORCH_CHECK(out.scalar_type() == at::kFloat && grad_out.scalar_type() == at::kFloat && out.device() == gate.device() &&
+                    grad_out.device() == gate.device(),
+                "out and grad_out must be fp32 on gate's device");
+    const c10::cuda::CUDAGuard guard(gate.device());
+    const std::vector<at::Tensor> xs = contiguous_all(levels);
+    const at::Tensor g = gate.contiguous(), o = out.contiguous(), go = grad_out.contiguous();
+    std::vector<at::Tensor> gl;
+    std::vector<float*> glp;
+    for (const at::Tensor& x : xs) {
+        gl.push_back(at::empty_like(x));
+        glp.push_back(mptr(gl.back()));
+    }
+    at::Tensor gg = at::empty_like(g);
+    const int B = (int)g.size(0), C = (int)xs[0].size(1), H = (int)g.size(2), W = (int)g.size(3), L = (int)xs.size();
+    const Workspace ws(cspn_affinity_fuse2d_bwd_workspace_bytes(B, C, H, W, L, hw.data()), g);
+    check_rc(cspn_affinity_fuse2d_bwd_f32(level_ptrs(xs).data(), hw.data(), fptr(g), fptr(o), fptr(go), glp.data(), mptr(gg), B, C,
+                                          H, W, L, align_corners, (int)align_mode, ws.ptr(), ws.bytes, current_stream()),
+             "cspn_affinity_fuse2d_bwd_f32");
+    return {gl, gg};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -766,6 +853,9 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("gwc_volume_backward(Tensor left, Tensor right, Tensor grad_out) -> (Tensor, Tensor)");
     m.def("affinity_pool2d(Tensor feat, Tensor gate, int[] kernel_sizes) -> Tensor");
     m.def("affinity_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] kernel_sizes) -> (Tensor, Tensor)");
+    m.def("affinity_fuse2d(Tensor[] levels, Tensor gate, bool align_corners, int align_mode) -> Tensor");
+    m.def("affinity_fuse2d_backward(Tensor[] levels, Tensor gate, Tensor out, Tensor grad_out, bool align_corners, "
+          "int align_mode) -> (Tensor[], Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -797,4 +887,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("gwc_volume_backward", &gwc_volume_backward_cuda);
     m.impl("affinity_pool2d", &affinity_pool2d_cuda);
     m.impl("affinity_pool2d_backward", &affinity_pool2d_backward_cuda);
+    m.impl("affinity_fuse2d", &affinity_fuse2d_cuda);
+    m.impl("affinity_fuse2d_backward", &affinity_fuse2d_backward_cuda);
 }

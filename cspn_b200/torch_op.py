@@ -360,6 +360,31 @@ def _register():
 
     lib.register_autograd('cspn_b200::affinity_pool2d', backward_pool, setup_context=setup_pool)
 
+    @lib.register_fake('cspn_b200::affinity_fuse2d')
+    def _(levels, gate, align_corners, align_mode):
+        torch._check(1 <= len(levels) <= 8 and gate.dim() == 4 and gate.shape[1] == len(levels) and align_mode in (0, 1),
+                     lambda: 'levels must be 1..8 tensors (B, C, h, w) and gate (B, L, H, W)')
+        torch._check(all(x.dim() == 4 and x.shape[:2] == levels[0].shape[:2] for x in levels),
+                     lambda: 'every level must be (B, C, h, w) with one B and C')
+        return gate.new_empty((gate.shape[0], levels[0].shape[1], gate.shape[2], gate.shape[3]))
+
+    @lib.register_fake('cspn_b200::affinity_fuse2d_backward')
+    def _(levels, gate, out, grad_out, align_corners, align_mode):
+        torch._check(gate.dim() == 4 and out.shape == grad_out.shape, lambda: 'gate must be 4D and grad_out match out')
+        return [x.new_empty(x.shape) for x in levels], gate.new_empty(gate.shape)
+
+    def setup_fuse(ctx, inputs, output):
+        levels, gate, align_corners, align_mode = inputs
+        ctx.cfg = (align_corners, align_mode)
+        ctx.save_for_backward(gate, output, *levels)
+
+    def backward_fuse(ctx, grad_out):
+        gate, out, *levels = ctx.saved_tensors
+        gl, gg = torch.ops.cspn_b200.affinity_fuse2d_backward(levels, gate, out, grad_out.contiguous(), *ctx.cfg)
+        return list(gl), gg, None, None
+
+    lib.register_autograd('cspn_b200::affinity_fuse2d', backward_fuse, setup_context=setup_fuse)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

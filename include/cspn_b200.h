@@ -474,6 +474,36 @@ CSPN_API int cspn_affinity_pool2d_bwd_f32(const float* feat, const float* gate, 
                                   float* grad_feat, float* grad_gate, int B, int C, int H, int W, int L,
                                   const int* kernel_sizes, cspn_stream_t stream);
 
+/* ---- affinity fusion: the CSPN stereo network's spatial pyramid fusion --------------------------------------------------
+ * levels a HOST array of L DEVICE pointers, level l [B][C][h_l][w_l]; level_hw a HOST array (h_0, w_0, h_1, w_1, ...) of 2L
+ * ints, 1 <= L <= 8, any h_l, w_l >= 1 (a level may be finer than the output); gate [B][L][H][W], channel l the raw
+ * affinity of level l, shared by all C channels; out [B][C][H][W].  At every pixel q:
+ *   a_l = |gate_l(q)|,  S = sum_l a_l,  w_l = a_l / S,  out[c](q) = sum_l w_l * u_l[c](q)
+ * u_l is level l resampled bilinearly to H x W with resize_trilinear's per-axis rule (align_corners, align_mode as there):
+ *   u = l0h*(l0w*x[h0][w0] + l1w*x[h0][w1]) + l1h*(l0w*x[h1][w0] + l1w*x[h1][w1]), every product computed.
+ * S and out summed in ascending l from the first term; backward
+ *   grad_gate_l(q) = ((sum_c grad_out[c](q) * (u_l[c](q) - out[c](q)), ascending c) / S) * sgn(gate_l(q))
+ *   grad_levels[l] = resize_trilinear's gather over H and W of v = w_l * grad_out: sum_oh (sum_ow v * lw) * lh, each sum
+ *                    from 0 in ascending o, both products (v * l0 first) where i1 == i0; +0.0 where no output reads a cell
+ * every operation rounded on its own (DESIGN.md section 4.18).  All-zero gates at a pixel give NaN (0/0) in every channel
+ * there.  Levels may alias one another (the caller adds their gradients).  CSPN_ERR_INVALID_ARGUMENT for a null or not
+ * 4-byte aligned pointer, a size < 1, L outside [1, 8], an align flag outside {0, 1}, and an output (the workspace
+ * included) that overlaps an input or another output.  CSPN_ERR_UNSUPPORTED for H*W >= 2^31 or h_l*w_l >= 2^31 (the grids
+ * then stay within their limits).  No atomics, no memset, every output element written once; the bits depend on the
+ * arguments only.  The forward is one launch; the backward three, with
+ * cspn_affinity_fuse2d_bwd_workspace_bytes() bytes of 4-byte aligned workspace (0 for invalid sizes).  No allocation, no
+ * synchronisation. */
+CSPN_API int cspn_affinity_fuse2d_fwd_f32(const float* const* levels, const int* level_hw, const float* gate, float* out,
+                                  int B, int C, int H, int W, int L, int align_corners, int align_mode,
+                                  cspn_stream_t stream);
+
+CSPN_API size_t cspn_affinity_fuse2d_bwd_workspace_bytes(int B, int C, int H, int W, int L, const int* level_hw);
+
+CSPN_API int cspn_affinity_fuse2d_bwd_f32(const float* const* levels, const int* level_hw, const float* gate,
+                                  const float* out, const float* grad_out, float* const* grad_levels, float* grad_gate,
+                                  int B, int C, int H, int W, int L, int align_corners, int align_mode, void* workspace,
+                                  size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
