@@ -80,6 +80,9 @@ SIGNATURES = {
     'cspn_affinity_fuse2d_fwd_f32': (_i, [_vp] * 4 + [_i] * 7 + [_vp]),
     'cspn_affinity_fuse2d_bwd_workspace_bytes': (_sz, [_i] * 5 + [_vp]),
     'cspn_affinity_fuse2d_bwd_f32': (_i, [_vp] * 7 + [_i] * 7 + [_vp, _sz, _vp]),
+    'cspn_affinity_atrous2d_fwd_f32': (_i, [_vp] * 3 + [_i] * 5 + [_vp] * 2),
+    'cspn_affinity_atrous2d_bwd_workspace_bytes': (_sz, [_i] * 5 + [_vp]),
+    'cspn_affinity_atrous2d_bwd_f32': (_i, [_vp] * 6 + [_i] * 5 + [_vp, _vp, _sz, _vp]),
     'cspn_host_alloc': (_vp, [_sz]),
     'cspn_host_free': (None, [_vp]),
     'cspn_last_error': (_cp, []),

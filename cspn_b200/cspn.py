@@ -1437,3 +1437,100 @@ def affinity_fuse2d(levels, gate, align_corners=True, align_mode=1):
     if torch.is_grad_enabled() and (gate.requires_grad or any(x.requires_grad for x in lv)):
         return _AffinityFuseFn.apply(align_corners, align_mode, gate, *lv)
     return _fuse_fwd(lv, gate, align_corners, align_mode)
+
+
+# ---- atrous affinity pooling: the CSPN stereo network's atrous spatial pyramid pooling (ACSPP) ---------------------------------
+def _check_affinity_atrous(feat, gate, dilations):
+    """The checks of affinity_atrous_pool2d; every refusal comes before anything is allocated or narrowed to int.  Returns
+    the rates as a tuple of ints."""
+    if feat.dim() != 4 or gate.dim() != 4:
+        raise ValueError(f'feat must be (B,C,H,W) and gate (B,9L,H,W), got {tuple(feat.shape)} and {tuple(gate.shape)}')
+    B, C, H, W = feat.shape
+    if min(B, C, H, W) < 1:
+        raise ValueError(f'feat must not be empty, got {tuple(feat.shape)}')
+    if (isinstance(dilations, (str, bytes)) or not hasattr(dilations, '__len__')
+            or any(isinstance(r, bool) or not isinstance(r, int) for r in dilations)):
+        raise ValueError(f'dilations must be a sequence of ints, got {dilations!r}')
+    rates = tuple(dilations)
+    if not 1 <= len(rates) <= 8:
+        raise ValueError(f'dilations must hold 1 to 8 rates, got {len(rates)}')
+    if any(not 1 <= r <= max(H, W) for r in rates):
+        raise ValueError(f'dilations must be in [1, max(H, W) = {max(H, W)}], got {rates}')
+    if tuple(gate.shape) != (B, 9 * len(rates), H, W):
+        raise ValueError(f'gate must be (B, 9L, H, W) = {(B, 9 * len(rates), H, W)}, got {tuple(gate.shape)}')
+    if feat.dtype != torch.float32 or gate.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if feat.device != gate.device:
+        raise RuntimeError('feat and gate are on different devices')
+    if B > 2 ** 31 - 1 or C > 2 ** 31 - 1 or H * W >= 2 ** 31:
+        raise _lib.CspnError(f'affinity_atrous_pool2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got feat '
+                             f'{tuple(feat.shape)}')
+    if not feat.is_cuda:
+        raise _lib.CspnError('affinity_atrous_pool2d takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return rates
+
+
+def _atrous_fwd(feat, gate, rates):
+    """Forward only (no autograd) through cspn_affinity_atrous2d_fwd_f32, on the current stream."""
+    f, g = feat.contiguous(), gate.contiguous()
+    B, C, H, W = f.shape
+    out = f.new_empty((B, len(rates) * C, H, W))
+    with torch.cuda.device(f.device):
+        rc = _lib.lib().cspn_affinity_atrous2d_fwd_f32(_ptr(f), _ptr(g), _ptr(out), B, C, H, W, len(rates), _c_sizes(rates),
+                                                        _stream(f.device))
+    _lib.check(rc, 'cspn_affinity_atrous2d_fwd_f32')
+    return out
+
+
+def _atrous_bwd(feat, gate, out, grad_out, rates):
+    """grad_feat, grad_gate through cspn_affinity_atrous2d_bwd_f32."""
+    f, g, o, go = feat.contiguous(), gate.contiguous(), out.contiguous(), grad_out.contiguous()
+    B, C, H, W = f.shape
+    gf, gg = torch.empty_like(f), torch.empty_like(g)
+    r = _c_sizes(rates)
+    Lb = _lib.lib()
+    with torch.cuda.device(f.device):
+        ws_bytes = Lb.cspn_affinity_atrous2d_bwd_workspace_bytes(B, C, H, W, len(rates), r)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device)
+        rc = Lb.cspn_affinity_atrous2d_bwd_f32(_ptr(f), _ptr(g), _ptr(o), _ptr(go), _ptr(gf), _ptr(gg), B, C, H, W, len(rates), r,
+                                               _ptr(ws), ws_bytes, _stream(f.device))
+    _lib.check(rc, 'cspn_affinity_atrous2d_bwd_f32')
+    return gf, gg
+
+
+class _AffinityAtrousFn(torch.autograd.Function):
+    """autograd seam of affinity_atrous_pool2d without the torch-op shim: feat, gate and the output are saved."""
+
+    @staticmethod
+    def forward(ctx, feat, gate, rates):
+        out = _atrous_fwd(feat, gate, rates)
+        ctx.rates = rates
+        ctx.save_for_backward(feat, gate, out)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        feat, gate, out = ctx.saved_tensors
+        gf, gg = _atrous_bwd(feat, gate, out, grad_out, ctx.rates)
+        return gf, gg, None
+
+
+def affinity_atrous_pool2d(feat, gate, dilations):
+    """The CSPN stereo network's atrous spatial pyramid pooling (ACSPP), every level in one launch: each level is one CSPN
+    step at stride 1 over the 3x3 neighbourhood dilated by its rate.  feat (B, C, H, W) and gate (B, 9L, H, W) are fp32 CUDA
+    tensors and dilations holds L rates r_l (1 <= L <= 8, 1 <= r_l <= max(H, W), any order, repeats allowed).  Gate channel
+    9l + t is tap t of level l, offset (t // 3 - 1, t % 3 - 1) * r_l, tap 4 the centre, shared by all C channels.  At every
+    pixel w_t = |g_t| / sum_t |g_t| and out[:, l*C + c] = sum_t w_t * feat[:, c] at the tap, +0.0 outside the image (such a
+    tap still counts in the sum): F.unfold(feat, 3, dilation=r, padding=r) weighted and summed.  Returns (B, L*C, H, W),
+    the levels concatenated along the channels.  A constant gate gives the depthwise dilated 3x3 box filter; all-zero gates
+    of a level at a pixel give NaN there.  Differentiable in feat and gate, with a deterministic backward.  DESIGN.md
+    section 4.19."""
+    rates = _check_affinity_atrous(feat, gate, dilations)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.affinity_atrous_pool2d(feat, gate, list(rates))
+    if torch.is_grad_enabled() and (feat.requires_grad or gate.requires_grad):
+        return _AffinityAtrousFn.apply(feat, gate, rates)
+    return _atrous_fwd(feat, gate, rates)

@@ -1070,6 +1070,80 @@ int cspn_affinity_fuse2d_bwd_f32(const float* const* levels, const int* level_hw
     });
 }
 
+// ---- atrous affinity pooling (the CSPN stereo network's ACSPP) ---------------------------------------------------------------
+// The sizes, the levels and the rates: true when they are valid (the error is set otherwise)
+static bool atrous_args_ok(int B, int C, int H, int W, int L, const int* dilations) {
+    if (!positive(B, C, H, W)) { set_error("non-positive size B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (L < 1 || L > kAffinityAtrousMaxLevels) { set_error("the number of levels L=%d must be 1..8", L); return false; }
+    if (!dilations) { set_error("null dilations"); return false; }
+    const int lim = H > W ? H : W;
+    for (int l = 0; l < L; ++l)
+        if (dilations[l] < 1 || dilations[l] > lim) {
+            set_error("dilations[%d]=%d must be in [1, max(H, W)=%d]", l, dilations[l], lim);
+            return false;
+        }
+    return true;
+}
+
+// The sizes, the rates, the pointers, then the launch limits: `in` are read and `outs` written
+static int check_affinity_atrous(int B, int C, int H, int W, int L, const int* dilations, std::initializer_list<Buf> in,
+                                 std::initializer_list<Buf> outs) {
+    if (!atrous_args_ok(B, C, H, W, L, dilations)) return CSPN_ERR_INVALID_ARGUMENT;
+    uintptr_t bits = 0;
+    for (const auto* set : {&in, &outs})
+        for (const Buf& b : *set) {
+            if (!b.p) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+            bits |= reinterpret_cast<uintptr_t>(b.p);
+        }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!affinity_atrous_launchable(B, C, H, W, L, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    return CSPN_OK;
+}
+
+int cspn_affinity_atrous2d_fwd_f32(const float* feat, const float* gate, float* out, int B, int C, int H, int W, int L,
+                                   const int* dilations, cspn_stream_t stream) {
+    begin_call();
+    int rc = check_affinity_atrous(B, C, H, W, L, dilations, {{feat, 0, "feat"}, {gate, 0, "gate"}}, {{out, 0, "out"}});
+    if (rc != CSPN_OK) return rc;
+    const long long hw = (long long)H * W;
+    rc = check_disjoint({{feat, span_bytes(B, C, hw), "feat"}, {gate, span_bytes(B, 9 * L, hw), "gate"}},
+                        {{out, span_bytes(B, C, L * hw), "out"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return affinity_atrous_forward(feat, gate, out, B, C, H, W, L, dilations, (cudaStream_t)stream, launches);
+    });
+}
+
+size_t cspn_affinity_atrous2d_bwd_workspace_bytes(int B, int C, int H, int W, int L, const int* dilations) {
+    if (!atrous_args_ok(B, C, H, W, L, dilations)) return 0;
+    return affinity_atrous_bwd_workspace_bytes(B, H, W, L);
+}
+
+int cspn_affinity_atrous2d_bwd_f32(const float* feat, const float* gate, const float* out, const float* grad_out,
+                                   float* grad_feat, float* grad_gate, int B, int C, int H, int W, int L, const int* dilations,
+                                   void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    int rc = check_affinity_atrous(B, C, H, W, L, dilations,
+                                   {{feat, 0, "feat"}, {gate, 0, "gate"}, {out, 0, "out"}, {grad_out, 0, "grad_out"}},
+                                   {{grad_feat, 0, "grad_feat"}, {grad_gate, 0, "grad_gate"}});
+    if (rc != CSPN_OK) return rc;
+    const size_t need = affinity_atrous_bwd_workspace_bytes(B, H, W, L);
+    if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 3)) {
+        set_error("the backward needs %zu bytes of 4-byte aligned workspace (got %zu)", need, workspace_bytes);
+        return CSPN_ERR_WORKSPACE;
+    }
+    const long long hw = (long long)H * W;
+    const uintptr_t n_f = span_bytes(B, C, hw), n_g = span_bytes(B, 9 * L, hw), n_o = span_bytes(B, C, L * hw);
+    rc = check_disjoint({{feat, n_f, "feat"}, {gate, n_g, "gate"}, {out, n_o, "out"}, {grad_out, n_o, "grad_out"}},
+                        {{grad_feat, n_f, "grad_feat"}, {grad_gate, n_g, "grad_gate"}, {workspace, need, "the workspace"}});
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return affinity_atrous_backward(feat, gate, out, grad_out, grad_feat, grad_gate, B, C, H, W, L, dilations, workspace,
+                                        (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

@@ -227,4 +227,17 @@ int affinity_fuse_backward(const float* const* levels, const int* level_hw, cons
                            const float* grad_out, float* const* grad_levels, float* grad_gate, int B, int C, int H, int W, int L,
                            int align_corners, int align_mode, void* ws, cudaStream_t st, int* launches);
 
+// Atrous affinity pooling, the CSPN stereo network's ACSPP (affinity_atrous.cu): L <= 8 levels of feat (B, C, H, W), level l
+// a 3 x 3 CSPN step dilated by dilations[l] with the gates (B, 9L, H, W), into out (B, L*C, H, W); arguments checked by the
+// caller (sizes, rates, pointers, then launchable).  The backward's workspace holds the weight planes (B, 9L, H, W),
+// affinity_atrous_bwd_workspace_bytes() (0 when it would reach 2^60 bytes)
+constexpr int kAffinityAtrousMaxLevels = 8;
+int affinity_atrous_launchable(int B, int C, int H, int W, int L, const char** why);
+size_t affinity_atrous_bwd_workspace_bytes(int B, int H, int W, int L);
+int affinity_atrous_forward(const float* feat, const float* gate, float* out, int B, int C, int H, int W, int L,
+                            const int* dilations, cudaStream_t st, int* launches);
+int affinity_atrous_backward(const float* feat, const float* gate, const float* out, const float* grad_out, float* grad_feat,
+                             float* grad_gate, int B, int C, int H, int W, int L, const int* dilations, void* ws, cudaStream_t st,
+                             int* launches);
+
 }  // namespace cspn

@@ -64,6 +64,11 @@
 //       its normalised affinities -> (B, C, H, W))
 //   affinity_fuse2d_backward(Tensor[] levels, Tensor gate, Tensor out, Tensor grad_out, bool align_corners, int align_mode)
 //       -> (Tensor[], Tensor)   (grad_levels, grad_gate)
+//   affinity_atrous_pool2d(Tensor feat, Tensor gate, int[] dilations) -> Tensor
+//       (CSPN's atrous spatial pyramid pooling: feat (B, C, H, W) and gate (B, 9L, H, W) -> (B, L*C, H, W), level l a 3x3
+//       CSPN step dilated by dilations[l])
+//   affinity_atrous_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] dilations)
+//       -> (Tensor, Tensor)   (grad_feat, grad_gate)
 // There is no CPU kernel: CPU tensors reach the dispatcher's "no kernel for backend CPU" error, loudly.
 #include <ATen/ATen.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -810,6 +815,59 @@ std::tuple<std::vector<at::Tensor>, at::Tensor> affinity_fuse2d_backward_cuda(at
     return {gl, gg};
 }
 
+// Atrous affinity pooling: feat (B, C, H, W), gate (B, 9L, H, W), L rates -> (B, L*C, H, W).  The C ABI takes int sizes and
+// < 2^31 elements per (B, channel) slice: refuse the rest before allocating or narrowing to int.
+void check_affinity_atrous(const at::Tensor& feat, const at::Tensor& gate, at::IntArrayRef rates) {
+    TORCH_CHECK_VALUE(feat.dim() == 4 && gate.dim() == 4 && gate.size(0) == feat.size(0) && gate.size(2) == feat.size(2) &&
+                          gate.size(3) == feat.size(3),
+                      "feat must be (B,C,H,W) and gate (B,9L,H,W), got ", feat.sizes(), " and ", gate.sizes());
+    TORCH_CHECK_VALUE(rates.size() >= 1 && rates.size() <= 8 && gate.size(1) == 9 * (int64_t)rates.size(),
+                      "dilations must hold 1..8 rates, nine gate channels each, got ", rates, " for gate ", gate.sizes());
+    TORCH_CHECK(feat.scalar_type() == at::kFloat && gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(feat.device() == gate.device(), "feat and gate are on different devices");
+    const int64_t H = feat.size(2), W = feat.size(3);
+    TORCH_CHECK_VALUE(feat.numel() > 0, "feat must not be empty, got ", feat.sizes());
+    for (int64_t r : rates)
+        TORCH_CHECK_VALUE(r >= 1 && r <= std::max(H, W), "dilations must be in [1, max(H, W)], got ", rates, " for ", H, "x", W);
+    TORCH_CHECK(feat.size(0) < ((int64_t)1 << 31) && feat.size(1) < ((int64_t)1 << 31) && volume_fits_int(1, H, W),
+                "affinity_atrous_pool2d takes B, C < 2^31 and < 2^31 elements per (B, channel) slice, got feat ", feat.sizes());
+}
+
+at::Tensor affinity_atrous_pool2d_cuda(const at::Tensor& feat, const at::Tensor& gate, at::IntArrayRef rates) {
+    check_affinity_atrous(feat, gate, rates);
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), g = gate.contiguous();
+    at::Tensor out = at::empty({f.size(0), (int64_t)rates.size() * f.size(1), f.size(2), f.size(3)}, f.options());
+    const std::vector<int> r = int_sizes(rates);
+    check_rc(cspn_affinity_atrous2d_fwd_f32(fptr(f), fptr(g), mptr(out), (int)f.size(0), (int)f.size(1), (int)f.size(2),
+                                            (int)f.size(3), (int)r.size(), r.data(), current_stream()),
+             "cspn_affinity_atrous2d_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor> affinity_atrous_pool2d_backward_cuda(const at::Tensor& feat, const at::Tensor& gate,
+                                                                        const at::Tensor& out, const at::Tensor& grad_out,
+                                                                        at::IntArrayRef rates) {
+    check_affinity_atrous(feat, gate, rates);
+    const std::vector<int64_t> shape{feat.size(0), (int64_t)rates.size() * feat.size(1), feat.size(2), feat.size(3)};
+    TORCH_CHECK_VALUE(out.sizes() == at::IntArrayRef(shape) && grad_out.sizes() == at::IntArrayRef(shape),
+                      "out and grad_out must be (B, L*C, H, W) = ", at::IntArrayRef(shape), ", got ", out.sizes(), " and ",
+                      grad_out.sizes());
+    TORCH_CHECK(out.scalar_type() == at::kFloat && grad_out.scalar_type() == at::kFloat && out.device() == feat.device() &&
+                    grad_out.device() == feat.device(),
+                "out and grad_out must be fp32 on feat's device");
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), g = gate.contiguous(), o = out.contiguous(), go = grad_out.contiguous();
+    at::Tensor gf = at::empty_like(f), gg = at::empty_like(g);
+    const std::vector<int> r = int_sizes(rates);
+    const int B = (int)f.size(0), C = (int)f.size(1), H = (int)f.size(2), W = (int)f.size(3), L = (int)r.size();
+    const Workspace ws(cspn_affinity_atrous2d_bwd_workspace_bytes(B, C, H, W, L, r.data()), f);
+    check_rc(cspn_affinity_atrous2d_bwd_f32(fptr(f), fptr(g), fptr(o), fptr(go), mptr(gf), mptr(gg), B, C, H, W, L, r.data(),
+                                            ws.ptr(), ws.bytes, current_stream()),
+             "cspn_affinity_atrous2d_bwd_f32");
+    return {gf, gg};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(cspn_b200, m) {
@@ -856,6 +914,9 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("affinity_fuse2d(Tensor[] levels, Tensor gate, bool align_corners, int align_mode) -> Tensor");
     m.def("affinity_fuse2d_backward(Tensor[] levels, Tensor gate, Tensor out, Tensor grad_out, bool align_corners, "
           "int align_mode) -> (Tensor[], Tensor)");
+    m.def("affinity_atrous_pool2d(Tensor feat, Tensor gate, int[] dilations) -> Tensor");
+    m.def("affinity_atrous_pool2d_backward(Tensor feat, Tensor gate, Tensor out, Tensor grad_out, int[] dilations) -> "
+          "(Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
@@ -889,4 +950,6 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("affinity_pool2d_backward", &affinity_pool2d_backward_cuda);
     m.impl("affinity_fuse2d", &affinity_fuse2d_cuda);
     m.impl("affinity_fuse2d_backward", &affinity_fuse2d_backward_cuda);
+    m.impl("affinity_atrous_pool2d", &affinity_atrous_pool2d_cuda);
+    m.impl("affinity_atrous_pool2d_backward", &affinity_atrous_pool2d_backward_cuda);
 }

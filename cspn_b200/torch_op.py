@@ -385,6 +385,32 @@ def _register():
 
     lib.register_autograd('cspn_b200::affinity_fuse2d', backward_fuse, setup_context=setup_fuse)
 
+    @lib.register_fake('cspn_b200::affinity_atrous_pool2d')
+    def _(feat, gate, dilations):
+        torch._check(feat.dim() == 4 and gate.dim() == 4 and 1 <= len(dilations) <= 8 and gate.shape[1] == 9 * len(dilations),
+                     lambda: 'feat must be (B,C,H,W), gate (B,9L,H,W) and dilations L <= 8 ints')
+        B, C, H, W = feat.shape
+        torch._check(all(1 <= r <= max(H, W) for r in dilations), lambda: 'dilations must be in [1, max(H, W)]')
+        return feat.new_empty((B, len(dilations) * C, H, W))
+
+    @lib.register_fake('cspn_b200::affinity_atrous_pool2d_backward')
+    def _(feat, gate, out, grad_out, dilations):
+        torch._check(feat.dim() == 4 and gate.dim() == 4 and out.dim() == 4 and grad_out.shape == out.shape,
+                     lambda: 'feat, gate and out must be 4D, and grad_out match out')
+        return feat.new_empty(feat.shape), gate.new_empty(gate.shape)
+
+    def setup_atrous(ctx, inputs, output):
+        feat, gate, dilations = inputs
+        ctx.dilations = dilations
+        ctx.save_for_backward(feat, gate, output)
+
+    def backward_atrous(ctx, grad_out):
+        feat, gate, out = ctx.saved_tensors
+        gf, gg = torch.ops.cspn_b200.affinity_atrous_pool2d_backward(feat, gate, out, grad_out.contiguous(), ctx.dilations)
+        return gf, gg, None
+
+    lib.register_autograd('cspn_b200::affinity_atrous_pool2d', backward_atrous, setup_context=setup_atrous)
+
 
 def _register_gates(lib, nd):
     """Fake kernels and autograd of affinity_propagate{nd}d (fluid.layers.affinity_propagate with the caller's gates)."""

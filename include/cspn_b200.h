@@ -504,6 +504,33 @@ CSPN_API int cspn_affinity_fuse2d_bwd_f32(const float* const* levels, const int*
                                   int B, int C, int H, int W, int L, int align_corners, int align_mode, void* workspace,
                                   size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- atrous affinity pooling: the CSPN stereo network's atrous spatial pyramid pooling (ACSPP) --------------------------
+ * feat [B][C][H][W]; dilations a HOST array of L ints, 1 <= L <= 8, each 1 <= r_l <= max(H, W), in any order, repeats
+ * allowed; gate [B][9L][H][W], channel 9l + t the raw affinity of tap t of level l, offset (dy, dx) = (t/3 - 1, t%3 - 1)
+ * (tap 4 the centre, learned like the others), shared by all C channels; out [B][L*C][H][W], channels lC .. lC + C - 1
+ * level l.  At every pixel p, with r = r_l and feat = +0.0 outside the image (a tap there still counts in S):
+ *   a_t = |gate[9l + t](p)|,  S = sum_t a_t,  w_t = a_t / S,  out[lC + c](p) = sum_t w_t * feat[c](p + r (dy_t, dx_t))
+ * S and out summed in ascending t from the first term; backward
+ *   grad_gate[9l + t](p) = ((sum_c grad_out[lC + c](p) * (feat[c](p + r d_t) - out[lC + c](p)), ascending c) / S) * sgn(gate)
+ *   grad_feat[c](q)      = sum over l ascending, then t ascending, of w_{l,t}(q - r_l d_t) * grad_out[lC + c](q - r_l d_t),
+ *                          over the terms whose source pixel lies in the image
+ * every operation rounded on its own (DESIGN.md section 4.19).  All-zero gates of a level at a pixel give NaN (0/0) in
+ * every channel of that level there.  CSPN_ERR_INVALID_ARGUMENT for a null or not 4-byte aligned pointer, a size < 1,
+ * L outside [1, 8], a null dilations or an r_l outside [1, max(H, W)], and an output (the workspace included) that
+ * overlaps an input or another output; CSPN_ERR_WORKSPACE for a null, short or not 4-byte aligned workspace.
+ * CSPN_ERR_UNSUPPORTED for H*W >= 2^31 and a grid of 2^31 blocks or more.  No atomics, no memset, every output element
+ * written once; the bits depend on the arguments only.  The forward is one launch; the backward two, with
+ * cspn_affinity_atrous2d_bwd_workspace_bytes() bytes of 4-byte aligned workspace (4 * B*9L*H*W, the weight planes; 0 for
+ * invalid arguments).  No allocation, no synchronisation. */
+CSPN_API int cspn_affinity_atrous2d_fwd_f32(const float* feat, const float* gate, float* out, int B, int C, int H, int W,
+                                    int L, const int* dilations, cspn_stream_t stream);
+
+CSPN_API size_t cspn_affinity_atrous2d_bwd_workspace_bytes(int B, int C, int H, int W, int L, const int* dilations);
+
+CSPN_API int cspn_affinity_atrous2d_bwd_f32(const float* feat, const float* gate, const float* out, const float* grad_out,
+                                    float* grad_feat, float* grad_gate, int B, int C, int H, int W, int L,
+                                    const int* dilations, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- what the reference does with the result on the HOST after every step, on the device ------------------------
  * utils.evaluate_error(gt_depth, pred_depth) (cspn_pytorch/utils.py:19-47; called at train.py:206, eval.py:150 after a
  * `.cpu()` of both tensors) and Wighted_L1_Loss (loss.py:12-23).  One pass over n = B*C*H*W elements; out12 (DEVICE):
