@@ -502,6 +502,108 @@ class Affinity_PropagateK(nn.Module):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, norm_type={self.norm_type!r}{keep}'
 
 
+# ---- aggregation of the 2D steps: CSPN++'s context-aware CSPN (DESIGN.md section 4.20) ------------------------------------
+def _check_aggregate(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, steps):
+    """The checks of propagate2d_aggregate, every refusal of an argument before the device check; returns the steps as a
+    tuple of ints (default 1..T)."""
+    if step_weight.dim() != 4 or blur_depth.dim() != 4:
+        raise ValueError(f'step_weight and blur_depth must be (B,T,H,W) and (B,C,H,W), got {tuple(step_weight.shape)} and '
+                         f'{tuple(blur_depth.shape)}')
+    B, C, H, W = blur_depth.shape
+    T = step_weight.shape[1]
+    if steps is None:
+        steps = tuple(range(1, T + 1))
+    if (isinstance(steps, (str, bytes)) or not hasattr(steps, '__len__')
+            or any(isinstance(s, bool) or not isinstance(s, int) for s in steps)):
+        raise ValueError(f'steps must be a sequence of ints, got {steps!r}')
+    steps = tuple(steps)
+    if not steps or steps[0] < 1 or any(a >= b for a, b in zip(steps, steps[1:])) or steps[-1] > 2 ** 31 - 1:
+        raise ValueError(f'steps must be strictly increasing ints >= 1, got {steps}')
+    if tuple(step_weight.shape) != (B, len(steps), H, W):
+        raise ValueError(f'step_weight must be (B, len(steps), H, W) = {(B, len(steps), H, W)}, got {tuple(step_weight.shape)}')
+    if step_weight.dtype != torch.float32 or step_weight.device != blur_depth.device:
+        raise RuntimeError('step_weight must be fp32 on the device of blur_depth')
+    _check_inputs_2d_k(guidance, blur_depth, sparse_depth, prop_kernel)
+    return steps
+
+
+def _aggregate_fwd(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps):
+    """Forward only (no autograd) through cspn2d_agg_fwd_f32, on the current stream."""
+    L = _lib.lib()
+    B, C, H, W = blur_depth.shape
+    g, d, w = guidance.contiguous(), blur_depth.contiguous(), step_weight.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    out = torch.empty_like(d)
+    st = _c_sizes(steps)
+    with torch.cuda.device(d.device):
+        ws_bytes = L.cspn2d_agg_workspace_bytes(B, C, H, W, prop_kernel, st, len(steps), int(keep))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+        rc = L.cspn2d_agg_fwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(w), _ptr(out), B, C, H, W, g.shape[1], prop_kernel, st, len(steps),
+                                  code, int(keep), _ptr(ws), ws_bytes, _stream(d.device))
+    _lib.check(rc, 'cspn2d_agg_fwd_f32')
+    return out
+
+
+class _Propagate2dAggregateFn(torch.autograd.Function):
+    """autograd seam of propagate2d_aggregate without the torch-op shim: native forward + native adjoint
+    (cspn2d_agg_bwd_f32), differentiable in guidance, blur_depth, step_weight and, in keep mode, sparse_depth."""
+
+    @staticmethod
+    def forward(ctx, guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps):
+        ctx.save_for_backward(guidance, blur_depth, step_weight, sparse_depth)
+        ctx.cfg = (prop_kernel, code, keep, steps)
+        return _aggregate_fwd(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        guidance, blur_depth, step_weight, sparse_depth = ctx.saved_tensors
+        prop_kernel, code, keep, steps = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        B, C, H, W = blur_depth.shape
+        g, d, w, go = guidance.contiguous(), blur_depth.contiguous(), step_weight.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        need_g, need_d, need_w, need_s = ctx.needs_input_grad[:4]
+        need_s = need_s and keep
+        gg = torch.empty_like(g) if need_g else None
+        gd = torch.empty_like(d) if need_d else None
+        gw = torch.empty_like(w) if need_w else None
+        gs = torch.empty_like(s) if need_s and s is not None else None
+        st = _c_sizes(steps)
+        with torch.cuda.device(d.device):
+            ws_bytes = L.cspn2d_agg_bwd_workspace_bytes(B, C, H, W, prop_kernel, st, len(steps), int(keep))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+            rc = L.cspn2d_agg_bwd_f32(_ptr(g), _ptr(d), _ptr(s), _ptr(w), _ptr(go), _ptr(gg), _ptr(gd), _ptr(gs), _ptr(gw), B, C, H, W,
+                                      g.shape[1], prop_kernel, st, len(steps), code, int(keep), _ptr(ws), ws_bytes, _stream(d.device))
+        _lib.check(rc, 'cspn2d_agg_bwd_f32')
+        return gg, gd, gw, gs, None, None, None, None
+
+
+def propagate2d_aggregate(guidance, blur_depth, step_weight, sparse_depth=None, prop_kernel=3, norm_type=None, keep_sparse=False,
+                          steps=None):
+    """CSPN++'s context-aware CSPN for one kernel size: a per-pixel weighted sum of the 2D propagation's iterates,
+        out = sum_j step_weight[:, j] * d_{steps[j]},
+    where d_0 = blur_depth and d_{t+1} is one step of propagate2d_k(..., prop_kernel, keep_sparse=keep_sparse), so the run
+    is steps[-1] steps long.  guidance (B, >=K*K-1, H, W), blur_depth (B, C, H, W), sparse_depth (B, 1, H, W) or None and
+    step_weight (B, T, H, W), shared by the C channels, are fp32 CUDA tensors; steps holds T strictly increasing ints >= 1
+    (default 1..T).  The weights are used as given: apply CSPN++'s softmax before the call.  No iterate is stored: the
+    forward keeps the running sum in the output.  Differentiable in guidance, blur_depth, step_weight and, with
+    keep_sparse=True, sparse_depth.  DESIGN.md section 4.20."""
+    code = norm_code_2d_k(prop_kernel, norm_type)
+    steps = _check_aggregate(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, steps)
+    keep = bool(keep_sparse)
+    if not keep and sparse_depth is not None:
+        sparse_depth = sparse_depth.detach()       # the default mode's m = sign(sparse) takes no gradient
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.propagate2d_aggregate(guidance, blur_depth, sparse_depth, step_weight, list(steps), prop_kernel,
+                                                         code, keep)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (guidance, blur_depth, step_weight, sparse_depth)):
+        return _Propagate2dAggregateFn.apply(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps)
+    return _aggregate_fwd(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps)
+
+
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
 KERNEL_SIZES_3D = (3, 5)
 

@@ -1144,6 +1144,109 @@ int cspn_affinity_atrous2d_bwd_f32(const float* feat, const float* gate, const f
     });
 }
 
+// ---- 2D aggregation of the steps, K in {3, 5, 7} (DESIGN.md section 4.20): the K x K kernels of cspn2d_wide.cu at every K --
+// The sizes, K, the norm, keep and the step list: true when they are valid (the error is set otherwise)
+static bool agg_args_ok(int B, int C, int H, int W, int K, int gch, const int* steps, int n_steps, int norm_type, int keep) {
+    if (!positive(B, C, H, W)) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (!kernel_size_ok(2, K)) { set_error("2D kernel size must be 3, 5 or 7, got %d", K); return false; }
+    if (gch < K * K - 1) { set_error("a %dx%d kernel needs >= %d guidance channels, got %d", K, K, K * K - 1, gch); return false; }
+    if (norm_type < 0 || norm_type > (int)CSPN_NORM_8SUM_ABS) { set_error("unknown norm_type %d", norm_type); return false; }
+    if (keep != 0 && keep != 1) { set_error("keep must be 0 or 1, got %d", keep); return false; }
+    if (n_steps < 1 || !steps) { set_error("the aggregation needs n_steps >= 1 and a step array, got %d", n_steps); return false; }
+    for (int j = 0; j < n_steps; ++j)
+        if (steps[j] < 1 || (j > 0 && steps[j] <= steps[j - 1])) {
+            set_error("steps must be strictly increasing ints >= 1 (steps[%d]=%d)", j, steps[j]);
+            return false;
+        }
+    return true;
+}
+
+// The alignment of the non-null pointers, the launch grid, the overlaps (`in` are read and `outs` written; null entries are
+// absent buffers), then the workspace: the checks of an aggregation entry after its mandatory pointers and arguments
+static int check_agg_buffers(int B, int C, std::vector<Buf> in, std::vector<Buf> outs, const void* ws, size_t ws_bytes,
+                             size_t need) {
+    uintptr_t bits = 0;
+    for (auto* set : {&in, &outs}) {
+        std::vector<Buf> kept;
+        for (const Buf& b : *set)
+            if (b.p) {
+                bits |= reinterpret_cast<uintptr_t>(b.p);
+                kept.push_back(b);
+            }
+        *set = kept;
+    }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if ((long long)B * C > 65535) { set_error("2D aggregation: B*C=%lld exceeds gridDim.z", (long long)B * C); return CSPN_ERR_UNSUPPORTED; }
+    const int rc = check_disjoint(in, outs);
+    if (rc != CSPN_OK) return rc;
+    if (!ws || ws_bytes < need) {
+        set_error("2D aggregation needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    return CSPN_OK;
+}
+
+size_t cspn2d_agg_workspace_bytes(int B, int C, int H, int W, int K, const int* steps, int n_steps, int keep) {
+    if (!agg_args_ok(B, C, H, W, K, K * K - 1, steps, n_steps, 0, keep)) return 0;
+    return aggregate2d_workspace_bytes(B, C, H, W, K, keep);
+}
+
+size_t cspn2d_agg_bwd_workspace_bytes(int B, int C, int H, int W, int K, const int* steps, int n_steps, int keep) {
+    if (!agg_args_ok(B, C, H, W, K, K * K - 1, steps, n_steps, 0, keep)) return 0;
+    return aggregate2d_bwd_workspace_bytes(B, C, H, W, K, steps[n_steps - 1], keep);
+}
+
+int cspn2d_agg_fwd_f32(const float* guidance, const float* blur, const float* sparse, const float* step_weight, float* out, int B,
+                       int C, int H, int W, int guidance_channels, int K, const int* steps, int n_steps, int norm_type, int keep,
+                       void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!guidance || !blur || !step_weight || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!agg_args_ok(B, C, H, W, K, guidance_channels, steps, n_steps, norm_type, keep)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const size_t need = aggregate2d_workspace_bytes(B, C, H, W, K, keep && sparse);
+    const int rc = check_agg_buffers(B, C,
+                                     {{guidance, span_bytes(B, guidance_channels, hw), "guidance"}, {blur, span_bytes(B, C, hw), "blur"},
+                                      {sparse, span_bytes(B, 1, hw), "sparse"}, {step_weight, span_bytes(B, n_steps, hw), "step_weight"}},
+                                     {{out, span_bytes(B, C, hw), "out"}, {workspace, need, "the workspace"}}, workspace,
+                                     workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        Problem2D p{guidance, blur, sparse, out, B, C, H, W, guidance_channels, steps[n_steps - 1], norm_type == CSPN_NORM_8SUM_ABS};
+        p.keep = keep && sparse;
+        return aggregate2d_forward(p, K, step_weight, steps, n_steps, workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn2d_agg_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* step_weight, const float* grad_out,
+                       float* grad_guidance, float* grad_blur, float* grad_sparse, float* grad_step_weight, int B, int C, int H,
+                       int W, int guidance_channels, int K, const int* steps, int n_steps, int norm_type, int keep, void* workspace,
+                       size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!guidance || !blur || !step_weight || !grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!agg_args_ok(B, C, H, W, K, guidance_channels, steps, n_steps, norm_type, keep)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_g = span_bytes(B, guidance_channels, hw), n_d = span_bytes(B, C, hw), n_s = span_bytes(B, 1, hw),
+                    n_w = span_bytes(B, n_steps, hw);
+    const size_t need = aggregate2d_bwd_workspace_bytes(B, C, H, W, K, steps[n_steps - 1], keep && sparse);
+    const int rc = check_agg_buffers(B, C,
+                                     {{guidance, n_g, "guidance"}, {blur, n_d, "blur"}, {sparse, n_s, "sparse"},
+                                      {step_weight, n_w, "step_weight"}, {grad_out, n_d, "grad_out"}},
+                                     {{grad_guidance, n_g, "grad_guidance"}, {grad_blur, n_d, "grad_blur"},
+                                      {grad_sparse, n_s, "grad_sparse"}, {grad_step_weight, n_w, "grad_step_weight"},
+                                      {workspace, need, "the workspace"}},
+                                     workspace, workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) -> int {
+        Problem2D p{guidance, blur, sparse, nullptr, B, C, H, W, guidance_channels, steps[n_steps - 1], norm_type == CSPN_NORM_8SUM_ABS};
+        p.keep = keep && sparse;
+        // the default mode's m = sign(sparse) is not differentiated (Affinity_PropagateK detaches it); no samples, no gradient
+        if (grad_sparse && !p.keep)
+            CSPN_CUDA_TRY(cudaMemsetAsync(grad_sparse, 0, (size_t)B * H * W * sizeof(float), (cudaStream_t)stream));
+        return aggregate2d_backward(p, K, step_weight, steps, n_steps, grad_out, grad_guidance, grad_blur, p.keep ? grad_sparse : nullptr,
+                                    grad_step_weight, workspace, workspace_bytes, (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

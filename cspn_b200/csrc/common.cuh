@@ -144,6 +144,16 @@ size_t widek_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters, F
 int widek_backward(const Problem2D& p, int K, Family family, const float* grad_out, float* grad_guidance, float* grad_blur,
                    void* ws, size_t ws_bytes, cudaStream_t stream, int* launches, float* grad_sparse = nullptr);
 
+// 2D aggregation of the normalised family (DESIGN.md section 4.20): out = sum_j step_weight[j] * d_{steps[j]}, p.iters =
+// steps[n_steps-1]; p.keep as above.  grad_* may be null
+size_t aggregate2d_workspace_bytes(int B, int C, int H, int W, int K, bool keep);
+size_t aggregate2d_bwd_workspace_bytes(int B, int C, int H, int W, int K, int N, bool keep);
+int aggregate2d_forward(const Problem2D& p, int K, const float* step_weight, const int* steps, int n_steps, void* ws,
+                        size_t ws_bytes, cudaStream_t stream, int* launches);
+int aggregate2d_backward(const Problem2D& p, int K, const float* step_weight, const int* steps, int n_steps, const float* grad_out,
+                         float* grad_guidance, float* grad_blur, float* grad_sparse, float* grad_step_weight, void* ws,
+                         size_t ws_bytes, cudaStream_t stream, int* launches);
+
 // volumes per launch group of the 3D paths: `planes` workspace planes per volume (27 for 3x3x3, K^3 for K x K x K)
 int group3d(int B, int C, int D, int H, int W, int iters, int planes);
 size_t generic3d_workspace_bytes(int B, int C, int D, int H, int W, int iters);

@@ -37,6 +37,12 @@
 // stores each result also to the same element of every peer GPU's gather buffer (NVLink stores) and / or to one NVLS
 // multicast address (multimem.st).  Only the last step of a launch group, the one that writes `out`, runs it; the
 // intermediate iterates never leave the GPU.
+//
+// Aggregation (CSPN++'s context-aware CSPN, DESIGN.md section 4.20), the normalised family at K in {3, 5, 7}:
+//   out = sum_j sw_j * d_{s_j}.  The forward's aggregated steps run stepk_agg_*_kernel, whose epilogue adds sw_j * d to
+// `out` (the accumulator); the backward recomputes d_1..d_N, writes the weight gradient and mu_N = sw_{T-1} * grad_out in
+// agg_gradw_kernel, injects sw_j * grad_out into the adjoint at the aggregated steps (adjk_inject_kernel), and runs the
+// gather above with mu_N as its last adjoint.
 #include <cstdlib>
 #include <cstring>
 
@@ -154,10 +160,14 @@ prepk_paddle_kernel(const float* __restrict__ guidance, float* __restrict__ wk, 
 // FAN: the result also goes to fan's destinations (the last step of a fused gather); fan is not read otherwise.
 constexpr int kVecTW = 64, kVecTH = 16;
 
-template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
-__global__ void __launch_bounds__(256)
-stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-                 float* __restrict__ dst, int C, int H, int W, const Fan fan) {
+// AGG (aggregation, DESIGN.md section 4.20; not with PADDLE, RAW or FAN): the step also adds lam * d_{t+1} to agg, the
+// running sum (first: agg = lam * d_{t+1}, agg not read); lam is plane j of the step weights [image][nw][H][W]; a null dst
+// stores no iterate (the last step).
+template <int R, bool PADDLE, bool RAW, bool FAN, bool AGG>
+__device__ __forceinline__ void stepk_vec_body(const float* __restrict__ wk, const float* __restrict__ d0,
+                                               const float* __restrict__ cur, float* __restrict__ dst, int C, int H, int W,
+                                               const Fan& fan, const float* __restrict__ lam, int nw, float* __restrict__ agg,
+                                               int first) {
     using T = Taps<R>;
     constexpr int SH = kVecTH + 2 * R, SQ = kVecTW / 4 + 2;
     __shared__ float4 tile[SH][SQ];
@@ -202,8 +212,34 @@ stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, con
     }
     const size_t o = (size_t)bc * HW + p;
     const float4 v = make_float4(acc0, acc1, acc2, acc3);
+    if constexpr (AGG) {
+        if (dst) *reinterpret_cast<float4*>(dst + o) = v;
+        const float4 l = __ldg(reinterpret_cast<const float4*>(lam + (size_t)(bc / C) * nw * HW + p));
+        float4 a = make_float4(__fmul_rn(l.x, v.x), __fmul_rn(l.y, v.y), __fmul_rn(l.z, v.z), __fmul_rn(l.w, v.w));
+        if (!first) {
+            const float4 q = *reinterpret_cast<const float4*>(agg + o);
+            a = make_float4(__fadd_rn(q.x, a.x), __fadd_rn(q.y, a.y), __fadd_rn(q.z, a.z), __fadd_rn(q.w, a.w));
+        }
+        *reinterpret_cast<float4*>(agg + o) = a;
+        return;
+    }
     *reinterpret_cast<float4*>(dst + o) = v;
     if constexpr (FAN) fan_store(fan, o, v);
+}
+
+template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
+__global__ void __launch_bounds__(256)
+stepk_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                 float* __restrict__ dst, int C, int H, int W, const Fan fan) {
+    stepk_vec_body<R, PADDLE, RAW, FAN, false>(wk, d0, cur, dst, C, H, W, fan, nullptr, 0, nullptr, 0);
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+stepk_agg_vec_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                     float* __restrict__ dst, const float* __restrict__ lam, int nw, float* __restrict__ agg, int first, int C,
+                     int H, int W) {
+    stepk_vec_body<R, false, false, false, true>(wk, d0, cur, dst, C, H, W, Fan{}, lam, nw, agg, first);
 }
 
 // ---- step / adjoint, one pixel per thread (any W, any alignment).  Tile 32 x 8 pixels + R halo --------------------
@@ -220,10 +256,12 @@ __device__ __forceinline__ void load_tile_scalar(float (*tile)[kSclTW + 2 * R], 
     }
 }
 
-template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
-__global__ void __launch_bounds__(256)
-stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
-                    float* __restrict__ dst, int C, int H, int W, const Fan fan) {
+// AGG: as in stepk_vec_body
+template <int R, bool PADDLE, bool RAW, bool FAN, bool AGG>
+__device__ __forceinline__ void stepk_scalar_body(const float* __restrict__ wk, const float* __restrict__ d0,
+                                                  const float* __restrict__ cur, float* __restrict__ dst, int C, int H, int W,
+                                                  const Fan& fan, const float* __restrict__ lam, int nw, float* __restrict__ agg,
+                                                  int first) {
     using T = Taps<R>;
     __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
     const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, bc = blockIdx.z;
@@ -238,16 +276,39 @@ stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, 
 #pragma unroll
     for (int k = 0; k < T::NT; ++k) acc = fmaf(__ldg(w + k * HW), tile[ty + R + T::dy(k)][tx + R + T::dx(k)], acc);
     const size_t o = (size_t)bc * HW + p;
+    if constexpr (AGG) {
+        if (dst) dst[o] = acc;
+        const float a = __fmul_rn(__ldg(lam + (size_t)(bc / C) * nw * HW + p), acc);
+        agg[o] = first ? a : __fadd_rn(agg[o], a);
+        return;
+    }
     dst[o] = acc;
     if constexpr (FAN) fan_store(fan, o, acc);
 }
 
+template <int R, bool PADDLE = false, bool RAW = false, bool FAN = false>
+__global__ void __launch_bounds__(256)
+stepk_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                    float* __restrict__ dst, int C, int H, int W, const Fan fan) {
+    stepk_scalar_body<R, PADDLE, RAW, FAN, false>(wk, d0, cur, dst, C, H, W, fan, nullptr, 0, nullptr, 0);
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+stepk_agg_scalar_kernel(const float* __restrict__ wk, const float* __restrict__ d0, const float* __restrict__ cur,
+                        float* __restrict__ dst, const float* __restrict__ lam, int nw, float* __restrict__ agg, int first, int C,
+                        int H, int W) {
+    stepk_scalar_body<R, false, false, false, true>(wk, d0, cur, dst, C, H, W, Fan{}, lam, nw, agg, first);
+}
+
 // lambda_t(q) = sum_k w'_k(q - off_k) lambda_{t+1}(q - off_k): the transposed stencil, source pixels inside the image only.
 // RAW: wk is the caller's gates, NT planes per image.
-template <int R, bool RAW = false>
-__global__ void __launch_bounds__(256)
-adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out, int C, int H,
-            int W) {
+// INJ (aggregation backward, mu_t of DESIGN.md section 4.20): then lam_out = lam_out + sw * grad_out, sw plane j of the step
+// weights [image][nw][H][W], each operation rounded on its own.
+template <int R, bool RAW, bool INJ>
+__device__ __forceinline__ void adjk_body(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out,
+                                          int C, int H, int W, const float* __restrict__ sw, int nw,
+                                          const float* __restrict__ grad_out) {
     using T = Taps<R>;
     __shared__ float tile[kSclTH + 2 * R][kSclTW + 2 * R];
     const int x0 = blockIdx.x * kSclTW, y0 = blockIdx.y * kSclTH, bc = blockIdx.z;
@@ -264,7 +325,55 @@ adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, floa
         if (inside(ys, xs, H, W))
             acc = fmaf(__ldg(w + k * HW + (size_t)ys * W + xs), tile[ty + R - T::dy(k)][tx + R - T::dx(k)], acc);
     }
-    lam_out[(size_t)bc * HW + (size_t)y * W + x] = acc;
+    const size_t p = (size_t)y * W + x;
+    if constexpr (INJ)
+        acc = __fadd_rn(acc, __fmul_rn(__ldg(sw + (size_t)(bc / C) * nw * HW + p), __ldg(grad_out + (size_t)bc * HW + p)));
+    lam_out[(size_t)bc * HW + p] = acc;
+}
+
+template <int R, bool RAW = false>
+__global__ void __launch_bounds__(256)
+adjk_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out, int C, int H,
+            int W) {
+    adjk_body<R, RAW, false>(wk, lam_in, lam_out, C, H, W, nullptr, 0, nullptr);
+}
+
+template <int R>
+__global__ void __launch_bounds__(256)
+adjk_inject_kernel(const float* __restrict__ wk, const float* __restrict__ lam_in, float* __restrict__ lam_out,
+                   const float* __restrict__ sw, int nw, const float* __restrict__ grad_out, int C, int H, int W) {
+    adjk_body<R, false, true>(wk, lam_in, lam_out, C, H, W, sw, nw, grad_out);
+}
+
+// The step-weight gradient and the last adjoint of the aggregation (DESIGN.md section 4.20), one pixel per thread, grid
+// z = image of the group: for the steps s_j, j = j0 .. j0+ns-1, of `sel`
+//   grad_sw[j](p) = sum_c grad_out[c](p) * d_{s_j}[c](p)     (c ascending from the first term; skipped when grad_sw is null)
+// and, when mu is non-null, mu[c](p) = sw[nw-1](p) * grad_out[c](p) = mu_N.  d_s is plane s-1 of `iters` (planes n floats
+// apart); every pointer is offset to the group's first image.
+constexpr int kAggStepsPerLaunch = 64;
+struct StepSel {
+    int s[kAggStepsPerLaunch];
+};
+
+__global__ void __launch_bounds__(256)
+agg_gradw_kernel(const float* __restrict__ grad_out, const float* __restrict__ iters, long long n, const float* __restrict__ sw,
+                 float* __restrict__ grad_sw, float* __restrict__ mu, const StepSel sel, int j0, int ns, int nw, int C,
+                 long long HW) {
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.z;
+    if (p >= HW) return;
+    const float* g = grad_out + (size_t)b * C * HW + p;
+    if (grad_sw)
+        for (int j = 0; j < ns; ++j) {
+            const float* d = iters + (size_t)(sel.s[j] - 1) * n + (size_t)b * C * HW + p;
+            float a = __fmul_rn(__ldg(g), __ldg(d));
+            for (int c = 1; c < C; ++c) a = __fadd_rn(a, __fmul_rn(__ldg(g + c * HW), __ldg(d + c * HW)));
+            grad_sw[((size_t)b * nw + j0 + j) * HW + p] = a;
+        }
+    if (mu) {
+        const float l = __ldg(sw + ((size_t)b * nw + nw - 1) * HW + p);
+        for (int c = 0; c < C; ++c) mu[(size_t)b * C * HW + c * HW + p] = __fmul_rn(l, __ldg(g + c * HW));
+    }
 }
 
 // Gw_k(p) = sum_t lambda_{t+1}(p) d_t(p + off_k) with d_t staged tile by tile, Gc = sum_t lambda_{t+1}; then the finalize
@@ -549,6 +658,131 @@ int backward_k(const Problem2D& p, const float* grad_out, float* grad_guidance, 
     return CSPN_OK;
 }
 
+// Aggregation (DESIGN.md section 4.20), the normalised family: out = sum_j sw_j * d_{s_j}, steps s_0 < ... < s_{nw-1} = N.
+// Workspace: the K*K weight planes, two ping-pong planes (out is the running sum, so no iterate is stored there), keep's d0'.
+template <int R>
+int aggregate_forward_k(const Problem2D& p, const float* sw, const int* steps, int nw, void* ws, cudaStream_t stream,
+                        int* launches) {
+    constexpr int NPL = Taps<R>::NP;
+    const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
+    float* wk_ws = static_cast<float*>(ws);
+    float* buf[2] = {wk_ws + (size_t)p.B * NPL * HW, wk_ws + (size_t)p.B * NPL * HW + (size_t)p.B * plane};
+    float* d0_all = buf[1] + (size_t)p.B * plane;
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(p.out) && aligned16(ws) && aligned16(sw);
+    const dim3 vgrid((p.W + kVecTW - 1) / kVecTW, (p.H + kVecTH - 1) / kVecTH), sgrid((p.W + kSclTW - 1) / kSclTW, (p.H + kSclTH - 1) / kSclTH);
+    const int G = group_size(p.B);
+    for (int b0 = 0; b0 < p.B; b0 += G) {
+        const int nimg = p.B - b0 < G ? p.B - b0 : G;
+        const size_t off = (size_t)b0 * plane;
+        const float* wk = wk_ws + (size_t)b0 * NPL * HW;
+        const float* blur = p.blur + off;
+        float* d0 = p.keep ? d0_all + off : nullptr;
+        if (p.keep)
+            launch_prep_keep(2 * R + 1, p.guidance + (size_t)b0 * p.gch * HW, p.sparse + (size_t)b0 * HW, blur, wk_ws + (size_t)b0 * NPL * HW,
+                             d0, nimg, p.C, p.H, p.W, p.gch, p.norm_abs, stream);
+        else
+            launch_prep<R, false>(p.guidance + (size_t)b0 * p.gch * HW, p.sparse ? p.sparse + (size_t)b0 * HW : nullptr,
+                                  wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+        ++*launches;
+        const float* cur = blur;
+        for (int t = 0, j = 0; t < p.iters; ++t) {           // d_{t+1} = step(d_t)
+            float* dst = t + 1 == p.iters ? nullptr : buf[t & 1] + off;
+            if (steps[j] == t + 1) {
+                const float* lam = sw + ((size_t)b0 * nw + j) * HW;
+                const int nbc = nimg * p.C;
+                if (vec)
+                    stepk_agg_vec_kernel<R><<<dim3(vgrid.x, vgrid.y, nbc), dim3(16, 16), 0, stream>>>(
+                            wk, p.keep ? d0 : blur, cur, dst, lam, nw, p.out + off, j == 0, p.C, p.H, p.W);
+                else
+                    stepk_agg_scalar_kernel<R><<<dim3(sgrid.x, sgrid.y, nbc), dim3(kSclTW, kSclTH), 0, stream>>>(
+                            wk, p.keep ? d0 : blur, cur, dst, lam, nw, p.out + off, j == 0, p.C, p.H, p.W);
+                ++j;
+            } else {
+                launch_step<R, false>(vec, wk, p.keep ? d0 : blur, cur, dst, nimg * p.C, p.C, p.H, p.W, stream);
+            }
+            ++*launches;
+            cur = dst;
+        }
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
+// Backward: prep, N forward steps that keep d_1..d_N, the step-weight gradient with mu_N = sw_{nw-1} * grad_out, N adjoint
+// steps mu_t = adj(mu_{t+1}) (+ sw_j * grad_out where t = s_j), and the gather of backward_k reading mu_N as its last adjoint.
+// Workspace: the weight planes, d_1..d_N, mu_0..mu_N, keep's d0'.
+template <int R>
+int aggregate_backward_k(const Problem2D& p, const float* sw, const int* steps, int nw, const float* grad_out, float* grad_guidance,
+                         float* grad_blur, float* grad_sparse, float* grad_sw, void* ws, cudaStream_t stream, int* launches) {
+    constexpr int NPL = Taps<R>::NP;
+    const int N = p.iters;
+    const size_t HW = (size_t)p.H * p.W, plane = (size_t)p.C * HW;
+    const long long n = (long long)p.B * plane;
+    float* wk_ws = static_cast<float*>(ws);
+    float* its = wk_ws + (size_t)p.B * NPL * HW;          // its[t] = d_{t+1}, t < N
+    float* lam = its + (size_t)N * n;                     // lam[t] = mu_t, t <= N
+    float* d0_all = lam + (size_t)(N + 1) * n;
+    const bool vec = p.W % 4 == 0 && aligned16(p.blur) && aligned16(ws);
+    const int G = group_size(p.B);
+    for (int b0 = 0; b0 < p.B; b0 += G) {
+        const int nimg = p.B - b0 < G ? p.B - b0 : G;
+        const size_t off = (size_t)b0 * plane;
+        const float* wk = wk_ws + (size_t)b0 * NPL * HW;
+        const float* blur = p.blur + off;
+        const float* guidance = p.guidance + (size_t)b0 * p.gch * HW;
+        const float* sparse = p.sparse ? p.sparse + (size_t)b0 * HW : nullptr;
+        const float* swg = sw + (size_t)b0 * nw * HW;
+        float* d0 = p.keep ? d0_all + off : nullptr;
+        if (p.keep)
+            launch_prep_keep(2 * R + 1, guidance, sparse, blur, wk_ws + (size_t)b0 * NPL * HW, d0, nimg, p.C, p.H, p.W, p.gch,
+                             p.norm_abs, stream);
+        else
+            launch_prep<R, false>(guidance, sparse, wk_ws + (size_t)b0 * NPL * HW, nimg, p.H, p.W, p.gch, p.norm_abs, stream);
+        ++*launches;
+        for (int t = 0; t < N; ++t) {
+            launch_step<R, false>(vec, wk, p.keep ? d0 : blur, t == 0 ? blur : its + (size_t)(t - 1) * n + off,
+                                  its + (size_t)t * n + off, nimg * p.C, p.C, p.H, p.W, stream);
+            ++*launches;
+        }
+        float* mu_n = lam + (size_t)N * n + off;
+        for (int j0 = 0; j0 < nw; j0 += kAggStepsPerLaunch) {
+            StepSel sel{};
+            const int ns = nw - j0 < kAggStepsPerLaunch ? nw - j0 : kAggStepsPerLaunch;
+            for (int j = 0; j < ns; ++j) sel.s[j] = steps[j0 + j];
+            agg_gradw_kernel<<<dim3((unsigned)((HW + 255) / 256), 1, nimg), 256, 0, stream>>>(
+                    grad_out + off, its + off, n, swg, grad_sw ? grad_sw + (size_t)b0 * nw * HW : nullptr,
+                    j0 + ns == nw ? mu_n : nullptr, sel, j0, ns, nw, p.C, (long long)HW);
+            ++*launches;
+        }
+        const dim3 grid((p.W + kSclTW - 1) / kSclTW, (p.H + kSclTH - 1) / kSclTH, nimg * p.C);
+        for (int t = N - 1, j = nw - 2; t >= 0; --t) {    // mu_t from mu_{t+1}
+            const float* lin = lam + (size_t)(t + 1) * n + off;
+            float* lout = lam + (size_t)t * n + off;
+            if (j >= 0 && steps[j] == t) {
+                adjk_inject_kernel<R><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lout, swg + (size_t)j * HW, nw,
+                                                                                 grad_out + off, p.C, p.H, p.W);
+                --j;
+            } else {
+                adjk_kernel<R, false><<<grid, dim3(kSclTW, kSclTH), 0, stream>>>(wk, lin, lout, p.C, p.H, p.W);
+            }
+            ++*launches;
+        }
+        float* gg = grad_guidance ? grad_guidance + (size_t)b0 * p.gch * HW : nullptr;
+        float* gb = grad_blur ? grad_blur + off : nullptr;
+        const dim3 ggrid(grid.x, grid.y, nimg);
+        if (p.keep)
+            gatherk_keep_kernel<R><<<ggrid, dim3(kSclTW, kSclTH), 0, stream>>>(
+                    guidance, blur, sparse, wk, its + off, lam + off, mu_n, gg, gb, grad_sparse ? grad_sparse + (size_t)b0 * HW : nullptr,
+                    n, N, p.C, p.H, p.W, p.gch, p.norm_abs);
+        else
+            gatherk_kernel<R, false, false><<<ggrid, dim3(kSclTW, kSclTH), 0, stream>>>(
+                    guidance, blur, sparse, wk, its + off, lam + off, mu_n, gg, gb, n, N, p.C, p.H, p.W, p.gch, p.norm_abs);
+        ++*launches;
+    }
+    CSPN_CUDA_TRY(cudaGetLastError());
+    return CSPN_OK;
+}
+
 // What the three families' fronts do differently; their kernels differ by the PADDLE / RAW flags (see with_kernels)
 struct FamilyTraits {
     const char* name;        // follows "KxK 2D" in messages
@@ -653,6 +887,40 @@ int widek_backward(const Problem2D& p, int K, Family family, const float* grad_o
     if (t.no_grad_is_no_op && !grad_guidance && !grad_blur) return CSPN_OK;
     return with_kernels(K, family, [&](auto R, auto PADDLE, auto RAW) {
         return backward_k<R(), PADDLE(), RAW()>(p, grad_out, grad_guidance, grad_blur, ws, stream, launches, grad_sparse);
+    });
+}
+
+size_t aggregate2d_workspace_bytes(int B, int C, int H, int W, int K, bool keep) {
+    const size_t HW = (size_t)H * W;
+    return sizeof(float) * ((size_t)B * K * K * HW + (keep ? 3 : 2) * (size_t)B * C * HW);
+}
+
+size_t aggregate2d_bwd_workspace_bytes(int B, int C, int H, int W, int K, int N, bool keep) {
+    const size_t HW = (size_t)H * W;
+    return sizeof(float) * ((size_t)B * K * K * HW + (2 * (size_t)N + 1 + (keep ? 1 : 0)) * B * C * HW);
+}
+
+int aggregate2d_forward(const Problem2D& p, int K, const float* step_weight, const int* steps, int n_steps, void* ws,
+                        size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const int rc = check_launch(p, K, traits(Family::Normalised), "aggregation",
+                                aggregate2d_workspace_bytes(p.B, p.C, p.H, p.W, K, p.keep), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    return with_kernels(K, Family::Normalised, [&](auto R, auto, auto) {
+        return aggregate_forward_k<R()>(p, step_weight, steps, n_steps, ws, stream, launches);
+    });
+}
+
+int aggregate2d_backward(const Problem2D& p, int K, const float* step_weight, const int* steps, int n_steps, const float* grad_out,
+                         float* grad_guidance, float* grad_blur, float* grad_sparse, float* grad_step_weight, void* ws,
+                         size_t ws_bytes, cudaStream_t stream, int* launches) {
+    const int rc = check_launch(p, K, traits(Family::Normalised), "aggregation backward",
+                                aggregate2d_bwd_workspace_bytes(p.B, p.C, p.H, p.W, K, p.iters, p.keep), ws, ws_bytes);
+    if (rc != CSPN_OK) return rc;
+    if (grad_guidance)   // channels >= K*K-1 and taps that read the padding get no store, as in widek_backward
+        CSPN_CUDA_TRY(cudaMemsetAsync(grad_guidance, 0, (size_t)p.B * p.gch * p.H * p.W * sizeof(float), stream));
+    return with_kernels(K, Family::Normalised, [&](auto R, auto, auto) {
+        return aggregate_backward_k<R()>(p, step_weight, steps, n_steps, grad_out, grad_guidance, grad_blur, grad_sparse,
+                                         grad_step_weight, ws, stream, launches);
     });
 }
 

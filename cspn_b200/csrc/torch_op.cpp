@@ -19,6 +19,13 @@
 //   propagate2d_keep_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size,
 //                             int prop_time, int norm_type, bool need_guidance, bool need_blur, bool need_sparse)
 //       -> (Tensor, Tensor, Tensor)
+//   propagate2d_aggregate(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor step_weight, int[] steps,
+//                         int kernel_size, int norm_type, bool keep) -> Tensor
+//       (CSPN++'s context-aware CSPN: sum_j step_weight[:, j] * d_{steps[j]}, K in {3, 5, 7}, keep the keep-sparse mode)
+//   propagate2d_aggregate_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor step_weight,
+//                                  Tensor grad_out, int[] steps, int kernel_size, int norm_type, bool keep,
+//                                  bool need_guidance, bool need_blur, bool need_sparse, bool need_step_weight)
+//       -> (Tensor, Tensor, Tensor, Tensor)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -259,6 +266,56 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor> propagate2d_keep_backward_cuda(
                                  (int)K, (int)prop_time, (int)norm_type, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_keep_bwd_f32");
     return {grad_or_empty(gg, g), grad_or_empty(gd, d), grad_or_empty(gs, d)};
+}
+
+// Aggregation of the steps, K in {3, 5, 7}: cspn2d_agg_*_f32.  step_weight (B, T, H, W) with T = len(steps)
+std::vector<int> check2d_agg(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                             const at::Tensor& step_weight, at::IntArrayRef steps, int64_t K) {
+    check2d_k(guidance, blur, sparse, K);
+    TORCH_CHECK(!steps.empty(), "steps must hold at least one step");
+    for (size_t j = 0; j < steps.size(); ++j)
+        TORCH_CHECK(steps[j] >= 1 && steps[j] <= INT32_MAX && (j == 0 || steps[j] > steps[j - 1]),
+                    "steps must be strictly increasing ints >= 1, got ", steps);
+    TORCH_CHECK(step_weight.dim() == 4 && step_weight.size(0) == blur.size(0) && step_weight.size(1) == (int64_t)steps.size() &&
+                    step_weight.size(2) == blur.size(2) && step_weight.size(3) == blur.size(3),
+                "step_weight must be (B, len(steps), H, W), got ", step_weight.sizes());
+    TORCH_CHECK(step_weight.scalar_type() == at::kFloat && step_weight.device() == blur.device(),
+                "step_weight must be fp32 on the device of blur_depth");
+    return std::vector<int>(steps.begin(), steps.end());
+}
+
+at::Tensor propagate2d_aggregate_cuda(const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                                      const at::Tensor& step_weight, at::IntArrayRef steps, int64_t K, int64_t norm_type, bool keep) {
+    const std::vector<int> st = check2d_agg(guidance, blur, sparse, step_weight, steps, K);
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), w = step_weight.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(d);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3), T = (int)st.size();
+    const Workspace ws(cspn2d_agg_workspace_bytes(B, C, H, W, (int)K, st.data(), T, keep), d);
+    check_rc(cspn2d_agg_fwd_f32(fptr(g), fptr(d), fptr(s), fptr(w), mptr(out), B, C, H, W, (int)g.size(1), (int)K, st.data(), T,
+                                (int)norm_type, keep, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_agg_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_aggregate_backward_cuda(
+        const at::Tensor& guidance, const at::Tensor& blur, const std::optional<at::Tensor>& sparse, const at::Tensor& step_weight,
+        const at::Tensor& grad_out, at::IntArrayRef steps, int64_t K, int64_t norm_type, bool keep, bool need_g, bool need_d,
+        bool need_s, bool need_w) {
+    const std::vector<int> st = check2d_agg(guidance, blur, sparse, step_weight, steps, K);
+    check_grad_out(grad_out, blur, "blur_depth");
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor g = guidance.contiguous(), d = blur.contiguous(), w = step_weight.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor gg = new_grad(need_g, g), gd = new_grad(need_d, d), gs = s.defined() ? new_grad(need_s, s) : at::Tensor(),
+               gw = new_grad(need_w, w);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3), T = (int)st.size();
+    const Workspace ws(cspn2d_agg_bwd_workspace_bytes(B, C, H, W, (int)K, st.data(), T, keep), d);
+    check_rc(cspn2d_agg_bwd_f32(fptr(g), fptr(d), fptr(s), fptr(w), fptr(go), mptr(gg), mptr(gd), mptr(gs), mptr(gw), B, C, H, W,
+                                (int)g.size(1), (int)K, st.data(), T, (int)norm_type, keep, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_agg_bwd_f32");
+    return {grad_or_empty(gg, g), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gw, w)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -882,6 +939,11 @@ TORCH_LIBRARY(cspn_b200, m) {
           "int norm_type, int algo) -> Tensor");
     m.def("propagate2d_keep_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor grad_out, int kernel_size, "
           "int prop_time, int norm_type, bool need_guidance, bool need_blur, bool need_sparse) -> (Tensor, Tensor, Tensor)");
+    m.def("propagate2d_aggregate(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor step_weight, int[] steps, "
+          "int kernel_size, int norm_type, bool keep) -> Tensor");
+    m.def("propagate2d_aggregate_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor step_weight, "
+          "Tensor grad_out, int[] steps, int kernel_size, int norm_type, bool keep, bool need_guidance, bool need_blur, "
+          "bool need_sparse, bool need_step_weight) -> (Tensor, Tensor, Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -926,6 +988,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_k_backward", &propagate2d_k_backward_cuda);
     m.impl("propagate2d_keep", &propagate2d_keep_cuda);
     m.impl("propagate2d_keep_backward", &propagate2d_keep_backward_cuda);
+    m.impl("propagate2d_aggregate", &propagate2d_aggregate_cuda);
+    m.impl("propagate2d_aggregate_backward", &propagate2d_aggregate_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

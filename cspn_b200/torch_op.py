@@ -100,6 +100,45 @@ def _register():
 
     lib.register_autograd('cspn_b200::propagate2d_keep', backward2d_keep, setup_context=setup2d_keep)
 
+    @lib.register_fake('cspn_b200::propagate2d_aggregate')
+    def _(guidance, blur_depth, sparse_depth, step_weight, steps, kernel_size, norm_type, keep):
+        torch._check(guidance.dim() == 4 and blur_depth.dim() == 4, lambda: 'guidance and blur_depth must be (B,C,H,W)')
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        torch._check(guidance.shape[1] >= kernel_size * kernel_size - 1,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs >= {kernel_size * kernel_size - 1} guidance channels')
+        torch._check(len(steps) >= 1 and all(s >= 1 for s in steps) and all(a < b for a, b in zip(steps, steps[1:])),
+                     lambda: 'steps must be strictly increasing ints >= 1')
+        torch._check(step_weight.dim() == 4 and step_weight.shape[1] == len(steps), lambda: 'step_weight must be (B, len(steps), H, W)')
+        return torch.empty_like(blur_depth, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_aggregate_backward')
+    def _(guidance, blur_depth, sparse_depth, step_weight, grad_out, steps, kernel_size, norm_type, keep, need_guidance,
+          need_blur, need_sparse, need_step_weight):
+        gg = torch.empty_like(guidance, memory_format=torch.contiguous_format) if need_guidance else guidance.new_empty(0)
+        gd = torch.empty_like(blur_depth, memory_format=torch.contiguous_format) if need_blur else blur_depth.new_empty(0)
+        gs = (torch.empty_like(sparse_depth, memory_format=torch.contiguous_format) if need_sparse and sparse_depth is not None
+              else blur_depth.new_empty(0))
+        gw = torch.empty_like(step_weight, memory_format=torch.contiguous_format) if need_step_weight else step_weight.new_empty(0)
+        return gg, gd, gs, gw
+
+    def setup2d_aggregate(ctx, inputs, output):
+        guidance, blur_depth, sparse_depth, step_weight, steps, kernel_size, norm_type, keep = inputs
+        ctx.save_for_backward(guidance, blur_depth, sparse_depth, step_weight)
+        ctx.cfg = (steps, kernel_size, norm_type, keep)
+
+    def backward2d_aggregate(ctx, grad_out):
+        guidance, blur_depth, sparse_depth, step_weight = ctx.saved_tensors
+        steps, kernel_size, norm_type, keep = ctx.cfg
+        need_g, need_d, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[3]
+        need_s = bool(keep) and ctx.needs_input_grad[2]     # the default mode's sign(sparse) is not differentiated
+        gg, gd, gs, gw = torch.ops.cspn_b200.propagate2d_aggregate_backward(
+            guidance, blur_depth, sparse_depth, step_weight, grad_out.contiguous(), steps, kernel_size, norm_type, keep, need_g,
+            need_d, need_s, need_w)
+        return ((gg if need_g else None), (gd if need_d else None), (gs if need_s else None), (gw if need_w else None),
+                None, None, None, None)
+
+    lib.register_autograd('cspn_b200::propagate2d_aggregate', backward2d_aggregate, setup_context=setup2d_aggregate)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

@@ -196,6 +196,40 @@ CSPN_API int cspn2d_keep_bwd_f32(const float* guidance, const float* blur, const
                         int guidance_channels, int K, int iters, int norm_type,
                         void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D aggregation of the steps, K in {3, 5, 7}: CSPN++'s context-aware CSPN (DESIGN.md section 4.20) --------------
+ * d_0 = blur and d_{t+1} the step of cspn2d_k_fwd_f32 (keep = 0; sparse may be NULL) or of cspn2d_keep_fwd_f32 (keep = 1;
+ * a NULL sparse gives the keep = 0 bits), every K on the K x K kernels; then, for the steps s_0 < ... < s_{T-1}
+ * (steps, a HOST array of T = n_steps ints >= 1, strictly increasing; N = s_{T-1} steps run)
+ *   out[b][c](p) = sum_j step_weight[b][j](p) * d_{s_j}[b][c](p)
+ * summed over j ascending from the first term, every product and sum rounded on its own.  step_weight [B][T][H][W] is
+ * used as given (no |.|, no normalisation) and shared by the C channels; a zero weight does not hide a NaN or an infinite
+ * iterate (0 * inf = NaN).  guidance, blur, sparse, out, guidance_channels and norm_type as in the K x K calls above.
+ * The backward writes grad_guidance [B][guidance_channels][H][W] (zero-filled first, as cspn2d_k_bwd_f32 does),
+ * grad_blur [B][C][H][W], grad_sparse [B][1][H][W] (keep mode with a sparse: m * sum_c Gc_c as in cspn2d_keep_bwd_f32;
+ * zero otherwise) and grad_step_weight [B][T][H][W] = sum_c grad_out[b][c](p) * d_{s_j}[b][c](p), c ascending from the
+ * first term; any of the four may be NULL.
+ * Workspace (floats; the queries return bytes, 0 for invalid arguments): forward B*K*K*H*W + (2 + keep)*B*C*H*W,
+ * backward B*K*K*H*W + (2N + 1 + keep)*B*C*H*W, neither dependent on the device.  Launches: forward 1 + N, backward
+ * 2 + 2N + ceil(T / 64).  No atomics; the only memsets are those of the K x K backward.
+ * CSPN_ERR_INVALID_ARGUMENT for a null guidance / blur / step_weight / out (grad_out in the backward), a non-positive
+ * shape, K not in {3, 5, 7}, guidance_channels < K*K-1, an unknown norm, keep not 0 or 1, n_steps < 1, a null steps, steps
+ * not strictly increasing or < 1, a pointer that is not 4-byte aligned, and an output (the workspace included) that
+ * overlaps an input or another output; CSPN_ERR_UNSUPPORTED for B*C > 65535; CSPN_ERR_WORKSPACE for a missing or short
+ * workspace.  All of these come before any device work. */
+CSPN_API size_t cspn2d_agg_workspace_bytes(int B, int C, int H, int W, int K, const int* steps, int n_steps, int keep);
+
+CSPN_API int cspn2d_agg_fwd_f32(const float* guidance, const float* blur, const float* sparse, const float* step_weight,
+                       float* out, int B, int C, int H, int W, int guidance_channels, int K, const int* steps,
+                       int n_steps, int norm_type, int keep, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_agg_bwd_workspace_bytes(int B, int C, int H, int W, int K, const int* steps, int n_steps, int keep);
+
+CSPN_API int cspn2d_agg_bwd_f32(const float* guidance, const float* blur, const float* sparse, const float* step_weight,
+                       const float* grad_out, float* grad_guidance, float* grad_blur, float* grad_sparse,
+                       float* grad_step_weight, int B, int C, int H, int W, int guidance_channels, int K,
+                       const int* steps, int n_steps, int norm_type, int keep, void* workspace, size_t workspace_bytes,
+                       cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
