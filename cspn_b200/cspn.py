@@ -604,6 +604,128 @@ def propagate2d_aggregate(guidance, blur_depth, step_weight, sparse_depth=None, 
     return _aggregate_fwd(guidance, blur_depth, step_weight, sparse_depth, prop_kernel, code, keep, steps)
 
 
+# ---- non-local 2D propagation: NLSPN's (DESIGN.md section 4.21) ----------------------------------------------------------
+def _check_nonlocal(feat, offset, affinity, sparse_depth, prop_kernel, prop_time):
+    """The checks of propagate2d_nonlocal; every refusal comes before anything is allocated or narrowed to int."""
+    if prop_kernel not in (3, 5, 7) or isinstance(prop_kernel, bool):
+        raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+    if isinstance(prop_time, bool) or not isinstance(prop_time, int) or not 0 <= prop_time <= 2 ** 31 - 1:
+        raise ValueError(f'prop_time must be an int >= 0, got {prop_time!r}')
+    T = prop_kernel * prop_kernel - 1
+    if feat.dim() != 4 or min(feat.shape) < 1:
+        raise ValueError(f'feat must be a non-empty (B,C,H,W), got {tuple(feat.shape)}')
+    B, C, H, W = feat.shape
+    if tuple(offset.shape) != (B, 2 * T, H, W):
+        raise ValueError(f'offset must be (B, 2T, H, W) = {(B, 2 * T, H, W)}, got {tuple(offset.shape)}')
+    if tuple(affinity.shape) != (B, T, H, W):
+        raise ValueError(f'affinity must be (B, T, H, W) = {(B, T, H, W)}, got {tuple(affinity.shape)}')
+    if sparse_depth is not None and tuple(sparse_depth.shape) != (B, C, H, W):
+        raise ValueError(f'sparse_depth must have feat\'s shape {(B, C, H, W)}, got {tuple(sparse_depth.shape)}')
+    ts = [t for t in (feat, offset, affinity, sparse_depth) if t is not None]
+    if any(t.dtype != torch.float32 for t in ts):
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if any(t.device != feat.device for t in ts):
+        raise RuntimeError('feat, offset, affinity and sparse_depth must be on one device')
+    if B > 2 ** 31 - 1 or C > 2 ** 31 - 1 or H * W * T >= 2 ** 31:
+        raise _lib.CspnError(f'propagate2d_nonlocal takes B, C < 2^31 and H*W*T < 2^31, got feat {tuple(feat.shape)} at K={prop_kernel}')
+    if not feat.is_cuda:
+        raise _lib.CspnError('propagate2d_nonlocal takes CUDA tensors only (there is no host-buffer entry point for it)')
+
+
+def _nonlocal_fwd(feat, offset, affinity, sparse_depth, prop_kernel, prop_time):
+    """Forward only (no autograd) through cspn2d_nl_fwd_f32, on the current stream."""
+    L = _lib.lib()
+    f, o, a = feat.contiguous(), offset.contiguous(), affinity.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    B, C, H, W = f.shape
+    out = torch.empty_like(f)
+    with torch.cuda.device(f.device):
+        ws_bytes = L.cspn2d_nl_workspace_bytes(B, C, H, W, prop_kernel, prop_time)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+        rc = L.cspn2d_nl_fwd_f32(_ptr(f), _ptr(o), _ptr(a), _ptr(s), _ptr(out), B, C, H, W, prop_kernel, prop_time, _ptr(ws), ws_bytes,
+                                 _stream(f.device))
+    _lib.check(rc, 'cspn2d_nl_fwd_f32')
+    return out
+
+
+class _Propagate2dNonlocalFn(torch.autograd.Function):
+    """autograd seam of propagate2d_nonlocal without the torch-op shim: native forward + native backward
+    (cspn2d_nl_bwd_f32), differentiable in feat, offset, affinity and sparse_depth."""
+
+    @staticmethod
+    def forward(ctx, feat, offset, affinity, sparse_depth, prop_kernel, prop_time):
+        ctx.save_for_backward(feat, offset, affinity, sparse_depth)
+        ctx.cfg = (prop_kernel, prop_time)
+        return _nonlocal_fwd(feat, offset, affinity, sparse_depth, prop_kernel, prop_time)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        feat, offset, affinity, sparse_depth = ctx.saved_tensors
+        prop_kernel, prop_time = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        f, o, a, go = feat.contiguous(), offset.contiguous(), affinity.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        need_f, need_o, need_a, need_s = ctx.needs_input_grad[:4]
+        need_s = need_s and s is not None
+        gf = torch.empty_like(f) if need_f else None
+        gof = torch.empty_like(o) if need_o else None
+        ga = torch.empty_like(a) if need_a else None
+        gs = torch.empty_like(s) if need_s else None
+        B, C, H, W = f.shape
+        with torch.cuda.device(f.device):
+            ws_bytes = L.cspn2d_nl_bwd_workspace_bytes(B, C, H, W, prop_kernel, prop_time)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=f.device) if ws_bytes else None
+            rc = L.cspn2d_nl_bwd_f32(_ptr(f), _ptr(o), _ptr(a), _ptr(s), _ptr(go), _ptr(gf), _ptr(gof), _ptr(ga), _ptr(gs), B, C, H, W,
+                                     prop_kernel, prop_time, _ptr(ws), ws_bytes, _stream(f.device))
+        _lib.check(rc, 'cspn2d_nl_bwd_f32')
+        return gf, gof, ga, gs, None, None
+
+
+def propagate2d_nonlocal(feat, offset, affinity, sparse_depth=None, prop_kernel=3, prop_time=18):
+    """NLSPN's non-local 2D propagation (Park et al., ECCV 2020): each of a pixel's T = K*K - 1 neighbours sits at a learned,
+    fractional offset from its grid position and is read by bilinear sampling (torchvision's deform_conv2d sampling).
+    feat (B, C, H, W) is h_0; offset (B, 2T, H, W) holds (dy, dx) of tap k in channels 2k, 2k + 1; affinity (B, T, H, W)
+    the weights a_k, used as given (normalise them before the call) and shared by the C channels; sparse_depth, of feat's
+    shape, or None.  All fp32 CUDA tensors; prop_kernel K in {3, 5, 7}.  Tap k runs over (i, j) in [0, K)^2 in raster order
+    without the centre, base offset (i - R, j - R), R = (K - 1) // 2: torchvision's and DCN's order, the reverse of the
+    K x K propagation's (R - t, R - l).  prop_time steps of
+        h_{t+1}(p) = a_c(p) h~_t(p) + sum_k a_k(p) S(h~_t, p + base_k + offset_k(p)),  a_c = 1 - sum_k a_k,
+    where h~_t = (1 - m) h_t + m sparse_depth with m = 1[sparse_depth > 0] (h~_t = h_t without it); the result h_N is not
+    replaced.  One step is deform_conv2d(h~_t, offset with a zero centre, ones(C, 1, K, K), padding=R, mask=affinity with
+    a_c at the centre) with groups = C.  Differentiable in feat, offset, affinity and sparse_depth, with a deterministic
+    backward (no floating-point atomics).  prop_time == 0 returns feat itself.  DESIGN.md section 4.21."""
+    _check_nonlocal(feat, offset, affinity, sparse_depth, prop_kernel, prop_time)
+    if prop_time == 0:
+        return feat
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.propagate2d_nonlocal(feat, offset, affinity, sparse_depth, prop_kernel, prop_time)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (feat, offset, affinity, sparse_depth)):
+        return _Propagate2dNonlocalFn.apply(feat, offset, affinity, sparse_depth, prop_kernel, prop_time)
+    return _nonlocal_fwd(feat, offset, affinity, sparse_depth, prop_kernel, prop_time)
+
+
+class Affinity_PropagateNonLocal(nn.Module):
+    """NLSPN's non-local propagation as a module: forward(feat, offset, affinity, sparse_depth=None) is
+    propagate2d_nonlocal(feat, offset, affinity, sparse_depth, prop_kernel, prop_time).  No parameters, no buffers: the
+    offsets and affinities come from the caller's guidance network (INTEGRATION.md section 2f)."""
+
+    def __init__(self, prop_time, prop_kernel=3):
+        super().__init__()
+        if prop_kernel not in (3, 5, 7):
+            raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+
+    def forward(self, feat, offset, affinity, sparse_depth=None):
+        return propagate2d_nonlocal(feat, offset, affinity, sparse_depth, self.prop_kernel, self.prop_time)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'
+
+
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
 KERNEL_SIZES_3D = (3, 5)
 

@@ -1247,6 +1247,103 @@ int cspn2d_agg_bwd_f32(const float* guidance, const float* blur, const float* sp
     });
 }
 
+// ---- 2D non-local propagation, NLSPN's (DESIGN.md section 4.21): cspn2d_nonlocal.cu ----------------------------------------
+// The sizes, K and the step count: true when they are valid (the error is set otherwise)
+static bool nl_args_ok(int B, int C, int H, int W, int K, int iters) {
+    if (!positive(B, C, H, W)) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (!kernel_size_ok(2, K)) { set_error("2D kernel size must be 3, 5 or 7, got %d", K); return false; }
+    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return false; }
+    return true;
+}
+
+// The alignment of the non-null pointers, the launch limits, the overlaps (`in` are read and `outs` written; null entries
+// are absent buffers), then the workspace (none needed when need is 0)
+static int check_nl_buffers(int B, int C, int H, int W, int K, std::vector<Buf> in, std::vector<Buf> outs, const void* ws,
+                            size_t ws_bytes, size_t need) {
+    uintptr_t bits = 0;
+    for (auto* set : {&in, &outs}) {
+        std::vector<Buf> kept;
+        for (const Buf& b : *set)
+            if (b.p) {
+                bits |= reinterpret_cast<uintptr_t>(b.p);
+                kept.push_back(b);
+            }
+        *set = kept;
+    }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!nonlocal2d_launchable(B, C, H, W, K, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    const int rc = check_disjoint(in, outs);
+    if (rc != CSPN_OK) return rc;
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("the non-local propagation needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    return CSPN_OK;
+}
+
+size_t cspn2d_nl_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!nl_args_ok(B, C, H, W, K, iters)) return 0;
+    return nonlocal2d_workspace_bytes(B, C, H, W, iters);
+}
+
+size_t cspn2d_nl_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!nl_args_ok(B, C, H, W, K, iters)) return 0;
+    const char* why = "";
+    if (!nonlocal2d_launchable(B, C, H, W, K, &why)) return 0;
+    return nonlocal2d_bwd_workspace_bytes(B, C, H, W, K, iters);
+}
+
+int cspn2d_nl_fwd_f32(const float* feat, const float* offset, const float* affinity, const float* sparse, float* out, int B, int C,
+                      int H, int W, int K, int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!feat || !offset || !affinity || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!nl_args_ok(B, C, H, W, K, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W, T = (long long)K * K - 1;
+    const uintptr_t n_f = span_bytes(B, C, hw);
+    const size_t need = nonlocal2d_workspace_bytes(B, C, H, W, iters);
+    const int rc = check_nl_buffers(B, C, H, W, K,
+                                    {{feat, n_f, "feat"}, {offset, span_bytes(B, (int)(2 * T), hw), "offset"},
+                                     {affinity, span_bytes(B, (int)T, hw), "affinity"}, {sparse, n_f, "sparse"}},
+                                    {{out, n_f, "out"}, {need ? workspace : nullptr, need, "the workspace"}}, workspace,
+                                    workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return nonlocal2d_forward(feat, offset, affinity, sparse, out, B, C, H, W, K, iters, workspace, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn2d_nl_bwd_f32(const float* feat, const float* offset, const float* affinity, const float* sparse, const float* grad_out,
+                      float* grad_feat, float* grad_offset, float* grad_affinity, float* grad_sparse, int B, int C, int H, int W, int K,
+                      int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!feat || !offset || !affinity || !grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!nl_args_ok(B, C, H, W, K, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    if (grad_sparse && !sparse) { set_error("grad_sparse needs a sparse input"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const long long hw = (long long)H * W, T = (long long)K * K - 1;
+    const uintptr_t n_f = span_bytes(B, C, hw), n_o = span_bytes(B, (int)(2 * T), hw), n_a = span_bytes(B, (int)T, hw);
+    const std::vector<Buf> in{{feat, n_f, "feat"}, {offset, n_o, "offset"}, {affinity, n_a, "affinity"}, {sparse, n_f, "sparse"},
+                              {grad_out, n_f, "grad_out"}};
+    const std::vector<Buf> outs{{grad_feat, n_f, "grad_feat"}, {grad_offset, n_o, "grad_offset"}, {grad_affinity, n_a, "grad_affinity"},
+                                {grad_sparse, n_f, "grad_sparse"}};
+    int rc = check_nl_buffers(B, C, H, W, K, in, outs, nullptr, 0, 0);
+    if (rc != CSPN_OK) return rc;
+    // the radix sort sizes its scratch for the current device's architecture: the one query that needs the CUDA runtime
+    const size_t need = iters > 0 ? nonlocal2d_bwd_workspace_bytes(B, C, H, W, K, iters) : 0;
+    if (iters > 0 && need == 0) { set_error("cannot size the backward's workspace (no CUDA device?)"); return CSPN_ERR_CUDA; }
+    if (need) {
+        std::vector<Buf> all;
+        for (const Buf& b : in) if (b.p) all.push_back(b);
+        for (const Buf& b : outs) if (b.p) all.push_back(b);
+        rc = check_nl_buffers(B, C, H, W, K, all, {{workspace, need, "the workspace"}}, workspace, workspace_bytes, need);
+        if (rc != CSPN_OK) return rc;
+    }
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return nonlocal2d_backward(feat, offset, affinity, sparse, grad_out, grad_feat, grad_offset, grad_affinity, grad_sparse, B, C,
+                                   H, W, K, iters, workspace, (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

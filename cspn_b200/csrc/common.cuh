@@ -250,4 +250,17 @@ int affinity_atrous_backward(const float* feat, const float* gate, const float* 
                              float* grad_gate, int B, int C, int H, int W, int L, const int* dilations, void* ws, cudaStream_t st,
                              int* launches);
 
+// Non-local 2D propagation, NLSPN's (cspn2d_nonlocal.cu): K in {3, 5, 7}, N steps of feat (B, C, H, W) with the learned
+// offsets (B, 2T, H, W) and affinities (B, T, H, W), sparse (B, C, H, W) or nullptr; arguments checked by the caller (sizes,
+// pointers, then launchable).  The forward's workspace is the h~ ping-pong; the backward's also holds every h~_t and
+// lambda~_t, the transposed index and the radix sort's scratch (0 when the sort cannot be sized)
+int nonlocal2d_launchable(int B, int C, int H, int W, int K, const char** why);
+size_t nonlocal2d_workspace_bytes(int B, int C, int H, int W, int N);
+size_t nonlocal2d_bwd_workspace_bytes(int B, int C, int H, int W, int K, int N);
+int nonlocal2d_forward(const float* feat, const float* offset, const float* affinity, const float* sparse, float* out, int B, int C,
+                       int H, int W, int K, int N, void* ws, cudaStream_t st, int* launches);
+int nonlocal2d_backward(const float* feat, const float* offset, const float* affinity, const float* sparse, const float* grad_out,
+                        float* grad_feat, float* grad_offset, float* grad_affinity, float* grad_sparse, int B, int C, int H, int W,
+                        int K, int N, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

@@ -26,6 +26,11 @@
 //                                  Tensor grad_out, int[] steps, int kernel_size, int norm_type, bool keep,
 //                                  bool need_guidance, bool need_blur, bool need_sparse, bool need_step_weight)
 //       -> (Tensor, Tensor, Tensor, Tensor)
+//   propagate2d_nonlocal(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, int kernel_size, int prop_time)
+//       -> Tensor   (NLSPN's non-local propagation: offset (B, 2T, H, W), affinity (B, T, H, W), T = K*K-1, K in {3, 5, 7})
+//   propagate2d_nonlocal_backward(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, Tensor grad_out,
+//                                 int kernel_size, int prop_time, bool need_feat, bool need_offset, bool need_affinity,
+//                                 bool need_sparse) -> (Tensor, Tensor, Tensor, Tensor)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -316,6 +321,65 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_aggregate
                                 (int)g.size(1), (int)K, st.data(), T, (int)norm_type, keep, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_agg_bwd_f32");
     return {grad_or_empty(gg, g), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gw, w)};
+}
+
+// Non-local propagation, K in {3, 5, 7}: cspn2d_nl_*_f32.  feat (B, C, H, W), offset (B, 2T, H, W), affinity (B, T, H, W),
+// sparse_depth of feat's shape
+void check2d_nl(const at::Tensor& feat, const at::Tensor& offset, const at::Tensor& affinity, const std::optional<at::Tensor>& sparse,
+                int64_t K, int64_t prop_time) {
+    TORCH_CHECK_VALUE(kernel_size_ok(K, 2), "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK_VALUE(prop_time >= 0 && prop_time <= INT32_MAX, "prop_time must be >= 0, got ", prop_time);
+    const int64_t T = neighbours(K, 2);
+    TORCH_CHECK_VALUE(feat.dim() == 4 && feat.numel() > 0, "feat must be a non-empty (B,C,H,W), got ", feat.sizes());
+    const int64_t B = feat.size(0), H = feat.size(2), W = feat.size(3);
+    TORCH_CHECK_VALUE(offset.dim() == 4 && offset.size(0) == B && offset.size(1) == 2 * T && offset.size(2) == H && offset.size(3) == W,
+                      "offset must be (B, 2T, H, W) = (", B, ", ", 2 * T, ", ", H, ", ", W, "), got ", offset.sizes());
+    TORCH_CHECK_VALUE(affinity.dim() == 4 && affinity.size(0) == B && affinity.size(1) == T && affinity.size(2) == H &&
+                          affinity.size(3) == W,
+                      "affinity must be (B, T, H, W) = (", B, ", ", T, ", ", H, ", ", W, "), got ", affinity.sizes());
+    TORCH_CHECK(feat.scalar_type() == at::kFloat && offset.scalar_type() == at::kFloat && affinity.scalar_type() == at::kFloat,
+                "cspn_b200 is fp32 only");
+    TORCH_CHECK(offset.device() == feat.device() && affinity.device() == feat.device(), "feat, offset and affinity are on different devices");
+    if (sparse.has_value()) {
+        TORCH_CHECK_VALUE(sparse->sizes() == feat.sizes(), "sparse_depth must have feat's shape ", feat.sizes(), ", got ", sparse->sizes());
+        TORCH_CHECK(sparse->scalar_type() == at::kFloat && sparse->device() == feat.device(), "sparse_depth must be fp32 on the device of feat");
+    }
+    TORCH_CHECK(B < ((int64_t)1 << 31) && feat.size(1) < ((int64_t)1 << 31) && H * W * T < ((int64_t)1 << 31),
+                "propagate2d_nonlocal takes B, C < 2^31 and H*W*T < 2^31, got feat ", feat.sizes(), " at K=", K);
+}
+
+at::Tensor propagate2d_nonlocal_cuda(const at::Tensor& feat, const at::Tensor& offset, const at::Tensor& affinity,
+                                     const std::optional<at::Tensor>& sparse, int64_t K, int64_t prop_time) {
+    check2d_nl(feat, offset, affinity, sparse, K, prop_time);
+    if (prop_time == 0) return feat.clone();           // a dispatcher op may not return its input
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), o = offset.contiguous(), a = affinity.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(f);
+    const int B = (int)f.size(0), C = (int)f.size(1), H = (int)f.size(2), W = (int)f.size(3);
+    const Workspace ws(cspn2d_nl_workspace_bytes(B, C, H, W, (int)K, (int)prop_time), f);
+    check_rc(cspn2d_nl_fwd_f32(fptr(f), fptr(o), fptr(a), fptr(s), mptr(out), B, C, H, W, (int)K, (int)prop_time, ws.ptr(), ws.bytes,
+                               current_stream()),
+             "cspn2d_nl_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_nonlocal_backward_cuda(
+        const at::Tensor& feat, const at::Tensor& offset, const at::Tensor& affinity, const std::optional<at::Tensor>& sparse,
+        const at::Tensor& grad_out, int64_t K, int64_t prop_time, bool need_f, bool need_o, bool need_a, bool need_s) {
+    check2d_nl(feat, offset, affinity, sparse, K, prop_time);
+    check_grad_out(grad_out, feat, "feat");
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor f = feat.contiguous(), o = offset.contiguous(), a = affinity.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    at::Tensor gf = new_grad(need_f, f), gof = new_grad(need_o, o), ga = new_grad(need_a, a),
+               gs = s.defined() ? new_grad(need_s, s) : at::Tensor();
+    const int B = (int)f.size(0), C = (int)f.size(1), H = (int)f.size(2), W = (int)f.size(3);
+    const Workspace ws(prop_time > 0 ? cspn2d_nl_bwd_workspace_bytes(B, C, H, W, (int)K, (int)prop_time) : 0, f);
+    check_rc(cspn2d_nl_bwd_f32(fptr(f), fptr(o), fptr(a), fptr(s), fptr(go), mptr(gf), mptr(gof), mptr(ga), mptr(gs), B, C, H, W, (int)K,
+                               (int)prop_time, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_nl_bwd_f32");
+    return {grad_or_empty(gf, f), grad_or_empty(gof, o), grad_or_empty(ga, a), grad_or_empty(gs, f)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -944,6 +1008,11 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate2d_aggregate_backward(Tensor guidance, Tensor blur_depth, Tensor? sparse_depth, Tensor step_weight, "
           "Tensor grad_out, int[] steps, int kernel_size, int norm_type, bool keep, bool need_guidance, bool need_blur, "
           "bool need_sparse, bool need_step_weight) -> (Tensor, Tensor, Tensor, Tensor)");
+    m.def("propagate2d_nonlocal(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, int kernel_size, int prop_time) "
+          "-> Tensor");
+    m.def("propagate2d_nonlocal_backward(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, Tensor grad_out, "
+          "int kernel_size, int prop_time, bool need_feat, bool need_offset, bool need_affinity, bool need_sparse) -> "
+          "(Tensor, Tensor, Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -990,6 +1059,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_keep_backward", &propagate2d_keep_backward_cuda);
     m.impl("propagate2d_aggregate", &propagate2d_aggregate_cuda);
     m.impl("propagate2d_aggregate_backward", &propagate2d_aggregate_backward_cuda);
+    m.impl("propagate2d_nonlocal", &propagate2d_nonlocal_cuda);
+    m.impl("propagate2d_nonlocal_backward", &propagate2d_nonlocal_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

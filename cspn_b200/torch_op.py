@@ -139,6 +139,40 @@ def _register():
 
     lib.register_autograd('cspn_b200::propagate2d_aggregate', backward2d_aggregate, setup_context=setup2d_aggregate)
 
+    @lib.register_fake('cspn_b200::propagate2d_nonlocal')
+    def _(feat, offset, affinity, sparse_depth, kernel_size, prop_time):
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        nt = kernel_size * kernel_size - 1
+        torch._check(feat.dim() == 4 and offset.dim() == 4 and affinity.dim() == 4, lambda: 'feat, offset and affinity must be 4D')
+        torch._check(offset.shape[1] == 2 * nt and affinity.shape[1] == nt,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs offset (B,{2 * nt},H,W) and affinity (B,{nt},H,W)')
+        torch._check(prop_time >= 0, lambda: 'prop_time must be >= 0')
+        return torch.empty_like(feat, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_nonlocal_backward')
+    def _(feat, offset, affinity, sparse_depth, grad_out, kernel_size, prop_time, need_feat, need_offset, need_affinity,
+          need_sparse):
+        new = lambda need, x: torch.empty_like(x, memory_format=torch.contiguous_format) if need else x.new_empty(0)
+        gs = new(need_sparse, sparse_depth) if sparse_depth is not None else feat.new_empty(0)
+        return new(need_feat, feat), new(need_offset, offset), new(need_affinity, affinity), gs
+
+    def setup2d_nonlocal(ctx, inputs, output):
+        feat, offset, affinity, sparse_depth, kernel_size, prop_time = inputs
+        ctx.save_for_backward(feat, offset, affinity, sparse_depth)
+        ctx.cfg = (kernel_size, prop_time)
+
+    def backward2d_nonlocal(ctx, grad_out):
+        feat, offset, affinity, sparse_depth = ctx.saved_tensors
+        kernel_size, prop_time = ctx.cfg
+        need_f, need_o, need_a = ctx.needs_input_grad[:3]
+        need_s = ctx.needs_input_grad[3] and sparse_depth is not None
+        gf, go, ga, gs = torch.ops.cspn_b200.propagate2d_nonlocal_backward(
+            feat, offset, affinity, sparse_depth, grad_out.contiguous(), kernel_size, prop_time, need_f, need_o, need_a, need_s)
+        return ((gf if need_f else None), (go if need_o else None), (ga if need_a else None), (gs if need_s else None),
+                None, None)
+
+    lib.register_autograd('cspn_b200::propagate2d_nonlocal', backward2d_nonlocal, setup_context=setup2d_nonlocal)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

@@ -230,6 +230,47 @@ CSPN_API int cspn2d_agg_bwd_f32(const float* guidance, const float* blur, const 
                        const int* steps, int n_steps, int norm_type, int keep, void* workspace, size_t workspace_bytes,
                        cspn_stream_t stream);
 
+/* ---- 2D non-local propagation, K in {3, 5, 7}: NLSPN's (Park et al., ECCV 2020) (DESIGN.md section 4.21) ---------
+ * feat [B][C][H][W] is h_0; offset [B][2T][H][W], T = K*K - 1, channel 2k the dy and 2k + 1 the dx of tap k; affinity
+ * [B][T][H][W] the weights a_k, used as given and shared by the C channels; sparse [B][C][H][W] or NULL.  Tap k runs over
+ * (i, j) in [0, K)^2 in raster order without the centre, base offset (i - R, j - R), R = (K - 1) / 2: torchvision's and
+ * DCN's order, the reverse of the K x K calls' (R - t, R - l).  S(h, y, x) is torchvision's bilinear_interpolate: 0 when
+ * y <= -1, y >= H, x <= -1 or x >= W, NaN for a NaN position, otherwise the four corners at floor(y), floor(x) and one past,
+ * a corner outside the image contributing nothing and one inside weight * value even when its weight is 0.  Then
+ *   h_{t+1}(p) = a_c S(h~_t, p) + sum_k a_k S(h~_t, p + base_k + (dy_k(p), dx_k(p))),  a_c = 1 - sum_k a_k,
+ *   h~_t = (1 - m) h_t + m sparse with m = 1[sparse > 0] (h~_t = h_t without a sparse); out = h_N, not replaced.
+ * One step is deform_conv2d(h~_t, offset with a zero centre, ones(C, 1, K, K), padding = R, mask = affinity with a_c at
+ * the centre), groups = C; the backward gives that composition's autograd gradients (torchvision's: a corner of weight
+ * exactly 0 takes no part in grad_feat, and the offsets' coordinate weight has no window test).  Every operation is
+ * rounded on its own in the order of DESIGN.md section 4.21: taps, then steps and channels ascending in every sum.
+ * The backward writes any of grad_feat [B][C][H][W], grad_offset [B][2T][H][W], grad_affinity [B][T][H][W] and
+ * grad_sparse [B][C][H][W] (sum_t m lambda~_t; needs a sparse) that is not NULL, and skips the work only the NULL ones need.
+ * iters = 0: the forward copies feat to out, the backward copies grad_out and zero-fills the others.
+ * Workspace (bytes; the queries return 0 for invalid arguments): forward 4 * min(iters - 1, 2) * B*C*H*W (0 for
+ * iters <= 1).  Backward, with P = B*C*H*W, n = B*H*W*T and each region rounded up to 256 bytes:
+ *   4 * (2 * iters * P + 2 * P + B*H*W + 8 * n) + 8 * (B*(H + 1)*(W + 1) + 1) + the radix sort's scratch + 256,
+ * the last 256 bytes leaving room to start the regions at a 256-byte boundary of a 4-byte aligned workspace,
+ * which CUB sizes for the current device: cspn2d_nl_bwd_workspace_bytes needs the CUDA runtime and a device and answers
+ * 0 without one.  Launches: forward iters; backward at most (iters - 1) + 4 + the sort's + iters + 1.  No floating-point
+ * atomics (the radix sort counts with integer ones); the bits depend on the arguments only.
+ * CSPN_ERR_INVALID_ARGUMENT for a null feat / offset / affinity / out (grad_out in the backward), a non-positive shape, K
+ * not in {3, 5, 7}, iters < 0, a grad_sparse without a sparse, a pointer that is not 4-byte aligned, and an output (the
+ * workspace included) that overlaps an input or another output; CSPN_ERR_UNSUPPORTED for H*W*T >= 2^31,
+ * B*ceil(C/4) > 65535 or B*(H+1)*(W+1) >= 2^32 - 1; CSPN_ERR_WORKSPACE for a missing or short workspace.  All of these come
+ * before any device work. */
+CSPN_API size_t cspn2d_nl_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_nl_fwd_f32(const float* feat, const float* offset, const float* affinity, const float* sparse,
+                      float* out, int B, int C, int H, int W, int K, int iters, void* workspace,
+                      size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_nl_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_nl_bwd_f32(const float* feat, const float* offset, const float* affinity, const float* sparse,
+                      const float* grad_out, float* grad_feat, float* grad_offset, float* grad_affinity,
+                      float* grad_sparse, int B, int C, int H, int W, int K, int iters, void* workspace,
+                      size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
