@@ -726,6 +726,135 @@ class Affinity_PropagateNonLocal(nn.Module):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'
 
 
+# ---- dilated 2D propagation with a centre weight and a learned confidence: PENet's DA-CSPN++ (DESIGN.md section 4.22) ------
+def _check_dilated(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time):
+    """The checks of propagate2d_dilated; every refusal comes before anything is allocated or narrowed to int."""
+    if prop_kernel not in (3, 5, 7) or isinstance(prop_kernel, bool):
+        raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+    if isinstance(dilation, bool) or not isinstance(dilation, int) or not 1 <= dilation <= 4:
+        raise ValueError(f'dilation must be an int in [1, 4], got {dilation!r}')
+    if isinstance(prop_time, bool) or not isinstance(prop_time, int) or not 0 <= prop_time <= 2 ** 31 - 1:
+        raise ValueError(f'prop_time must be an int >= 0, got {prop_time!r}')
+    if (sparse_depth is None) != (confidence is None):
+        raise ValueError('sparse_depth and confidence come together or not at all')
+    if blur_depth.dim() != 4 or min(blur_depth.shape) < 1:
+        raise ValueError(f'blur_depth must be a non-empty (B,C,H,W), got {tuple(blur_depth.shape)}')
+    B, C, H, W = blur_depth.shape
+    KK = prop_kernel * prop_kernel
+    if tuple(kernel.shape) != (B, KK, H, W):
+        raise ValueError(f'kernel must be (B, K*K, H, W) = {(B, KK, H, W)}, got {tuple(kernel.shape)}')
+    for name, t in (('sparse_depth', sparse_depth), ('confidence', confidence)):
+        if t is not None and tuple(t.shape) != (B, 1, H, W):
+            raise ValueError(f'{name} must be (B, 1, H, W) = {(B, 1, H, W)}, got {tuple(t.shape)}')
+    ts = [t for t in (kernel, blur_depth, sparse_depth, confidence) if t is not None]
+    if any(t.dtype != torch.float32 for t in ts):
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if any(t.device != blur_depth.device for t in ts):
+        raise RuntimeError('kernel, blur_depth, sparse_depth and confidence must be on one device')
+    if B * C > 65535 or -(-H // 16) > 65535 or W > 2 ** 31 - 1:
+        raise _lib.CspnError(f'propagate2d_dilated takes B*C <= 65535 and ceil(H/16) <= 65535, got blur_depth {tuple(blur_depth.shape)}')
+    if not blur_depth.is_cuda:
+        raise _lib.CspnError('propagate2d_dilated takes CUDA tensors only (there is no host-buffer entry point for it)')
+
+
+def _dilated_fwd(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time):
+    """Forward only (no autograd) through cspn2d_dil_fwd_f32, on the current stream."""
+    L = _lib.lib()
+    k, d = kernel.contiguous(), blur_depth.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    m = None if confidence is None else confidence.contiguous()
+    B, C, H, W = d.shape
+    out = torch.empty_like(d)
+    with torch.cuda.device(d.device):
+        ws_bytes = L.cspn2d_dil_workspace_bytes(B, C, H, W, prop_kernel, dilation, prop_time)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+        rc = L.cspn2d_dil_fwd_f32(_ptr(k), _ptr(d), _ptr(s), _ptr(m), _ptr(out), B, C, H, W, prop_kernel, dilation, prop_time,
+                                  _ptr(ws), ws_bytes, _stream(d.device))
+    _lib.check(rc, 'cspn2d_dil_fwd_f32')
+    return out
+
+
+class _Propagate2dDilatedFn(torch.autograd.Function):
+    """autograd seam of propagate2d_dilated without the torch-op shim: native forward + native backward
+    (cspn2d_dil_bwd_f32), differentiable in kernel, blur_depth, sparse_depth and confidence."""
+
+    @staticmethod
+    def forward(ctx, kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time):
+        ctx.save_for_backward(kernel, blur_depth, sparse_depth, confidence)
+        ctx.cfg = (prop_kernel, dilation, prop_time)
+        return _dilated_fwd(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        kernel, blur_depth, sparse_depth, confidence = ctx.saved_tensors
+        prop_kernel, dilation, prop_time = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        k, d, go = kernel.contiguous(), blur_depth.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        m = None if confidence is None else confidence.contiguous()
+        need_k, need_d, need_s, need_m = ctx.needs_input_grad[:4]
+        need_s, need_m = need_s and s is not None, need_m and m is not None
+        gk = torch.empty_like(k) if need_k else None
+        gd = torch.empty_like(d) if need_d else None
+        gs = torch.empty_like(s) if need_s else None
+        gm = torch.empty_like(m) if need_m else None
+        B, C, H, W = d.shape
+        with torch.cuda.device(d.device):
+            ws_bytes = L.cspn2d_dil_bwd_workspace_bytes(B, C, H, W, prop_kernel, dilation, prop_time)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+            rc = L.cspn2d_dil_bwd_f32(_ptr(k), _ptr(d), _ptr(s), _ptr(m), _ptr(go), _ptr(gk), _ptr(gd), _ptr(gs), _ptr(gm), B, C, H, W,
+                                      prop_kernel, dilation, prop_time, _ptr(ws), ws_bytes, _stream(d.device))
+        _lib.check(rc, 'cspn2d_dil_bwd_f32')
+        return gk, gd, gs, gm, None, None, None
+
+
+def propagate2d_dilated(kernel, blur_depth, sparse_depth=None, confidence=None, prop_kernel=3, dilation=1, prop_time=6):
+    """PENet's dilated and accelerated CSPN++ step (Hu et al., ICRA 2021), N = prop_time steps of
+        u_t(p) = sum_{j != c} w_j(p) d_t(p + dilation*o_j) + w_c(p) d_0(p),
+        d_{t+1} = m s + (1 - m) u_t   (d_{t+1} = u_t without samples),   out = d_N.
+    kernel (B, K*K, H, W) holds the weights exactly as given (no abs, no normalisation, no softmax), shared by the C
+    channels.  Channel j = i*K + l weights the value at p + dilation*(i - R, l - R), R = (K - 1) // 2: F.unfold's row
+    order, PENet's `kernel` argument.  The centre channel c = (K*K - 1) // 2 weights d_0 = blur_depth (B, C, H, W), not the
+    current iterate.  sparse_depth s and confidence m, (B, 1, H, W) and shared by the channels, come together or not at
+    all and are used as given; a hard mask is confidence = (sparse_depth > 0).float().  A read outside the image is 0.
+    All fp32 CUDA tensors; prop_kernel K in {3, 5, 7}, dilation in [1, 4].  Differentiable in kernel, blur_depth,
+    sparse_depth and confidence, with a deterministic backward.  prop_time == 0 returns blur_depth itself.
+    DESIGN.md section 4.22; INTEGRATION.md section 2g composes PENet's refinement from it."""
+    _check_dilated(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time)
+    if prop_time == 0:
+        return blur_depth
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.propagate2d_dilated(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (kernel, blur_depth, sparse_depth, confidence)):
+        return _Propagate2dDilatedFn.apply(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time)
+    return _dilated_fwd(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time)
+
+
+class Affinity_PropagateDilated(nn.Module):
+    """PENet's DA-CSPN++ propagation as a module: forward(kernel, blur_depth, sparse_depth=None, confidence=None) is
+    propagate2d_dilated(kernel, blur_depth, sparse_depth, confidence, prop_kernel, dilation, prop_time).  No parameters,
+    no buffers: the weights and the confidence come from the caller's network (INTEGRATION.md section 2g)."""
+
+    def __init__(self, prop_time, prop_kernel=3, dilation=1):
+        super().__init__()
+        if prop_kernel not in (3, 5, 7):
+            raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+        if dilation not in (1, 2, 3, 4):
+            raise ValueError(f'dilation must be in [1, 4], got {dilation!r}')
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+        self.dilation = dilation
+
+    def forward(self, kernel, blur_depth, sparse_depth=None, confidence=None):
+        return propagate2d_dilated(kernel, blur_depth, sparse_depth, confidence, self.prop_kernel, self.dilation, self.prop_time)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, dilation={self.dilation}'
+
+
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
 KERNEL_SIZES_3D = (3, 5)
 

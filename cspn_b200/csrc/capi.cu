@@ -1344,6 +1344,101 @@ int cspn2d_nl_bwd_f32(const float* feat, const float* offset, const float* affin
     });
 }
 
+// ---- 2D dilated propagation with a centre weight and a learned confidence, PENet's DA-CSPN++ (DESIGN.md section 4.22) ------
+// The sizes, K, the dilation and the step count: true when they are valid (the error is set otherwise)
+static bool dil_args_ok(int B, int C, int H, int W, int K, int dilation, int iters) {
+    if (!positive(B, C, H, W)) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (!kernel_size_ok(2, K)) { set_error("2D kernel size must be 3, 5 or 7, got %d", K); return false; }
+    if (dilation < 1 || dilation > 4) { set_error("dilation must be in [1, 4], got %d", dilation); return false; }
+    if (iters < 0) { set_error("prop_time must be >= 0, got %d", iters); return false; }
+    return true;
+}
+
+// The alignment of the non-null pointers, the launch limits, the overlaps (`in` are read and `outs` written; null entries
+// are absent buffers), then the workspace
+static int check_dil_buffers(int B, int C, int H, int W, std::vector<Buf> in, std::vector<Buf> outs, const void* ws, size_t ws_bytes,
+                             size_t need) {
+    uintptr_t bits = 0;
+    for (auto* set : {&in, &outs}) {
+        std::vector<Buf> kept;
+        for (const Buf& b : *set)
+            if (b.p) {
+                bits |= reinterpret_cast<uintptr_t>(b.p);
+                kept.push_back(b);
+            }
+        *set = kept;
+    }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!dilated2d_launchable(B, C, H, W, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    const int rc = check_disjoint(in, outs);
+    if (rc != CSPN_OK) return rc;
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("the dilated propagation needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    return CSPN_OK;
+}
+
+size_t cspn2d_dil_workspace_bytes(int B, int C, int H, int W, int K, int dilation, int iters) {
+    if (!dil_args_ok(B, C, H, W, K, dilation, iters)) return 0;
+    return dilated2d_workspace_bytes(B, C, H, W, iters);
+}
+
+size_t cspn2d_dil_bwd_workspace_bytes(int B, int C, int H, int W, int K, int dilation, int iters) {
+    if (!dil_args_ok(B, C, H, W, K, dilation, iters)) return 0;
+    return dilated2d_bwd_workspace_bytes(B, C, H, W, iters);
+}
+
+int cspn2d_dil_fwd_f32(const float* kernel, const float* blur, const float* sparse, const float* confidence, float* out, int B, int C,
+                       int H, int W, int K, int dilation, int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!kernel || !blur || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!sparse != !confidence) { set_error("sparse and confidence come together or not at all"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!dil_args_ok(B, C, H, W, K, dilation, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_b = span_bytes(B, C, hw), n_1 = span_bytes(B, 1, hw);
+    const size_t need = dilated2d_workspace_bytes(B, C, H, W, iters);
+    const int rc = check_dil_buffers(B, C, H, W,
+                                     {{kernel, span_bytes(B, K * K, hw), "kernel"}, {blur, n_b, "blur"}, {sparse, n_1, "sparse"},
+                                      {confidence, n_1, "confidence"}},
+                                     {{out, n_b, "out"}, {need ? workspace : nullptr, need, "the workspace"}}, workspace, workspace_bytes,
+                                     need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        return dilated2d_forward(kernel, blur, sparse, confidence, out, B, C, H, W, K, dilation, iters, workspace, (cudaStream_t)stream,
+                                 launches);
+    });
+}
+
+int cspn2d_dil_bwd_f32(const float* kernel, const float* blur, const float* sparse, const float* confidence, const float* grad_out,
+                       float* grad_kernel, float* grad_blur, float* grad_sparse, float* grad_confidence, int B, int C, int H, int W,
+                       int K, int dilation, int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!kernel || !blur || !grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!sparse != !confidence) { set_error("sparse and confidence come together or not at all"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if ((grad_sparse || grad_confidence) && !sparse) {
+        set_error("grad_sparse and grad_confidence need the samples");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (!dil_args_ok(B, C, H, W, K, dilation, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_b = span_bytes(B, C, hw), n_1 = span_bytes(B, 1, hw), n_k = span_bytes(B, K * K, hw);
+    const size_t need = dilated2d_bwd_workspace_bytes(B, C, H, W, iters);
+    const int rc = check_dil_buffers(
+            B, C, H, W,
+            {{kernel, n_k, "kernel"}, {blur, n_b, "blur"}, {sparse, n_1, "sparse"}, {confidence, n_1, "confidence"},
+             {grad_out, n_b, "grad_out"}},
+            {{grad_kernel, n_k, "grad_kernel"}, {grad_blur, n_b, "grad_blur"}, {grad_sparse, n_1, "grad_sparse"},
+             {grad_confidence, n_1, "grad_confidence"}, {need ? workspace : nullptr, need, "the workspace"}},
+            workspace, workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        return dilated2d_backward(kernel, blur, sparse, confidence, grad_out, grad_kernel, grad_blur, grad_sparse, grad_confidence, B, C,
+                                  H, W, K, dilation, iters, workspace, (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

@@ -263,4 +263,17 @@ int nonlocal2d_backward(const float* feat, const float* offset, const float* aff
                         float* grad_feat, float* grad_offset, float* grad_affinity, float* grad_sparse, int B, int C, int H, int W,
                         int K, int N, void* ws, cudaStream_t st, int* launches);
 
+// Dilated K x K propagation with a centre weight on d_0 and a learned confidence, PENet's DA-CSPN++ (cspn2d_dilated.cu):
+// K in {3, 5, 7}, dilation in [1, 4], N steps of blur (B, C, H, W) with kernel (B, K*K, H, W); sparse and conf (B, 1, H, W)
+// or both nullptr; arguments checked by the caller (sizes, pointers, then launchable).  The forward's workspace is the
+// ping-pong buffer; the backward's holds lambda_0 .. lambda_{N-1} and d_1 .. d_{N-1}
+int dilated2d_launchable(int B, int C, int H, int W, const char** why);
+size_t dilated2d_workspace_bytes(int B, int C, int H, int W, int N);
+size_t dilated2d_bwd_workspace_bytes(int B, int C, int H, int W, int N);
+int dilated2d_forward(const float* kern, const float* blur, const float* sparse, const float* conf, float* out, int B, int C, int H,
+                      int W, int K, int dil, int N, void* ws, cudaStream_t st, int* launches);
+int dilated2d_backward(const float* kern, const float* blur, const float* sparse, const float* conf, const float* grad_out,
+                       float* grad_kern, float* grad_blur, float* grad_sparse, float* grad_conf, int B, int C, int H, int W, int K,
+                       int dil, int N, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

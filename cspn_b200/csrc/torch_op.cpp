@@ -31,6 +31,12 @@
 //   propagate2d_nonlocal_backward(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, Tensor grad_out,
 //                                 int kernel_size, int prop_time, bool need_feat, bool need_offset, bool need_affinity,
 //                                 bool need_sparse) -> (Tensor, Tensor, Tensor, Tensor)
+//   propagate2d_dilated(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, int kernel_size,
+//                       int dilation, int prop_time) -> Tensor   (PENet's DA-CSPN++ step: kernel (B, K*K, H, W), sparse_depth
+//                       and confidence (B, 1, H, W), both or neither, K in {3, 5, 7}, dilation in [1, 4])
+//   propagate2d_dilated_backward(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, Tensor grad_out,
+//                                int kernel_size, int dilation, int prop_time, bool need_kernel, bool need_blur,
+//                                bool need_sparse, bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -380,6 +386,67 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_nonlocal_
                                (int)prop_time, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_nl_bwd_f32");
     return {grad_or_empty(gf, f), grad_or_empty(gof, o), grad_or_empty(ga, a), grad_or_empty(gs, f)};
+}
+
+// Dilated propagation, K in {3, 5, 7}: cspn2d_dil_*_f32.  kernel (B, K*K, H, W), blur_depth (B, C, H, W), sparse_depth and
+// confidence (B, 1, H, W), both or neither
+void check2d_dil(const at::Tensor& kernel, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                 const std::optional<at::Tensor>& conf, int64_t K, int64_t dilation, int64_t prop_time) {
+    TORCH_CHECK_VALUE(kernel_size_ok(K, 2), "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK_VALUE(dilation >= 1 && dilation <= 4, "dilation must be in [1, 4], got ", dilation);
+    TORCH_CHECK_VALUE(prop_time >= 0 && prop_time <= INT32_MAX, "prop_time must be >= 0, got ", prop_time);
+    TORCH_CHECK_VALUE(sparse.has_value() == conf.has_value(), "sparse_depth and confidence come together or not at all");
+    TORCH_CHECK_VALUE(blur.dim() == 4 && blur.numel() > 0, "blur_depth must be a non-empty (B,C,H,W), got ", blur.sizes());
+    const int64_t B = blur.size(0), C = blur.size(1), H = blur.size(2), W = blur.size(3);
+    TORCH_CHECK_VALUE(kernel.dim() == 4 && kernel.size(0) == B && kernel.size(1) == K * K && kernel.size(2) == H && kernel.size(3) == W,
+                      "kernel must be (B, K*K, H, W) = (", B, ", ", K * K, ", ", H, ", ", W, "), got ", kernel.sizes());
+    TORCH_CHECK(kernel.scalar_type() == at::kFloat && blur.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(kernel.device() == blur.device(), "kernel and blur_depth are on different devices");
+    for (const auto* t : {&sparse, &conf})
+        if (t->has_value()) {
+            TORCH_CHECK_VALUE((*t)->dim() == 4 && (*t)->size(0) == B && (*t)->size(1) == 1 && (*t)->size(2) == H && (*t)->size(3) == W,
+                              "sparse_depth and confidence must be (B, 1, H, W) = (", B, ", 1, ", H, ", ", W, "), got ", (*t)->sizes());
+            TORCH_CHECK((*t)->scalar_type() == at::kFloat && (*t)->device() == blur.device(),
+                        "sparse_depth and confidence must be fp32 on the device of blur_depth");
+        }
+    TORCH_CHECK(B * C <= 65535 && (H + 15) / 16 <= 65535 && W < ((int64_t)1 << 31),
+                "propagate2d_dilated takes B*C <= 65535 and ceil(H/16) <= 65535, got blur_depth ", blur.sizes());
+}
+
+at::Tensor propagate2d_dilated_cuda(const at::Tensor& kernel, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                                    const std::optional<at::Tensor>& conf, int64_t K, int64_t dilation, int64_t prop_time) {
+    check2d_dil(kernel, blur, sparse, conf, K, dilation, prop_time);
+    if (prop_time == 0) return blur.clone();           // a dispatcher op may not return its input
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor k = kernel.contiguous(), d = blur.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    const at::Tensor m = conf.has_value() ? conf->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(d);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const Workspace ws(cspn2d_dil_workspace_bytes(B, C, H, W, (int)K, (int)dilation, (int)prop_time), d);
+    check_rc(cspn2d_dil_fwd_f32(fptr(k), fptr(d), fptr(s), fptr(m), mptr(out), B, C, H, W, (int)K, (int)dilation, (int)prop_time,
+                                ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_dil_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_dilated_backward_cuda(
+        const at::Tensor& kernel, const at::Tensor& blur, const std::optional<at::Tensor>& sparse, const std::optional<at::Tensor>& conf,
+        const at::Tensor& grad_out, int64_t K, int64_t dilation, int64_t prop_time, bool need_k, bool need_d, bool need_s, bool need_m) {
+    check2d_dil(kernel, blur, sparse, conf, K, dilation, prop_time);
+    check_grad_out(grad_out, blur, "blur_depth");
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor k = kernel.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    const at::Tensor m = conf.has_value() ? conf->contiguous() : at::Tensor();
+    at::Tensor gk = new_grad(need_k, k), gd = new_grad(need_d, d);
+    at::Tensor gs = s.defined() ? new_grad(need_s, s) : at::Tensor(), gm = m.defined() ? new_grad(need_m, m) : at::Tensor();
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const Workspace ws(cspn2d_dil_bwd_workspace_bytes(B, C, H, W, (int)K, (int)dilation, (int)prop_time), d);
+    check_rc(cspn2d_dil_bwd_f32(fptr(k), fptr(d), fptr(s), fptr(m), fptr(go), mptr(gk), mptr(gd), mptr(gs), mptr(gm), B, C, H, W, (int)K,
+                                (int)dilation, (int)prop_time, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_dil_bwd_f32");
+    return {grad_or_empty(gk, k), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gm, d)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -1013,6 +1080,11 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate2d_nonlocal_backward(Tensor feat, Tensor offset, Tensor affinity, Tensor? sparse_depth, Tensor grad_out, "
           "int kernel_size, int prop_time, bool need_feat, bool need_offset, bool need_affinity, bool need_sparse) -> "
           "(Tensor, Tensor, Tensor, Tensor)");
+    m.def("propagate2d_dilated(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, int kernel_size, "
+          "int dilation, int prop_time) -> Tensor");
+    m.def("propagate2d_dilated_backward(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, Tensor grad_out, "
+          "int kernel_size, int dilation, int prop_time, bool need_kernel, bool need_blur, bool need_sparse, bool need_confidence) -> "
+          "(Tensor, Tensor, Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -1061,6 +1133,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_aggregate_backward", &propagate2d_aggregate_backward_cuda);
     m.impl("propagate2d_nonlocal", &propagate2d_nonlocal_cuda);
     m.impl("propagate2d_nonlocal_backward", &propagate2d_nonlocal_backward_cuda);
+    m.impl("propagate2d_dilated", &propagate2d_dilated_cuda);
+    m.impl("propagate2d_dilated_backward", &propagate2d_dilated_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

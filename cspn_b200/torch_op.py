@@ -173,6 +173,44 @@ def _register():
 
     lib.register_autograd('cspn_b200::propagate2d_nonlocal', backward2d_nonlocal, setup_context=setup2d_nonlocal)
 
+    @lib.register_fake('cspn_b200::propagate2d_dilated')
+    def _(kernel, blur_depth, sparse_depth, confidence, kernel_size, dilation, prop_time):
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        torch._check(1 <= dilation <= 4, lambda: 'dilation must be in [1, 4]')
+        torch._check(kernel.dim() == 4 and blur_depth.dim() == 4, lambda: 'kernel and blur_depth must be 4D')
+        torch._check(kernel.shape[1] == kernel_size * kernel_size,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs (B,{kernel_size * kernel_size},H,W) weights')
+        torch._check((sparse_depth is None) == (confidence is None), lambda: 'sparse_depth and confidence come together')
+        torch._check(prop_time >= 0, lambda: 'prop_time must be >= 0')
+        return torch.empty_like(blur_depth, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_dilated_backward')
+    def _(kernel, blur_depth, sparse_depth, confidence, grad_out, kernel_size, dilation, prop_time, need_kernel, need_blur,
+          need_sparse, need_confidence):
+        new = lambda need, x: torch.empty_like(x, memory_format=torch.contiguous_format) if need else blur_depth.new_empty(0)
+        gs = new(need_sparse, sparse_depth) if sparse_depth is not None else blur_depth.new_empty(0)
+        gm = new(need_confidence, confidence) if confidence is not None else blur_depth.new_empty(0)
+        return new(need_kernel, kernel), new(need_blur, blur_depth), gs, gm
+
+    def setup2d_dilated(ctx, inputs, output):
+        kernel, blur_depth, sparse_depth, confidence, kernel_size, dilation, prop_time = inputs
+        ctx.save_for_backward(kernel, blur_depth, sparse_depth, confidence)
+        ctx.cfg = (kernel_size, dilation, prop_time)
+
+    def backward2d_dilated(ctx, grad_out):
+        kernel, blur_depth, sparse_depth, confidence = ctx.saved_tensors
+        kernel_size, dilation, prop_time = ctx.cfg
+        need_k, need_d = ctx.needs_input_grad[:2]
+        need_s = ctx.needs_input_grad[2] and sparse_depth is not None
+        need_m = ctx.needs_input_grad[3] and confidence is not None
+        gk, gd, gs, gm = torch.ops.cspn_b200.propagate2d_dilated_backward(
+            kernel, blur_depth, sparse_depth, confidence, grad_out.contiguous(), kernel_size, dilation, prop_time, need_k, need_d,
+            need_s, need_m)
+        return ((gk if need_k else None), (gd if need_d else None), (gs if need_s else None), (gm if need_m else None),
+                None, None, None)
+
+    lib.register_autograd('cspn_b200::propagate2d_dilated', backward2d_dilated, setup_context=setup2d_dilated)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

@@ -271,6 +271,39 @@ CSPN_API int cspn2d_nl_bwd_f32(const float* feat, const float* offset, const flo
                       float* grad_sparse, int B, int C, int H, int W, int K, int iters, void* workspace,
                       size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D dilated propagation, K in {3, 5, 7}, dilation in [1, 4]: PENet's DA-CSPN++ (Hu et al., ICRA 2021) --------------
+ * (DESIGN.md section 4.22).  kernel [B][K*K][H][W] holds the weights as given (no abs, no normalisation), shared by the C
+ * channels: channel j = i*K + l weights d_t(p + dilation*(i - R, l - R)), R = (K - 1) / 2 (F.unfold's row order), and the
+ * centre channel c = (K*K - 1) / 2 weights blur(p).  blur [B][C][H][W] is d_0; sparse and confidence [B][1][H][W] are s and m,
+ * both or neither, used as given.  A read outside the image is 0.  iters steps of
+ *   u_t(p) = w_c(p) d_0(p) + sum_{j != c} w_j(p) d_t(p + dilation*o_j),  d_{t+1} = m s + (1 - m) u_t  (d_{t+1} = u_t without samples)
+ * and out = d_N.  Order of operations (DESIGN.md section 4.22): u starts from the rounded product w_c d_0 and adds the taps
+ * j = K*K-1 down to 0 by FMA; m s, (1 - m), its product with u and the sum are each rounded on their own.
+ * The backward writes any of grad_kernel [B][K*K][H][W], grad_blur [B][C][H][W], grad_sparse and grad_confidence
+ * [B][1][H][W] that is not NULL (the last two need the samples) and skips the work only the NULL ones need: without
+ * grad_kernel and grad_confidence it recomputes no iterate.  iters = 0: the forward copies blur to out, the backward copies
+ * grad_out and zero-fills the others (cudaMemsetAsync).
+ * Workspace (bytes, device-independent; the queries return 0 for invalid arguments): forward 4 * B*C*H*W for iters >= 2,
+ * else 0; backward 4 * (2 * iters - 1) * B*C*H*W (lambda_0 .. lambda_{N-1} and d_1 .. d_{N-1}), 0 for iters = 0.
+ * Launches: forward iters; backward at most (iters - 1) + iters + 1.  No atomics; the bits depend on the arguments only.
+ * CSPN_ERR_INVALID_ARGUMENT for a null kernel / blur / out (grad_out in the backward), exactly one of sparse and confidence,
+ * a grad_sparse or grad_confidence without the samples, a non-positive shape, K not in {3, 5, 7}, a dilation outside
+ * [1, 4], iters < 0, a pointer that is not 4-byte aligned, and an output (the workspace included) that overlaps an input
+ * or another output; CSPN_ERR_UNSUPPORTED for B*C > 65535 or ceil(H/16) > 65535; CSPN_ERR_WORKSPACE for a missing or
+ * short workspace.  All of these come before any device work. */
+CSPN_API size_t cspn2d_dil_workspace_bytes(int B, int C, int H, int W, int K, int dilation, int iters);
+
+CSPN_API int cspn2d_dil_fwd_f32(const float* kernel, const float* blur, const float* sparse, const float* confidence,
+                       float* out, int B, int C, int H, int W, int K, int dilation, int iters, void* workspace,
+                       size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_dil_bwd_workspace_bytes(int B, int C, int H, int W, int K, int dilation, int iters);
+
+CSPN_API int cspn2d_dil_bwd_f32(const float* kernel, const float* blur, const float* sparse, const float* confidence,
+                       const float* grad_out, float* grad_kernel, float* grad_blur, float* grad_sparse,
+                       float* grad_confidence, int B, int C, int H, int W, int K, int dilation, int iters,
+                       void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
