@@ -855,6 +855,145 @@ class Affinity_PropagateDilated(nn.Module):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}, dilation={self.dilation}'
 
 
+# ---- dynamic 2D propagation with per-step ring attention and an anchor to d_0: DySPN's step (DESIGN.md section 4.23) ------
+def _check_dynamic(affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel):
+    """The checks of propagate2d_dynamic; every refusal comes before anything is allocated or narrowed to int.  Returns N."""
+    if prop_kernel not in (3, 5, 7) or isinstance(prop_kernel, bool):
+        raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+    if (sparse_depth is None) != (confidence is None):
+        raise ValueError('sparse_depth and confidence come together or not at all')
+    if blur_depth.dim() != 4 or min(blur_depth.shape) < 1:
+        raise ValueError(f'blur_depth must be a non-empty (B,C,H,W), got {tuple(blur_depth.shape)}')
+    B, C, H, W = blur_depth.shape
+    KK, NR = prop_kernel * prop_kernel, (prop_kernel + 1) // 2
+    if tuple(affinity.shape) != (B, KK, H, W):
+        raise ValueError(f'affinity must be (B, K*K, H, W) = {(B, KK, H, W)}, got {tuple(affinity.shape)}')
+    if attention.dim() != 4 or tuple(attention.shape[::2]) != (B, H) or attention.shape[3] != W or attention.shape[1] % NR \
+            or attention.shape[1] > 2 ** 31 - 1:
+        raise ValueError(f'attention must be (B, N*(K+1)//2, H, W) with (K+1)//2 = {NR} and (B, H, W) = {(B, H, W)}, '
+                         f'got {tuple(attention.shape)}')
+    for name, t in (('sparse_depth', sparse_depth), ('confidence', confidence)):
+        if t is not None and tuple(t.shape) != (B, 1, H, W):
+            raise ValueError(f'{name} must be (B, 1, H, W) = {(B, 1, H, W)}, got {tuple(t.shape)}')
+    ts = [t for t in (affinity, attention, blur_depth, sparse_depth, confidence) if t is not None]
+    if any(t.dtype != torch.float32 for t in ts):
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if any(t.device != blur_depth.device for t in ts):
+        raise RuntimeError('affinity, attention, blur_depth, sparse_depth and confidence must be on one device')
+    if B * C > 65535 or -(-H // 16) > 65535 or W > 2 ** 31 - 1:
+        raise _lib.CspnError(f'propagate2d_dynamic takes B*C <= 65535 and ceil(H/16) <= 65535, got blur_depth {tuple(blur_depth.shape)}')
+    if not blur_depth.is_cuda:
+        raise _lib.CspnError('propagate2d_dynamic takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return attention.shape[1] // NR
+
+
+def _dynamic_fwd(affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel, N):
+    """Forward only (no autograd) through cspn2d_dyn_fwd_f32, on the current stream."""
+    L = _lib.lib()
+    a, at, d = affinity.contiguous(), attention.contiguous(), blur_depth.contiguous()
+    s = None if sparse_depth is None else sparse_depth.contiguous()
+    m = None if confidence is None else confidence.contiguous()
+    B, C, H, W = d.shape
+    out = torch.empty_like(d)
+    with torch.cuda.device(d.device):
+        ws_bytes = L.cspn2d_dyn_workspace_bytes(B, C, H, W, prop_kernel, N)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+        rc = L.cspn2d_dyn_fwd_f32(_ptr(a), _ptr(at), _ptr(d), _ptr(s), _ptr(m), _ptr(out), B, C, H, W, prop_kernel, N, _ptr(ws), ws_bytes,
+                                  _stream(d.device))
+    _lib.check(rc, 'cspn2d_dyn_fwd_f32')
+    return out
+
+
+class _Propagate2dDynamicFn(torch.autograd.Function):
+    """autograd seam of propagate2d_dynamic without the torch-op shim: native forward + native backward
+    (cspn2d_dyn_bwd_f32), differentiable in affinity, attention, blur_depth, sparse_depth and confidence."""
+
+    @staticmethod
+    def forward(ctx, affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel, N):
+        ctx.save_for_backward(affinity, attention, blur_depth, sparse_depth, confidence)
+        ctx.cfg = (prop_kernel, N)
+        return _dynamic_fwd(affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel, N)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        affinity, attention, blur_depth, sparse_depth, confidence = ctx.saved_tensors
+        prop_kernel, N = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        a, at, d, go = affinity.contiguous(), attention.contiguous(), blur_depth.contiguous(), grad_out.contiguous()
+        s = None if sparse_depth is None else sparse_depth.contiguous()
+        m = None if confidence is None else confidence.contiguous()
+        need_a, need_t, need_d, need_s, need_m = ctx.needs_input_grad[:5]
+        need_s, need_m = need_s and s is not None, need_m and m is not None
+        ga = torch.empty_like(a) if need_a else None
+        gt = torch.empty_like(at) if need_t else None
+        gd = torch.empty_like(d) if need_d else None
+        gs = torch.empty_like(s) if need_s else None
+        gm = torch.empty_like(m) if need_m else None
+        B, C, H, W = d.shape
+        with torch.cuda.device(d.device):
+            ws_bytes = L.cspn2d_dyn_bwd_workspace_bytes(B, C, H, W, prop_kernel, N)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=d.device) if ws_bytes else None
+            rc = L.cspn2d_dyn_bwd_f32(_ptr(a), _ptr(at), _ptr(d), _ptr(s), _ptr(m), _ptr(go), _ptr(ga), _ptr(gt), _ptr(gd), _ptr(gs),
+                                      _ptr(gm), B, C, H, W, prop_kernel, N, _ptr(ws), ws_bytes, _stream(d.device))
+        _lib.check(rc, 'cspn2d_dyn_bwd_f32')
+        return ga, gt, gd, gs, gm, None, None
+
+
+def propagate2d_dynamic(affinity, attention, blur_depth, sparse_depth=None, confidence=None, prop_kernel=7):
+    """DySPN's dynamic spatial propagation (Lin et al., AAAI 2022), N = attention.shape[1] // ((K + 1) // 2) steps of
+        w_{t,j}(p) = a_{t,ring(j)}(p) affinity_j(p),   rho_t(p) = 1 - sum_j w_{t,j}(p),
+        v_t(p) = rho_t(p) d_0(p) + sum_j w_{t,j}(p) d_t(p + o_j),
+        d_{t+1} = m s + (1 - m) v_t   (d_{t+1} = v_t without samples),   out = d_N.
+    affinity (B, K*K, H, W) holds all K*K taps, the centre included, exactly as given (no abs, no normalisation), shared by
+    the C channels.  Channel j = i*K + l weights d_t(p + o_j), o_j = (i - R, l - R), R = (K - 1) // 2: F.unfold's row
+    order.  Tap j lies on ring(j) = max(|i - R|, |l - R|): ring 0 is the centre, ring r holds 8r taps.  attention
+    (B, N*(R+1), H, W) holds, in channel t*(R+1) + r, the attention of ring r at step t, used as given (the caller applies
+    the sigmoid).  The weight the attention takes away goes back to d_0 = blur_depth (B, C, H, W) through rho.
+    sparse_depth s and confidence m, (B, 1, H, W) and shared by the channels, come together or not at all and are used as
+    given; a hard mask is confidence = (sparse_depth > 0).float().  A read outside the image is 0.  All fp32 CUDA tensors;
+    prop_kernel K in {3, 5, 7}.  Differentiable in affinity, attention, blur_depth, sparse_depth and confidence, with a
+    deterministic backward.  N == 0 returns blur_depth itself.
+    DESIGN.md section 4.23; INTEGRATION.md section 2h composes a DySPN head from it."""
+    N = _check_dynamic(affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel)
+    if N == 0:
+        return blur_depth
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.propagate2d_dynamic(affinity, attention, blur_depth, sparse_depth, confidence, prop_kernel)
+    ts = (affinity, attention, blur_depth, sparse_depth, confidence)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts):
+        return _Propagate2dDynamicFn.apply(*ts, prop_kernel, N)
+    return _dynamic_fwd(*ts, prop_kernel, N)
+
+
+class Affinity_PropagateDynamic(nn.Module):
+    """DySPN's dynamic propagation as a module: forward(affinity, attention, blur_depth, sparse_depth=None,
+    confidence=None) is propagate2d_dynamic(...) after checking that the attention has the prop_time * (K + 1) // 2
+    channels prop_time implies.  No parameters, no buffers: the affinity, the attention and the confidence come from the
+    caller's network (INTEGRATION.md section 2h)."""
+
+    def __init__(self, prop_time, prop_kernel=7):
+        super().__init__()
+        if prop_kernel not in (3, 5, 7) or isinstance(prop_kernel, bool):
+            raise ValueError(f'prop_kernel must be 3, 5 or 7, got {prop_kernel!r}')
+        if isinstance(prop_time, bool) or not isinstance(prop_time, int) or prop_time < 0:
+            raise ValueError(f'prop_time must be an int >= 0, got {prop_time!r}')
+        self.prop_time = prop_time
+        self.prop_kernel = prop_kernel
+
+    def forward(self, affinity, attention, blur_depth, sparse_depth=None, confidence=None):
+        want = self.prop_time * ((self.prop_kernel + 1) // 2)
+        if attention.dim() != 4 or attention.shape[1] != want:
+            raise ValueError(f'prop_time={self.prop_time} at prop_kernel={self.prop_kernel} needs {want} attention channels, '
+                             f'got attention {tuple(attention.shape)}')
+        return propagate2d_dynamic(affinity, attention, blur_depth, sparse_depth, confidence, self.prop_kernel)
+
+    def extra_repr(self):
+        return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'
+
+
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
 KERNEL_SIZES_3D = (3, 5)
 

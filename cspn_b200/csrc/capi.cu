@@ -1355,9 +1355,10 @@ static bool dil_args_ok(int B, int C, int H, int W, int K, int dilation, int ite
 }
 
 // The alignment of the non-null pointers, the launch limits, the overlaps (`in` are read and `outs` written; null entries
-// are absent buffers), then the workspace
+// are absent buffers), then the workspace.  Shared by the dilated and the dynamic propagation (`what`, `launchable`).
 static int check_dil_buffers(int B, int C, int H, int W, std::vector<Buf> in, std::vector<Buf> outs, const void* ws, size_t ws_bytes,
-                             size_t need) {
+                             size_t need, const char* what = "the dilated propagation",
+                             int (*launchable)(int, int, int, int, const char**) = dilated2d_launchable) {
     uintptr_t bits = 0;
     for (auto* set : {&in, &outs}) {
         std::vector<Buf> kept;
@@ -1370,11 +1371,11 @@ static int check_dil_buffers(int B, int C, int H, int W, std::vector<Buf> in, st
     }
     if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
     const char* why = "";
-    if (!dilated2d_launchable(B, C, H, W, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    if (!launchable(B, C, H, W, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
     const int rc = check_disjoint(in, outs);
     if (rc != CSPN_OK) return rc;
     if (need && (!ws || ws_bytes < need)) {
-        set_error("the dilated propagation needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
+        set_error("%s needs %zu workspace bytes, got %zu", what, need, ws ? ws_bytes : (size_t)0);
         return CSPN_ERR_WORKSPACE;
     }
     return CSPN_OK;
@@ -1436,6 +1437,81 @@ int cspn2d_dil_bwd_f32(const float* kernel, const float* blur, const float* spar
     return on_device_of(blur, "blur", [&](int* launches) {
         return dilated2d_backward(kernel, blur, sparse, confidence, grad_out, grad_kernel, grad_blur, grad_sparse, grad_confidence, B, C,
                                   H, W, K, dilation, iters, workspace, (cudaStream_t)stream, launches);
+    });
+}
+
+// ---- 2D dynamic propagation with per-step ring attention and an anchor to d_0, DySPN's step (DESIGN.md section 4.23) -------
+static bool dyn_args_ok(int B, int C, int H, int W, int K, int iters) {
+    if (!positive(B, C, H, W)) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (!kernel_size_ok(2, K)) { set_error("2D kernel size must be 3, 5 or 7, got %d", K); return false; }
+    if (iters < 0) { set_error("the step count must be >= 0, got %d", iters); return false; }
+    if ((long long)iters * ((K + 1) / 2) > INT32_MAX) { set_error("iters * (K + 1) / 2 attention channels exceed 2^31 - 1"); return false; }
+    return true;
+}
+
+size_t cspn2d_dyn_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!dyn_args_ok(B, C, H, W, K, iters)) return 0;
+    return dynamic2d_workspace_bytes(B, C, H, W, iters);
+}
+
+size_t cspn2d_dyn_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters) {
+    if (!dyn_args_ok(B, C, H, W, K, iters)) return 0;
+    return dynamic2d_bwd_workspace_bytes(B, C, H, W, iters);
+}
+
+int cspn2d_dyn_fwd_f32(const float* affinity, const float* attention, const float* blur, const float* sparse, const float* confidence,
+                       float* out, int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                       cspn_stream_t stream) {
+    begin_call();
+    if (!affinity || !blur || !out || (!attention && iters > 0)) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!sparse != !confidence) { set_error("sparse and confidence come together or not at all"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!dyn_args_ok(B, C, H, W, K, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_b = span_bytes(B, C, hw), n_1 = span_bytes(B, 1, hw);
+    const size_t need = dynamic2d_workspace_bytes(B, C, H, W, iters);
+    const int rc = check_dil_buffers(B, C, H, W,
+                                     {{affinity, span_bytes(B, K * K, hw), "affinity"},
+                                      {iters ? attention : nullptr, span_bytes(B, iters * ((K + 1) / 2), hw), "attention"},
+                                      {blur, n_b, "blur"}, {sparse, n_1, "sparse"}, {confidence, n_1, "confidence"}},
+                                     {{out, n_b, "out"}, {need ? workspace : nullptr, need, "the workspace"}}, workspace, workspace_bytes,
+                                     need, "the dynamic propagation", dynamic2d_launchable);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        return dynamic2d_forward(affinity, attention, blur, sparse, confidence, out, B, C, H, W, K, iters, workspace, (cudaStream_t)stream,
+                                 launches);
+    });
+}
+
+int cspn2d_dyn_bwd_f32(const float* affinity, const float* attention, const float* blur, const float* sparse, const float* confidence,
+                       const float* grad_out, float* grad_affinity, float* grad_attention, float* grad_blur, float* grad_sparse,
+                       float* grad_confidence, int B, int C, int H, int W, int K, int iters, void* workspace, size_t workspace_bytes,
+                       cspn_stream_t stream) {
+    begin_call();
+    if (!affinity || !blur || !grad_out || (!attention && iters > 0)) {
+        set_error("null tensor pointer");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (!sparse != !confidence) { set_error("sparse and confidence come together or not at all"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if ((grad_sparse || grad_confidence) && !sparse) {
+        set_error("grad_sparse and grad_confidence need the samples");
+        return CSPN_ERR_INVALID_ARGUMENT;
+    }
+    if (!dyn_args_ok(B, C, H, W, K, iters)) return CSPN_ERR_INVALID_ARGUMENT;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_b = span_bytes(B, C, hw), n_1 = span_bytes(B, 1, hw), n_k = span_bytes(B, K * K, hw);
+    const uintptr_t n_a = span_bytes(B, iters * ((K + 1) / 2), hw);
+    const size_t need = dynamic2d_bwd_workspace_bytes(B, C, H, W, iters);
+    const int rc = check_dil_buffers(
+            B, C, H, W,
+            {{affinity, n_k, "affinity"}, {iters ? attention : nullptr, n_a, "attention"}, {blur, n_b, "blur"}, {sparse, n_1, "sparse"},
+             {confidence, n_1, "confidence"}, {grad_out, n_b, "grad_out"}},
+            {{grad_affinity, n_k, "grad_affinity"}, {iters ? grad_attention : nullptr, n_a, "grad_attention"}, {grad_blur, n_b, "grad_blur"},
+             {grad_sparse, n_1, "grad_sparse"}, {grad_confidence, n_1, "grad_confidence"}, {need ? workspace : nullptr, need, "the workspace"}},
+            workspace, workspace_bytes, need, "the dynamic propagation", dynamic2d_launchable);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(blur, "blur", [&](int* launches) {
+        return dynamic2d_backward(affinity, attention, blur, sparse, confidence, grad_out, grad_affinity, iters ? grad_attention : nullptr,
+                                  grad_blur, grad_sparse, grad_confidence, B, C, H, W, K, iters, workspace, (cudaStream_t)stream, launches);
     });
 }
 

@@ -276,4 +276,17 @@ int dilated2d_backward(const float* kern, const float* blur, const float* sparse
                        float* grad_kern, float* grad_blur, float* grad_sparse, float* grad_conf, int B, int C, int H, int W, int K,
                        int dil, int N, void* ws, cudaStream_t st, int* launches);
 
+// Dynamic K x K propagation with per-step ring attention and an anchor to d_0, DySPN's step (cspn2d_dynamic.cu): K in
+// {3, 5, 7}, N steps of blur (B, C, H, W) with affinity (B, K*K, H, W) and attention (B, N*(K+1)/2, H, W); sparse and conf
+// (B, 1, H, W) or both nullptr; arguments checked by the caller (sizes, pointers, then launchable).  The forward's
+// workspace is the ping-pong buffer; the backward's holds lambda_0 .. lambda_{N-1} and d_1 .. d_{N-1}
+int dynamic2d_launchable(int B, int C, int H, int W, const char** why);
+size_t dynamic2d_workspace_bytes(int B, int C, int H, int W, int N);
+size_t dynamic2d_bwd_workspace_bytes(int B, int C, int H, int W, int N);
+int dynamic2d_forward(const float* aff, const float* att, const float* blur, const float* sparse, const float* conf, float* out, int B,
+                      int C, int H, int W, int K, int N, void* ws, cudaStream_t st, int* launches);
+int dynamic2d_backward(const float* aff, const float* att, const float* blur, const float* sparse, const float* conf,
+                       const float* grad_out, float* grad_aff, float* grad_att, float* grad_blur, float* grad_sparse, float* grad_conf,
+                       int B, int C, int H, int W, int K, int N, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

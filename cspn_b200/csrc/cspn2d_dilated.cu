@@ -29,9 +29,7 @@
 //   finalize  one launch: a thread per pixel and kernel row for grad_kernel, and a thread per pixel for the others,
 //             each over all channels and steps.
 // No atomics and no memsets (except the N = 0 backward's zero gradients); every output word is written by one thread.
-#include <initializer_list>
-
-#include "common.cuh"
+#include "cspn2d_stencil.cuh"
 
 namespace cspn {
 namespace {
@@ -39,33 +37,6 @@ namespace {
 constexpr int kTX = 32, kTY = 8, kRows = 2;          // threads per CTA (x, y); each thread runs kRows tile rows
 constexpr int kTH = kTY * kRows;                     // tile height
 constexpr int kFinThreads = 128;
-
-long long ceil_div(long long a, long long b) { return (a + b - 1) / b; }
-
-__device__ __forceinline__ bool in_image(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
-
-__device__ __forceinline__ float blend(float m, float s, float u) {
-    return __fadd_rn(__fmul_rn(m, s), __fmul_rn(__fsub_rn(1.f, m), u));
-}
-
-__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-
-// Stages rows y0 - h .. y0 + kTH - 1 + h and columns x0 - h .. x0 + TW - 1 + h of plane src into tile (pitch TW + 2h),
-// zeros outside the image.  With a: each value is a(q) * src(q) (the adjoint's mu = (1 - m) lambda).
-__device__ __forceinline__ void stage(float* tile, int pitch, const float* __restrict__ src, const float* __restrict__ a, int x0,
-                                      int y0, int h, int H, int W) {
-    const int n = (kTH + 2 * h) * pitch;
-    for (int i = threadIdx.y * kTX + threadIdx.x; i < n; i += kTX * kTY) {
-        const int gy = y0 - h + i / pitch, gx = x0 - h + i % pitch;
-        float v = 0.f;
-        if (in_image(gy, gx, H, W)) {
-            const size_t q = (size_t)gy * W + gx;
-            v = __ldg(src + q);
-            if (a) v = __fmul_rn(__fsub_rn(1.f, __ldg(a + q)), v);
-        }
-        tile[i] = v;
-    }
-}
 
 template <int K, int VEC, bool SAMP>
 __global__ void __launch_bounds__(kTX * kTY)
@@ -77,7 +48,7 @@ dil_step_kernel(const float* __restrict__ kern, const float* __restrict__ d0, co
     const int TW = kTX * VEC, h = dil * R, pitch = TW + 2 * h;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * kTH, bc = blockIdx.z, b = bc / C;
     const size_t HW = (size_t)H * W;
-    stage(tile, pitch, cur + (size_t)bc * HW, nullptr, x0, y0, h, H, W);
+    stage<kTX, kTY, kTH>(tile, pitch, cur + (size_t)bc * HW, nullptr, x0, y0, h, H, W);
     __syncthreads();
     const float* wk = kern + (size_t)b * KK * HW;
     const int tx = threadIdx.x * VEC, x = x0 + tx;
@@ -133,7 +104,7 @@ dil_adjoint_kernel(const float* __restrict__ kern, const float* __restrict__ lam
     const int h = dil * R, pitch = kTX + 2 * h;
     const int x0 = blockIdx.x * kTX, y0 = blockIdx.y * kTH, bc = blockIdx.z, b = bc / C;
     const size_t HW = (size_t)H * W;
-    stage(tile, pitch, lam_in + (size_t)bc * HW, conf ? conf + (size_t)b * HW : nullptr, x0, y0, h, H, W);
+    stage<kTX, kTY, kTH>(tile, pitch, lam_in + (size_t)bc * HW, conf ? conf + (size_t)b * HW : nullptr, x0, y0, h, H, W);
     __syncthreads();
     const float* wk = kern + (size_t)b * KK * HW;
     const int tx = threadIdx.x, x = x0 + tx;
@@ -246,8 +217,6 @@ dil_finalize_kernel(const float* __restrict__ kern, const float* __restrict__ d0
     }
 }
 
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 size_t tile_smem(int VEC, int h) { return (size_t)(kTH + 2 * h) * (kTX * VEC + 2 * h) * sizeof(float); }
 
 template <int K>
@@ -267,14 +236,6 @@ int launch_step(bool vec, const float* kern, const float* d0, const float* cur, 
         dil_step_kernel<K, 1, false><<<grid, block, sm, st>>>(kern, d0, cur, sparse, conf, dst, C, H, W, dil);
     CSPN_CUDA_TRY(cudaGetLastError());
     return CSPN_OK;
-}
-
-// The 4-pixel path: W % 4 == 0 and every plane it reads or writes with 16-byte accesses aligned
-bool vec_ok(int W, std::initializer_list<const void*> ptrs) {
-    if (W % 4) return false;
-    for (const void* p : ptrs)
-        if (p && !aligned16(p)) return false;
-    return true;
 }
 
 template <int K>

@@ -37,6 +37,12 @@
 //   propagate2d_dilated_backward(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, Tensor grad_out,
 //                                int kernel_size, int dilation, int prop_time, bool need_kernel, bool need_blur,
 //                                bool need_sparse, bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor)
+//   propagate2d_dynamic(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence,
+//                       int kernel_size) -> Tensor   (DySPN's step: affinity (B, K*K, H, W), attention (B, N*(K+1)/2, H, W),
+//                       sparse_depth and confidence (B, 1, H, W), both or neither, K in {3, 5, 7})
+//   propagate2d_dynamic_backward(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence,
+//                                Tensor grad_out, int kernel_size, bool need_affinity, bool need_attention, bool need_blur,
+//                                bool need_sparse, bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor, Tensor)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -447,6 +453,71 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_dilated_b
                                 (int)dilation, (int)prop_time, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_dil_bwd_f32");
     return {grad_or_empty(gk, k), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gm, d)};
+}
+
+// Dynamic propagation, K in {3, 5, 7}: cspn2d_dyn_*_f32.  affinity (B, K*K, H, W), attention (B, N*(K+1)/2, H, W), blur_depth
+// (B, C, H, W), sparse_depth and confidence (B, 1, H, W), both or neither.  Returns N.
+int64_t check2d_dyn(const at::Tensor& aff, const at::Tensor& att, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+                    const std::optional<at::Tensor>& conf, int64_t K) {
+    TORCH_CHECK_VALUE(kernel_size_ok(K, 2), "kernel_size must be 3, 5 or 7, got ", K);
+    TORCH_CHECK_VALUE(sparse.has_value() == conf.has_value(), "sparse_depth and confidence come together or not at all");
+    TORCH_CHECK_VALUE(blur.dim() == 4 && blur.numel() > 0, "blur_depth must be a non-empty (B,C,H,W), got ", blur.sizes());
+    const int64_t B = blur.size(0), C = blur.size(1), H = blur.size(2), W = blur.size(3), NR = (K + 1) / 2;
+    TORCH_CHECK_VALUE(aff.dim() == 4 && aff.size(0) == B && aff.size(1) == K * K && aff.size(2) == H && aff.size(3) == W,
+                      "affinity must be (B, K*K, H, W) = (", B, ", ", K * K, ", ", H, ", ", W, "), got ", aff.sizes());
+    TORCH_CHECK_VALUE(att.dim() == 4 && att.size(0) == B && att.size(1) % NR == 0 && att.size(2) == H && att.size(3) == W &&
+                              att.size(1) <= INT32_MAX,
+                      "attention must be (B, N*(K+1)/2, H, W) with (K+1)/2 = ", NR, " and H, W = ", H, ", ", W, ", got ", att.sizes());
+    TORCH_CHECK(aff.scalar_type() == at::kFloat && att.scalar_type() == at::kFloat && blur.scalar_type() == at::kFloat,
+                "cspn_b200 is fp32 only");
+    TORCH_CHECK(aff.device() == blur.device() && att.device() == blur.device(), "affinity, attention and blur_depth are on different devices");
+    for (const auto* t : {&sparse, &conf})
+        if (t->has_value()) {
+            TORCH_CHECK_VALUE((*t)->dim() == 4 && (*t)->size(0) == B && (*t)->size(1) == 1 && (*t)->size(2) == H && (*t)->size(3) == W,
+                              "sparse_depth and confidence must be (B, 1, H, W) = (", B, ", 1, ", H, ", ", W, "), got ", (*t)->sizes());
+            TORCH_CHECK((*t)->scalar_type() == at::kFloat && (*t)->device() == blur.device(),
+                        "sparse_depth and confidence must be fp32 on the device of blur_depth");
+        }
+    TORCH_CHECK(B * C <= 65535 && (H + 15) / 16 <= 65535 && W < ((int64_t)1 << 31),
+                "propagate2d_dynamic takes B*C <= 65535 and ceil(H/16) <= 65535, got blur_depth ", blur.sizes());
+    return att.size(1) / NR;
+}
+
+at::Tensor propagate2d_dynamic_cuda(const at::Tensor& aff, const at::Tensor& att, const at::Tensor& blur,
+                                    const std::optional<at::Tensor>& sparse, const std::optional<at::Tensor>& conf, int64_t K) {
+    const int64_t N = check2d_dyn(aff, att, blur, sparse, conf, K);
+    if (N == 0) return blur.clone();                   // a dispatcher op may not return its input
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor a = aff.contiguous(), at_ = att.contiguous(), d = blur.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    const at::Tensor m = conf.has_value() ? conf->contiguous() : at::Tensor();
+    at::Tensor out = at::empty_like(d);
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const Workspace ws(cspn2d_dyn_workspace_bytes(B, C, H, W, (int)K, (int)N), d);
+    check_rc(cspn2d_dyn_fwd_f32(fptr(a), fptr(at_), fptr(d), fptr(s), fptr(m), mptr(out), B, C, H, W, (int)K, (int)N, ws.ptr(), ws.bytes,
+                                current_stream()),
+             "cspn2d_dyn_fwd_f32");
+    return out;
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate2d_dynamic_backward_cuda(
+        const at::Tensor& aff, const at::Tensor& att, const at::Tensor& blur, const std::optional<at::Tensor>& sparse,
+        const std::optional<at::Tensor>& conf, const at::Tensor& grad_out, int64_t K, bool need_a, bool need_att, bool need_d, bool need_s,
+        bool need_m) {
+    const int64_t N = check2d_dyn(aff, att, blur, sparse, conf, K);
+    check_grad_out(grad_out, blur, "blur_depth");
+    const c10::cuda::CUDAGuard guard(blur.device());
+    const at::Tensor a = aff.contiguous(), at_ = att.contiguous(), d = blur.contiguous(), go = grad_out.contiguous();
+    const at::Tensor s = sparse.has_value() ? sparse->contiguous() : at::Tensor();
+    const at::Tensor m = conf.has_value() ? conf->contiguous() : at::Tensor();
+    at::Tensor ga = new_grad(need_a, a), gt = new_grad(need_att, at_), gd = new_grad(need_d, d);
+    at::Tensor gs = s.defined() ? new_grad(need_s, s) : at::Tensor(), gm = m.defined() ? new_grad(need_m, m) : at::Tensor();
+    const int B = (int)d.size(0), C = (int)d.size(1), H = (int)d.size(2), W = (int)d.size(3);
+    const Workspace ws(cspn2d_dyn_bwd_workspace_bytes(B, C, H, W, (int)K, (int)N), d);
+    check_rc(cspn2d_dyn_bwd_f32(fptr(a), fptr(at_), fptr(d), fptr(s), fptr(m), fptr(go), mptr(ga), mptr(gt), mptr(gd), mptr(gs), mptr(gm), B,
+                                C, H, W, (int)K, (int)N, ws.ptr(), ws.bytes, current_stream()),
+             "cspn2d_dyn_bwd_f32");
+    return {grad_or_empty(ga, a), grad_or_empty(gt, at_), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gm, d)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -1085,6 +1156,11 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate2d_dilated_backward(Tensor kernel, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, Tensor grad_out, "
           "int kernel_size, int dilation, int prop_time, bool need_kernel, bool need_blur, bool need_sparse, bool need_confidence) -> "
           "(Tensor, Tensor, Tensor, Tensor)");
+    m.def("propagate2d_dynamic(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, "
+          "int kernel_size) -> Tensor");
+    m.def("propagate2d_dynamic_backward(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, "
+          "Tensor grad_out, int kernel_size, bool need_affinity, bool need_attention, bool need_blur, bool need_sparse, "
+          "bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -1135,6 +1211,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_nonlocal_backward", &propagate2d_nonlocal_backward_cuda);
     m.impl("propagate2d_dilated", &propagate2d_dilated_cuda);
     m.impl("propagate2d_dilated_backward", &propagate2d_dilated_backward_cuda);
+    m.impl("propagate2d_dynamic", &propagate2d_dynamic_cuda);
+    m.impl("propagate2d_dynamic_backward", &propagate2d_dynamic_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

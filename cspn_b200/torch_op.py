@@ -211,6 +211,44 @@ def _register():
 
     lib.register_autograd('cspn_b200::propagate2d_dilated', backward2d_dilated, setup_context=setup2d_dilated)
 
+    @lib.register_fake('cspn_b200::propagate2d_dynamic')
+    def _(affinity, attention, blur_depth, sparse_depth, confidence, kernel_size):
+        torch._check(kernel_size in (3, 5, 7), lambda: 'kernel_size must be 3, 5 or 7')
+        torch._check(affinity.dim() == 4 and attention.dim() == 4 and blur_depth.dim() == 4,
+                     lambda: 'affinity, attention and blur_depth must be 4D')
+        torch._check(affinity.shape[1] == kernel_size * kernel_size,
+                     lambda: f'a {kernel_size}x{kernel_size} kernel needs (B,{kernel_size * kernel_size},H,W) affinities')
+        torch._check(attention.shape[1] % ((kernel_size + 1) // 2) == 0,
+                     lambda: f'the attention needs a multiple of {(kernel_size + 1) // 2} channels')
+        torch._check((sparse_depth is None) == (confidence is None), lambda: 'sparse_depth and confidence come together')
+        return torch.empty_like(blur_depth, memory_format=torch.contiguous_format)
+
+    @lib.register_fake('cspn_b200::propagate2d_dynamic_backward')
+    def _(affinity, attention, blur_depth, sparse_depth, confidence, grad_out, kernel_size, need_affinity, need_attention, need_blur,
+          need_sparse, need_confidence):
+        new = lambda need, x: torch.empty_like(x, memory_format=torch.contiguous_format) if need else blur_depth.new_empty(0)
+        gs = new(need_sparse, sparse_depth) if sparse_depth is not None else blur_depth.new_empty(0)
+        gm = new(need_confidence, confidence) if confidence is not None else blur_depth.new_empty(0)
+        return new(need_affinity, affinity), new(need_attention, attention), new(need_blur, blur_depth), gs, gm
+
+    def setup2d_dynamic(ctx, inputs, output):
+        affinity, attention, blur_depth, sparse_depth, confidence, kernel_size = inputs
+        ctx.save_for_backward(affinity, attention, blur_depth, sparse_depth, confidence)
+        ctx.kernel_size = kernel_size
+
+    def backward2d_dynamic(ctx, grad_out):
+        affinity, attention, blur_depth, sparse_depth, confidence = ctx.saved_tensors
+        need_a, need_t, need_d = ctx.needs_input_grad[:3]
+        need_s = ctx.needs_input_grad[3] and sparse_depth is not None
+        need_m = ctx.needs_input_grad[4] and confidence is not None
+        ga, gt, gd, gs, gm = torch.ops.cspn_b200.propagate2d_dynamic_backward(
+            affinity, attention, blur_depth, sparse_depth, confidence, grad_out.contiguous(), ctx.kernel_size, need_a, need_t, need_d,
+            need_s, need_m)
+        return ((ga if need_a else None), (gt if need_t else None), (gd if need_d else None), (gs if need_s else None),
+                (gm if need_m else None), None)
+
+    lib.register_autograd('cspn_b200::propagate2d_dynamic', backward2d_dynamic, setup_context=setup2d_dynamic)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

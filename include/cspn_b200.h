@@ -304,6 +304,42 @@ CSPN_API int cspn2d_dil_bwd_f32(const float* kernel, const float* blur, const fl
                        float* grad_confidence, int B, int C, int H, int W, int K, int dilation, int iters,
                        void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D dynamic propagation, K in {3, 5, 7}: DySPN's step (Lin et al., AAAI 2022; DESIGN.md section 4.23) ---------------
+ * affinity [B][K*K][H][W] holds all K*K taps, the centre included, as given (no abs, no normalisation), shared by the C
+ * channels: channel j = i*K + l weights d_t(p + o_j), o_j = (i - R, l - R), R = (K - 1) / 2 (F.unfold's row order).  Tap j
+ * lies on ring(j) = max(|i - R|, |l - R|).  attention [B][iters*(R+1)][H][W] holds, in channel t*(R+1) + r, the attention
+ * of ring r at step t, as given.  blur [B][C][H][W] is d_0; sparse and confidence [B][1][H][W] are s and m, both or neither.
+ * A read outside the image is 0.  iters steps of
+ *   w_j = a_{t,ring(j)} affinity_j,  rho = 1 - sum_j w_j,  v_t(p) = rho d_0(p) + sum_j w_j d_t(p + o_j),
+ *   d_{t+1} = m s + (1 - m) v_t  (d_{t+1} = v_t without samples)
+ * and out = d_N.  Order of operations (DESIGN.md section 4.23): w is one rounded product; the sum adds j ascending from w_0;
+ * v starts from the rounded product rho d_0 and adds the taps j = K*K-1 down to 0 by FMA, the centre included.
+ * The backward writes any of grad_affinity [B][K*K][H][W], grad_attention [B][iters*(R+1)][H][W], grad_blur [B][C][H][W],
+ * grad_sparse and grad_confidence [B][1][H][W] that is not NULL (the last two need the samples) and skips the work only the
+ * NULL ones need: without grad_affinity, grad_attention and grad_confidence it recomputes no iterate.  iters = 0: attention
+ * and grad_attention may be NULL (they have no channels); the forward copies blur to out, the backward copies grad_out and
+ * zero-fills grad_affinity, grad_sparse and grad_confidence (cudaMemsetAsync).
+ * Workspace (bytes, device-independent; the queries return 0 for invalid arguments): forward 4 * B*C*H*W for iters >= 2,
+ * else 0; backward 4 * (2 * iters - 1) * B*C*H*W (lambda_0 .. lambda_{N-1} and d_1 .. d_{N-1}), 0 for iters = 0.
+ * Launches: forward iters; backward at most (iters - 1) + iters + 1.  No atomics; the bits depend on the arguments only.
+ * CSPN_ERR_INVALID_ARGUMENT for a null affinity / blur / out (grad_out in the backward), a null attention with iters > 0,
+ * exactly one of sparse and confidence, a grad_sparse or grad_confidence without the samples, a non-positive shape, K not
+ * in {3, 5, 7}, iters < 0, a pointer that is not 4-byte aligned, and an output (the workspace included) that overlaps an
+ * input or another output; CSPN_ERR_UNSUPPORTED for B*C > 65535 or ceil(H/16) > 65535; CSPN_ERR_WORKSPACE for a missing or
+ * short workspace.  All of these come before any device work. */
+CSPN_API size_t cspn2d_dyn_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_dyn_fwd_f32(const float* affinity, const float* attention, const float* blur, const float* sparse,
+                       const float* confidence, float* out, int B, int C, int H, int W, int K, int iters, void* workspace,
+                       size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_dyn_bwd_workspace_bytes(int B, int C, int H, int W, int K, int iters);
+
+CSPN_API int cspn2d_dyn_bwd_f32(const float* affinity, const float* attention, const float* blur, const float* sparse,
+                       const float* confidence, const float* grad_out, float* grad_affinity, float* grad_attention,
+                       float* grad_blur, float* grad_sparse, float* grad_confidence, int B, int C, int H, int W, int K,
+                       int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
