@@ -1,13 +1,15 @@
 """The premises of tests/test_depth_ops_at_scale_gpu.py, without a GPU.  That file runs the dilated (DESIGN.md section
-4.22), aggregating (section 4.20) and non-local (section 4.21) 2D propagations across CTA tiles and at the shapes the
-README times; here:
+4.22), aggregating (section 4.20), non-local (section 4.21) and dynamic (section 4.23) 2D propagations across CTA tiles
+and at the shapes the README times; here:
 
 - the tile constants, read from the CUDA sources, and each seam shape crossing what it is meant to cross (at least three
   tiles in x and in y with a partial last tile, halos reaching into the neighbouring tile, two aggregate launch groups,
-  more than 2^27 non-local samples with a sort key wider than 16 bits).  A retuned tile fails here, not silently there.
-- the exactness the GPU file's bit-for-bit checks rest on: on the dyadic dilated cases at the seam shapes and on the
-  non-local integer-offset case at the timing shape, the fp32 restatement equals the fp64 reference, output and every
-  gradient.
+  more than 2^27 non-local samples with a sort key wider than 16 bits, a partial last block of the dynamic finalize, step
+  counts on both sides of its 64 attention slices).  A retuned tile fails here, not silently there.
+- the exactness the GPU file's bit-for-bit checks rest on: on the dyadic dilated and dynamic cases at the seam shapes
+  and on the non-local integer-offset case at the timing shape, the fp32 restatement equals the fp64 reference, output
+  and every gradient.  (The dynamic op's random-input checks need no such premise: tests/dynamic_reference.py's
+  kernel_order states the kernels' order of operations, and the GPU file compares with it bit for bit.)
 - the hot bucket: every sample of the case lands on one fractional point, so one bucket holds them all.
 
 The input generators live here so that both files use the same inputs."""
@@ -18,20 +20,24 @@ import pytest
 import torch
 
 import dilated_reference as dr
+import dynamic_reference as yr
 import nonlocal_reference as nr
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(os.path.dirname(HERE), 'cspn_b200', 'csrc')
 
 # ---- shapes (B, C, H, W) ----------------------------------------------------------------------------------------------------
-TIMING = (8, 1, 352, 1216)                          # the README's timing shape of the three ops
-DIL_SEAMS = [(2, 2, 45, 260), (1, 3, 37, 1216)]
-DIL_N = {3: 3, 5: 2, 7: 2}                          # steps of the dyadic cases: every intermediate stays exact
+TIMING = (8, 1, 352, 1216)                          # the README's timing shape of the four ops
+DIL_SEAMS = [(2, 2, 45, 260), (1, 3, 37, 1216)]     # the seam shapes of the dilated and the dynamic op
+DIL_N = {3: 3, 5: 2, 7: 2}                          # steps of the dyadic cases of both: every intermediate stays exact
 AGG_SEAMS = [(2, 2, 37, 200), (1, 1, 45, 1216)]
 AGG_STEPS = [(1, 2, 5), tuple(range(1, 71))]        # T = 70: two launch groups of the step-weight gradient
 NL_LARGE_K, NL_LARGE_N = 7, 2
 NL_HOT = (1, 2, 64, 96)
 NL_HOT_POINT = (10.25, 20.5)
+DYN_WRAP_SHAPE, DYN_WRAP_K = (1, 2, 17, 132), 5
+DYN_WRAP_N = (63, 64, 65, 70, 129)                  # one short of the 64 attention slices, one step each, then wrapping
+DYN_TIMING = [(3, 6), (5, 6), (7, 6), (5, 24)]      # (K, N) at TIMING
 
 
 def ceil_div(a, b):
@@ -54,6 +60,20 @@ def dilated_tiles():
     th = c['kTY'] * c['kRows']
     # (tile width, tile height) of the 4-pixel step, the 1-pixel step and the adjoint (always 1 pixel per thread)
     return {'vec': (4 * c['kTX'], th), 'scalar': (c['kTX'], th), 'adjoint': (c['kTX'], th)}
+
+
+def dynamic_tiles():
+    """(tiles as dilated_tiles gives them, finalize threads per block, attention slices) of cspn2d_dynamic.cu."""
+    c, _ = _constants('cspn2d_dynamic.cu', ('kTX', 'kTY', 'kRows', 'kFinThreads', 'kAttSlices'))
+    th = c['kTY'] * c['kRows']
+    return {'vec': (4 * c['kTX'], th), 'scalar': (c['kTX'], th), 'adjoint': (c['kTX'], th)}, c['kFinThreads'], c['kAttSlices']
+
+
+def attention_slices(N, slices):
+    """The steps each grid slice of the dynamic finalize forms grad_attention for: min(N, slices) slices, slice z taking
+    steps z, z + min(N, slices), ..."""
+    n = min(N, slices)
+    return [list(range(z, N, n)) for z in range(n)]
 
 
 def wide_tiles():
@@ -115,6 +135,10 @@ def nonlocal_exact(B, C, H, W, K, seed):
     return feat, offset, affinity, sparse, go
 
 
+def dyn_seed(shape, K, samples):
+    return shape[3] + 10 * K + (100 if samples else 0)
+
+
 def nl_seed(b):
     """The seed of image b of the large exact case: images are drawn one at a time, so any one is cheap to rebuild."""
     return 700 + b
@@ -140,6 +164,7 @@ def test_tile_constants_are_the_ones_the_shapes_were_chosen_for():
     assert dilated_tiles() == {'vec': (128, 16), 'scalar': (32, 16), 'adjoint': (32, 16)}
     assert wide_tiles() == ({'vec': (64, 16), 'scalar': (32, 8)}, 64)
     assert nonlocal_grid() == (128, 1 << 20)
+    assert dynamic_tiles() == ({'vec': (128, 16), 'scalar': (32, 16), 'adjoint': (32, 16)}, 128, 64)
 
 
 def crossings(extent, tile):
@@ -147,22 +172,54 @@ def crossings(extent, tile):
     return ceil_div(extent, tile), extent - (ceil_div(extent, tile) - 1) * tile
 
 
+def seam_tiles():
+    """The dilated and the dynamic op's tiles: both run their seam cases on DIL_SEAMS."""
+    return {'dilated': dilated_tiles(), 'dynamic': dynamic_tiles()[0]}
+
+
 @pytest.mark.parametrize('shape', DIL_SEAMS)
 def test_dilated_seam_shapes_cross_three_partial_tiles(shape):
     _, _, H, W = shape
-    tiles = dilated_tiles()
-    for path, (tw, th) in tiles.items():
-        nx, _ = crossings(W, tw)
-        ny, last_y = crossings(H, th)
-        assert nx >= 3 and ny >= 3, (path, nx, ny)
-        assert 0 < last_y < th, path                               # the last row tile is partial
-    nx, last_x = crossings(W, tiles['vec'][0])
-    assert 0 < last_x < tiles['vec'][0]                            # and so is the last 4-pixel tile in x
+    for op, tiles in seam_tiles().items():
+        for path, (tw, th) in tiles.items():
+            nx, _ = crossings(W, tw)
+            ny, last_y = crossings(H, th)
+            assert nx >= 3 and ny >= 3, (op, path, nx, ny)
+            assert 0 < last_y < th, (op, path)                         # the last row tile is partial
+        nx, last_x = crossings(W, tiles['vec'][0])
+        assert 0 < last_x < tiles['vec'][0], op                        # and so is the last 4-pixel tile in x
 
 
 def test_dilated_seam_shapes_partial_in_x_on_every_path():
-    for path, (tw, _) in dilated_tiles().items():
-        assert any(0 < crossings(W, tw)[1] < tw for _, _, _, W in DIL_SEAMS), path
+    for op, tiles in seam_tiles().items():
+        for path, (tw, _) in tiles.items():
+            assert any(0 < crossings(W, tw)[1] < tw for _, _, _, W in DIL_SEAMS), (op, path)
+
+
+def test_dynamic_shapes_leave_a_partial_finalize_block():
+    """The finalize runs ceil(H*W / kFinThreads) blocks per image; at the seam, slice-wrap and degenerate shapes the last
+    one is partial, so a block count one short leaves pixels unwritten there."""
+    _, threads, _ = dynamic_tiles()
+    for _, _, H, W in DIL_SEAMS + [DYN_WRAP_SHAPE]:
+        assert (H * W) % threads != 0, (H, W)
+    assert ceil_div(DYN_WRAP_SHAPE[2] * DYN_WRAP_SHAPE[3], threads) == 18
+    tiles = dynamic_tiles()[0]
+    _, _, H, W = DYN_WRAP_SHAPE
+    assert crossings(W, tiles['vec'][0])[0] == 2 and crossings(H, tiles['vec'][1])[0] == 2   # and a seam in x and y
+
+
+def test_dynamic_slice_wrap_step_counts():
+    """N = 63 uses 63 of the 64 attention slices, N = 64 all of them with one step each; from N = 65 on slice 0 takes
+    step 64 on a second pass, at N = 70 slices 0-5 do, and at N = 129 slice 0 takes steps 0, 64 and 128."""
+    _, _, slices = dynamic_tiles()
+    plan = {N: attention_slices(N, slices) for N in DYN_WRAP_N}
+    for N, p in plan.items():
+        assert sorted(t for steps in p for t in steps) == list(range(N)), N    # every step once
+    assert len(plan[63]) == 63 and all(len(x) == 1 for x in plan[63])
+    assert len(plan[64]) == 64 and all(len(x) == 1 for x in plan[64])
+    assert plan[65][0] == [0, 64] and all(len(x) == 1 for x in plan[65][1:])
+    assert [z for z, x in enumerate(plan[70]) if len(x) == 2] == list(range(6)) and max(map(len, plan[70])) == 2
+    assert plan[129][0] == [0, 64, 128] and plan[129][1] == [1, 65] and plan[129][63] == [63, 127]
 
 
 @pytest.mark.parametrize('K', [3, 5, 7])
@@ -239,6 +296,19 @@ def test_dilated_dyadic_cases_are_exact_at_the_seam_shapes(K, dil, samples, shap
     ref = dr.grads(dr.composition, *ins, K, dil, DIL_N[K], go, dtype=torch.float64)
     r32 = dr.grads(dr.explicit, *ins, K, dil, DIL_N[K], go)
     for name, x, y in zip(('out', 'kernel', 'blur', 'sparse', 'conf'), r32, ref):
+        assert (x is None) == (y is None), name
+        assert x is None or torch.equal(x, y.float()), name
+
+
+@pytest.mark.parametrize('K', [3, 5, 7])
+@pytest.mark.parametrize('samples', [None, 'soft'])
+@pytest.mark.parametrize('shape', DIL_SEAMS)
+def test_dynamic_dyadic_cases_are_exact_at_the_seam_shapes(K, samples, shape):
+    """The kernel-order restatement gives the fp64 composition's values on the dyadic cases, output and every gradient:
+    every intermediate is exact, so the GPU file may compare the library with fp64 bit for bit there."""
+    ins, go = yr.dyadic_inputs(*shape, K, DIL_N[K], samples, dyn_seed(shape, K, samples))
+    ref = yr.grads(yr.composition, *ins, K, go, dtype=torch.float64)
+    for name, x, y in zip(('out', 'affinity', 'attention', 'blur', 'sparse', 'conf'), yr.kernel_order(*ins, K, go), ref):
         assert (x is None) == (y is None), name
         assert x is None or torch.equal(x, y.float()), name
 

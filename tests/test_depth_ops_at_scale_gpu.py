@@ -1,19 +1,22 @@
-"""GPU tests of the dilated (DESIGN.md section 4.22), aggregating (section 4.20) and non-local (section 4.21) 2D
-propagations across CTA tiles and at 8x1x352x1216, the shape the README times them at.  The small images of
-test_dilated_gpu.py, test_aggregate_gpu.py and test_nonlocal_gpu.py fit in one or two tiles; here the 4-pixel and 1-pixel
-paths read their halos from neighbouring tiles (shapes in tests/test_depth_ops_at_scale_cpu.py, which also checks that
-they cross what they are meant to cross and that the exact cases are exact), the step-weight gradient runs in two launch
-groups, and the non-local backward index runs past 2^27 samples (a second grid-stride pass of its entries kernel, a
-22-bit sort key) and with every sample in one bucket.
+"""GPU tests of the dilated (DESIGN.md section 4.22), aggregating (section 4.20), non-local (section 4.21) and dynamic
+(section 4.23) 2D propagations across CTA tiles and at 8x1x352x1216, the shape the README times them at.  The small
+images of test_dilated_gpu.py, test_aggregate_gpu.py, test_nonlocal_gpu.py and test_dynamic_gpu.py fit in one or two
+tiles; here the 4-pixel and 1-pixel paths read their halos from neighbouring tiles (shapes in
+tests/test_depth_ops_at_scale_cpu.py, which also checks that they cross what they are meant to cross and that the exact
+cases are exact), the step-weight gradient runs in two launch groups, the non-local backward index runs past 2^27
+samples (a second grid-stride pass of its entries kernel, a 22-bit sort key) and with every sample in one bucket, and
+the dynamic finalize's 64 attention slices take a second and a third pass over the steps (N up to 129).
 
 Oracles: bit equality with an order-free reference where one exists (dyadic and integer-offset cases against fp64,
 separate propagations for the aggregate's forward, the other path or the batch split), else the op's own tolerance
-against fp64: `within` for the dilated op, ar.within for the aggregate's gradients, and for the non-local op a normwise
-distance at most 4x that of its eager fp32 restatement.  At the timing shape the library runs B = 8 and the fp64
-reference the first two images.
+against fp64: `within` for the dilated and dynamic ops, ar.within for the aggregate's gradients, and for the non-local
+op a normwise distance at most 4x that of its eager fp32 restatement.  The dynamic op also has an order-exact oracle,
+tests/dynamic_reference.py's kernel_order: on random inputs every output and gradient has its bits.  At the timing
+shape the library runs B = 8 and the fp64 reference the first two images (kernel_order all eight).
 
 First runs, on an NVIDIA H100 80GB HBM3 at a 700 W power limit: every bit-for-bit check held, the largest tolerance
-ratios are in each test's docstring, and the file's 201 tests took 62-66 s.
+ratios are in each test's docstring, and the file's 201 tests of the first three ops took 62-66 s; the dynamic op's 81
+took 69 s, and the whole file's 282 took 107 s.
 """
 import ctypes
 
@@ -25,6 +28,7 @@ from cspn_b200 import _lib
 from cspn_b200.cspn import _propagate2d_keep, norm_code_2d_k
 import aggregate_reference as ar
 import dilated_reference as dr
+import dynamic_reference as yr
 import memory_contract as mc
 import nonlocal_reference as nr
 import test_depth_ops_at_scale_cpu as pre
@@ -33,6 +37,7 @@ pytestmark = pytest.mark.gpu
 DIL_NAMES = ('out', 'kernel', 'blur', 'sparse', 'conf')
 AGG_NAMES = ('out', 'grad_guidance', 'grad_blur', 'grad_sparse', 'grad_step_weight')
 NL_NAMES = ('out', 'feat', 'offset', 'affinity', 'sparse')
+DYN_NAMES = ('out', 'affinity', 'attention', 'blur', 'sparse', 'conf')
 
 
 def bits(a, b):
@@ -76,11 +81,11 @@ def dil_ref(ins, K, dil, N, go):
     return dr.grads(dr.composition, *cuda(ins), K, dil, N, go.cuda(), dtype=torch.float64)
 
 
-def dil_within(got, ref, fwd_tol=1e-5, grad_tol=2e-3):
-    """test_dilated_gpu.py's `within`, element by element (a NaN fails it), returning the largest |got - ref| / bound
-    per name for the record."""
+def dil_within(got, ref, fwd_tol=1e-5, grad_tol=2e-3, names=DIL_NAMES):
+    """test_dilated_gpu.py's `within` (and test_dynamic_gpu.py's, with names=DYN_NAMES), element by element (a NaN fails
+    it), returning the largest |got - ref| / bound per name for the record."""
     out = {}
-    for name, g, r in zip(DIL_NAMES, got, ref):
+    for name, g, r in zip(names, got, ref):
         assert (g is None) == (r is None), name
         if r is not None:
             tol = fwd_tol if name == 'out' else grad_tol
@@ -431,3 +436,150 @@ def test_memory_contract_nonlocal_at_a_seam_shape():
     assert mc.unchanged(before, [f, o, a, s, go])
     want = nl_run(f, o, a, s, K, N, go)
     assert bits(out, want[0]) and all(bits(x, y) for x, y in zip(grads, want[1:]))
+
+
+# ---- dynamic ------------------------------------------------------------------------------------------------------------------
+def dyn_op(a, t, b, s, m, K):
+    return cspn_b200.propagate2d_dynamic(a, t, b, s, m, K)
+
+
+def dyn_run(ins, K, go):
+    return yr.grads(dyn_op, *ins, K, go)
+
+
+def dyn_ref(ins, K, go):
+    return yr.grads(yr.composition, *cuda(ins), K, go.cuda(), dtype=torch.float64)
+
+
+def dyn_bits(got, want, what):
+    for name, g, r in zip(DYN_NAMES, got, want):
+        assert bits(g, r), (what, name)
+
+
+def dyn_within(got, ref):
+    return dil_within(got, ref, names=DYN_NAMES)
+
+
+DYN_SEAM_N = 5
+
+
+@pytest.mark.parametrize('aligned', [True, False])
+@pytest.mark.parametrize('K', [3, 5, 7])
+@pytest.mark.parametrize('samples', [None, 'soft'])
+@pytest.mark.parametrize('shape', pre.DIL_SEAMS)
+def test_dynamic_seams_bit_for_bit(shape, samples, K, aligned):
+    """Three or more tiles in x and y with partial last tiles, and a partial last finalize block; aligned: the 4-pixel
+    step, else the 1-pixel one.  Dyadic inputs give the fp64 composition's bits; random ones, N = 5, the bits of the
+    kernels' stated order of operations (yr.kernel_order), which no order-free reference can check."""
+    ins, go = yr.dyadic_inputs(*shape, K, pre.DIL_N[K], samples, pre.dyn_seed(shape, K, samples))
+    ref = dyn_ref(ins, K, go)
+    got = dyn_run(place(cuda(ins), aligned), K, go.cuda())
+    for name, g, r in zip(DYN_NAMES, got, ref):
+        assert (g is None) == (r is None), name
+        assert r is None or torch.equal(g, r.float()), ('dyadic', name)
+    ins = yr.make_inputs(*shape, K, DYN_SEAM_N, samples, seed=pre.dyn_seed(shape, K, samples), device='cuda')
+    go = randn(*shape, seed=K)
+    dyn_bits(dyn_run(place(ins, aligned), K, go), yr.kernel_order(*ins, K, go), 'random')
+
+
+@pytest.mark.parametrize('K', [7, 3])
+@pytest.mark.parametrize('samples', [None, 'soft'])
+@pytest.mark.parametrize('H,W', DEGENERATE)
+def test_dynamic_degenerate_shapes(H, W, samples, K):
+    """1 x W, H x 1, one 4-pixel thread (W = 4) and images smaller than the R = 3 halo of K = 7, N = 5: the bits of
+    yr.kernel_order, and within `within` of fp64.  First H100 run: largest ratio to the bound 0.031 (out, 9x11, K = 7),
+    0.0015 for a gradient (attention, 9x11, K = 3)."""
+    ins = yr.make_inputs(2, 2, H, W, K, 5, samples, seed=H * 31 + W, device='cuda')
+    go = randn(2, 2, H, W)
+    got = dyn_run(ins, K, go)
+    dyn_bits(got, yr.kernel_order(*ins, K, go), 'kernel order')
+    ratios = dyn_within(got, dyn_ref(ins, K, go))
+    print(f'dynamic {H}x{W} K={K} {samples}:', ratios)
+
+
+def wrap_inputs(N, seed=0):
+    ins = yr.make_inputs(*pre.DYN_WRAP_SHAPE, pre.DYN_WRAP_K, N, 'soft', seed=N + seed, device='cuda')
+    return ins, randn(*pre.DYN_WRAP_SHAPE, seed=N + seed)
+
+
+@pytest.mark.parametrize('N', pre.DYN_WRAP_N)
+def test_dynamic_attention_slices_wrap(N):
+    """1x2x17x132, K = 5: the finalize's 64 attention slices take a second step from N = 65 on, a third at N = 129.
+    Every gradient has the bits of yr.kernel_order and is within `within` of fp64.  First H100 run: largest ratio to
+    the bound 0.052 (out, N = 70), 0.028 for a gradient (attention, N = 63); at N = 129 0.036 and 0.014, so the bound
+    holds past two wraps."""
+    ins, go = wrap_inputs(N)
+    got = dyn_run(ins, pre.DYN_WRAP_K, go)
+    dyn_bits(got, yr.kernel_order(*ins, pre.DYN_WRAP_K, go), N)
+    ratios = dyn_within(got, dyn_ref(ins, pre.DYN_WRAP_K, go))
+    print(f'dynamic slice wrap N={N}:', ratios)
+
+
+def test_dynamic_requested_gradients_past_the_attention_slices():
+    """N = 70: each requested subset gives the full call's bits.  Without the affinity gradient there are no affinity
+    slices, so the attention slices start at grid z = 0 (attention alone, and with the confidence)."""
+    K = pre.DYN_WRAP_K
+    ins, go = wrap_inputs(70, seed=1)
+    full = dyn_run(ins, K, go)
+    for need in [(0,), (1,), (2,), (3,), (4,), (0, 1), (1, 4), (2, 3)]:
+        leaves = [t.clone().requires_grad_(j in need) for j, t in enumerate(ins)]
+        gs = torch.autograd.grad(dyn_op(*leaves, K), [leaves[j] for j in need], go)
+        for j, g in zip(need, gs):
+            assert bits(g, full[1 + j]), (need, DYN_NAMES[1 + j])
+
+
+@pytest.mark.parametrize('offset', [0, 4])
+def test_memory_contract_dynamic_past_the_attention_slices(offset):
+    """N = 70 at 1x2x17x132, outputs and workspaces `offset` bytes into their allocations (4: the 1-pixel path): every
+    output word written, among them the attention gradient of steps 64-69 that the slices' second pass forms."""
+    B, C, H, W = pre.DYN_WRAP_SHAPE
+    K, N, NR = pre.DYN_WRAP_K, 70, (pre.DYN_WRAP_K + 1) // 2
+    L = _lib.lib()
+    (a, t, b, s, m), go = wrap_inputs(N, seed=offset)
+    before = mc.snapshot([a, t, b, s, m, go])
+
+    def fwd(fill):
+        out = mc.guarded(b.shape, offset)
+        ws = mc.workspace(L.cspn2d_dyn_workspace_bytes(B, C, H, W, K, N), offset, fill)
+        rc = L.cspn2d_dyn_fwd_f32(a.data_ptr(), t.data_ptr(), b.data_ptr(), s.data_ptr(), m.data_ptr(), out.ptr(), B, C, H, W, K, N,
+                                  ws.ptr(), ws.nbytes, _stream())
+        assert rc == 0, L.cspn_last_error()
+        return out, ws
+
+    def bwd(fill):
+        outs = [mc.guarded(x.shape, offset) for x in (a, t, b, s, m)]
+        ws = mc.workspace(L.cspn2d_dyn_bwd_workspace_bytes(B, C, H, W, K, N), offset, fill)
+        rc = L.cspn2d_dyn_bwd_f32(a.data_ptr(), t.data_ptr(), b.data_ptr(), s.data_ptr(), m.data_ptr(), go.data_ptr(),
+                                  *[x.ptr() for x in outs], B, C, H, W, K, N, ws.ptr(), ws.nbytes, _stream())
+        assert rc == 0, L.cspn_last_error()
+        return outs, ws
+
+    out, grads = contract(fwd, bwd, 5)
+    assert mc.n_unwritten(grads[1][:, 64 * NR:]) == 0
+    assert mc.unchanged(before, [a, t, b, s, m, go])
+    want = dyn_run((a, t, b, s, m), K, go)
+    assert bits(out, want[0]) and all(bits(x, y) for x, y in zip(grads, want[1:]))
+
+
+@pytest.mark.parametrize('K,N', pre.DYN_TIMING)
+def test_dynamic_timing_shape(K, N):
+    """8x1x352x1216, soft samples: every image bit for bit to yr.kernel_order, and images 0 and 1 within `within` of
+    the fp64 composition.  First H100 run: largest ratio to the bound 0.074 (out, K = 7, N = 6), 0.020 for a gradient
+    (attention, K = 5, N = 24)."""
+    ins = yr.make_inputs(*pre.TIMING, K, N, 'soft', seed=K * 100 + N, device='cuda')
+    go = randn(*pre.TIMING, seed=N)
+    got = dyn_run(ins, K, go)
+    dyn_bits(got, yr.kernel_order(*ins, K, go), 'kernel order')
+    ratios = dyn_within([t[:2] for t in got], dyn_ref([t[:2] for t in ins], K, go[:2]))
+    print(f'dynamic timing shape K={K} N={N}:', ratios)
+
+
+def test_dynamic_batch_split_at_the_timing_shape():
+    """K = 7, N = 6, soft samples: the B = 8 call has the bits of eight B = 1 calls."""
+    ins = yr.make_inputs(*pre.TIMING, 7, 6, 'soft', seed=8, device='cuda')
+    go = randn(*pre.TIMING, seed=8)
+    ref = dyn_run(ins, 7, go)
+    for b in range(8):
+        one = dyn_run([t[b:b + 1] for t in ins], 7, go[b:b + 1])
+        for name, x, y in zip(DYN_NAMES, one, ref):
+            assert bits(x, y[b:b + 1]), (b, name)

@@ -1,5 +1,7 @@
-"""CPU tests of the dynamic propagation (DySPN's step, DESIGN.md section 4.23): the two restatements of
-tests/dynamic_reference.py against each other in fp64, forward and autograd; the ring map; attention 1 as a fixed-weight
+"""CPU tests of the dynamic propagation (DySPN's step, DESIGN.md section 4.23): the two autograd restatements of
+tests/dynamic_reference.py against each other in fp64, forward and autograd; its fp32 FMA against exact rationals
+(midpoints where rounding in fp64 and then fp32 is wrong, signed zeros, subnormals, inf and NaN) and its kernel-order
+restatement against fp64; the ring map; attention 1 as a fixed-weight
 step; the C ABI's workspace formulas and refusals without a device; the op schemas and fake kernels; the Python refusals;
 no spills in the new translation unit; and the dilated propagation's machine code, unchanged by the shared tile helpers."""
 import hashlib
@@ -8,6 +10,7 @@ import os
 import re
 import shutil
 import subprocess
+from fractions import Fraction
 
 import pytest
 import torch
@@ -94,6 +97,164 @@ def test_steps_follow_the_attention_channels():
     one = yr.composition(aff, att[:, :2], b, K=3)
     assert one.shape == b.shape and not torch.equal(one, b)
     assert torch.equal(yr.composition(aff, att[:, :0], b, K=3), b)
+
+
+# ---- the kernels' order of operations ------------------------------------------------------------------------------------
+def f32(x):
+    return torch.tensor(x, dtype=torch.float32)
+
+
+def exact_f32(q):
+    """The Fraction q rounded to fp32, to nearest with ties to even, subnormals included, as a Python float."""
+    if q == 0:
+        return 0.0
+    sign, q = (-1.0 if q < 0 else 1.0), abs(q)
+    e = q.numerator.bit_length() - q.denominator.bit_length()        # 2^(e-1) <= q < 2^(e+1)
+    e = max(e - 24, -149)                                             # 24 significant bits, or the subnormal quantum
+    while q / Fraction(2) ** e >= 2 ** 24:
+        e += 1
+    m = round(q / Fraction(2) ** e)                                   # Fraction.__round__ ties to even
+    v = m * Fraction(2) ** e
+    if v >= Fraction(2) ** 128:
+        return sign * float('inf')
+    return sign * float(v)
+
+
+def fma_exact(a, b, c):
+    return exact_f32(Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c)))
+
+
+def naive(a, b, c):
+    """a*b + c rounded in fp64, then to fp32: the double rounding yr.fma avoids."""
+    return (a.double() * b.double() + c.double()).float()
+
+
+def f32_bits(x):
+    return int(torch.tensor(x, dtype=torch.float32).view(torch.int32))
+
+
+def test_fma_rounds_once_on_random_triples():
+    """Exponents over the whole fp32 range, products near -c so that the sum cancels, and results in the subnormal
+    range, against the exact value in Fractions rounded once."""
+    g = torch.Generator().manual_seed(0)
+    n = 3000
+    a = torch.randn(n, generator=g) * torch.exp2(torch.randint(-60, 60, (n,), generator=g).float())
+    b = torch.randn(n, generator=g) * torch.exp2(torch.randint(-60, 60, (n,), generator=g).float())
+    c = torch.randn(n, generator=g) * torch.exp2(torch.randint(-120, 120, (n,), generator=g).float())
+    near = torch.arange(n) % 3 == 1
+    c = torch.where(near, -(a * b) * (1 + torch.randn(n, generator=g) * 2 ** -20), c)         # cancellation
+    sub = torch.arange(n) % 3 == 2
+    a = torch.where(sub, torch.randn(n, generator=g) * 2 ** -70, a)                          # subnormal results
+    b = torch.where(sub, torch.randn(n, generator=g) * 2 ** -70, b)
+    c = torch.where(sub, torch.randn(n, generator=g) * 2 ** -135, c)
+    got = yr.fma(a, b, c)
+    want = torch.tensor([fma_exact(x, y, z) for x, y, z in zip(a.tolist(), b.tolist(), c.tolist())], dtype=torch.float32)
+    assert torch.equal(got.view(torch.int32), want.view(torch.int32))
+    assert int(((want != 0) & (want.abs() < 2 ** -126)).sum()) > 300                          # subnormals reached
+
+
+def midpoint_cases():
+    """(a, b, c) whose exact a*b + c lies within 2^-46 of an ulp of c from an fp32 midpoint, on the side the fp64 sum
+    cannot see: a*b = 2^-24 (1 - 2^-46) = (1 + 2^-23) * 2^-24 (1 - 2^-23) just below half an ulp of c = 1 + k 2^-23, or
+    2^-24 (1 + 4688 * 2^-46) = (1 + 2896 * 2^-23) * 2^-24 (1 - 2895 * 2^-23) just above it.  The fp64 sum rounds onto
+    the midpoint, and the fp32 tie then goes to the even neighbour, which is wrong when the exact value lies on the odd
+    side.  Scaled by powers of two and negated, so both signs and other binades are covered."""
+    below = (1 + 2 ** -23, 2 ** -24 * (1 - 2 ** -23))
+    above = (1 + 2896 * 2 ** -23, 2 ** -24 * (1 - 2895 * 2 ** -23))
+    out = []
+    for s in (1.0, -1.0):
+        for e in (0, 40, -40, -100):
+            sc = 2.0 ** e
+            out.append((below[0] * s, below[1] * sc, (1 + 2 ** -23) * s * sc))   # c odd: the tie goes up, exact is below
+            out.append((above[0] * s, above[1] * sc, (1 + 2 ** -22) * s * sc))   # c even: the tie stays, exact is above
+    return out
+
+
+def test_fma_is_right_where_the_fp64_then_fp32_rounding_is_wrong():
+    for a, b, c in midpoint_cases():
+        ta, tb, tc = f32([a]), f32([b]), f32([c])
+        assert (float(ta), float(tb), float(tc)) == (a, b, c)                           # exact fp32 operands
+        want = fma_exact(a, b, c)
+        assert f32_bits(float(yr.fma(ta, tb, tc))) == f32_bits(want), (a, b, c)
+        assert float(naive(ta, tb, tc)) != want, (a, b, c)                              # the double rounding's error
+        assert abs(f32_bits(float(naive(ta, tb, tc))) - f32_bits(want)) == 1                # of one ulp
+
+
+def test_fma_signed_zeros_and_special_operands():
+    inf, nan, big, tiny = float('inf'), float('nan'), 3.4028234663852886e38, 2.0 ** -100
+    cases = [  # (a, b, c, IEEE fmaf)
+        (-0.0, 1.0, 0.0, 0.0), (-0.0, 1.0, -0.0, -0.0), (0.0, -1.0, -0.0, -0.0), (0.0, 1.0, -0.0, 0.0),
+        (1.0, -1.0, 1.0, 0.0), (-1.0, 1.0, 1.0, 0.0),                          # exact cancellation: +0 to nearest
+        (tiny, -tiny, 0.0, -0.0), (tiny, tiny, -0.0, 0.0), (tiny, -tiny, -0.0, -0.0),   # underflow keeps the sign
+        (2.0 ** -75, 2.0 ** -75, 0.0, 2.0 ** -149 * 0),                        # 2^-150: a tie, to the even 0
+        (2.0 ** -75, 1.5 * 2.0 ** -75, 0.0, 2.0 ** -149),                      # 1.5 * 2^-150 rounds up
+        (2.0 ** -70, 2.0 ** -70, 2.0 ** -149, 2.0 ** -149 + 2.0 ** -140),      # subnormal sum, exact
+        (inf, 0.0, 1.0, nan), (0.0, -inf, 1.0, nan), (inf, 2.0, -inf, nan), (inf, 2.0, 1.0, inf), (-inf, 2.0, 1.0, -inf),
+        (2.0, 3.0, inf, inf), (2.0, 3.0, -inf, -inf), (nan, 0.0, 1.0, nan), (1.0, 1.0, nan, nan),
+        (big, 2.0, -inf, -inf), (big, 2.0, 0.0, inf), (big, -2.0, 0.0, -inf), (big, 2.0, -big, big),   # no overflow
+        (big, 1.0, big * 2.0 ** -24, inf), (big, 1.0, big * 2.0 ** -25, big),   # past max + half an ulp, and below it
+    ]
+    for a, b, c, want in cases:
+        got = float(yr.fma(f32([a]), f32([b]), f32([c])))
+        if want != want:
+            assert got != got, (a, b, c)
+        else:
+            assert f32_bits(got) == f32_bits(want), (a, b, c, got, want)
+            if abs(want) != inf and want != 0:                          # a Fraction has no signed zero
+                assert f32_bits(got) == f32_bits(fma_exact(a, b, c)), (a, b, c)
+
+
+def assert_within(got, ref, fwd_tol=1e-5, grad_tol=2e-3):
+    """test_dynamic_gpu.py's `within`: element by element, relative to |ref| plus its mean."""
+    for name, g, r in zip(NAMES, got, ref):
+        assert (g is None) == (r is None), name
+        if r is not None:
+            tol = fwd_tol if name == 'out' else grad_tol
+            bound = tol * (r.abs() + r.abs().mean())
+            assert bool(((g.double() - r).abs() <= bound).all()), name
+
+
+@pytest.mark.parametrize('K', [3, 5, 7])
+@pytest.mark.parametrize('samples', [None, 'soft', 'hard'])
+@pytest.mark.parametrize('shape,N', [((2, 3, 9, 11), 4), ((1, 1, 1, 13), 3), ((2, 2, 10, 1), 2), ((1, 2, 2, 3), 1)])
+def test_kernel_order_within_tolerance_of_fp64(K, samples, shape, N):
+    """Random inputs, the op's tolerance; 1 x W and H x 1 images and an image smaller than the halo included."""
+    ins = yr.make_inputs(*shape, K, N, samples, seed=K * 3 + N)
+    go = torch.randn(shape, generator=torch.Generator().manual_seed(2))
+    got = yr.kernel_order(*ins, K, go)
+    assert [None if g is None else tuple(g.shape) for g in got] == [None if t is None else tuple(t.shape) for t in
+                                                                     [ins[2], ins[0], ins[1], ins[2], ins[3], ins[4]]]
+    assert_within(got, yr.grads(yr.composition, *ins, K, go, dtype=D))
+
+
+@pytest.mark.parametrize('K,N', [(3, 3), (5, 2), (7, 2)])
+@pytest.mark.parametrize('samples', [None, 'soft', 'hard'])
+def test_kernel_order_equals_fp64_on_dyadic_inputs(K, N, samples):
+    ins, go = yr.dyadic_inputs(2, 2, 11, 13, K, N, samples, seed=K + N)
+    ref = yr.grads(yr.composition, *ins, K, go, dtype=D)
+    for name, g, r in zip(NAMES, yr.kernel_order(*ins, K, go), ref):
+        assert (g is None) == (r is None), name
+        assert g is None or torch.equal(g, r.float()), name
+
+
+def test_kernel_order_follows_the_stated_order():
+    """The restatement is not order-free: summing S with j descending, or swapping G1's channel order, changes bits
+    on random inputs.  So a kernel that did either would fail the bit-for-bit checks the restatement serves."""
+    K, N = 5, 3
+    ins = yr.make_inputs(1, 3, 12, 14, K, N, 'soft', seed=9)
+    go = torch.randn(1, 3, 12, 14, generator=torch.Generator().manual_seed(3))
+    a, t, b, s, m = ins
+    got = yr.kernel_order(*ins, K, go)
+    # channel order: with the channels reversed, G1 and G0 add them in the other order
+    rev = yr.kernel_order(a, t, b.flip(1), s, m, K, go.flip(1))
+    assert torch.equal(rev[0], got[0].flip(1))                                       # the forward is per channel
+    assert not torch.equal(rev[1], got[1]) and not torch.equal(rev[2], got[2])       # the channel sums are not
+    # tap order of S: on these inputs 1 - S in another order differs in at least one pixel
+    w = [t[:, yr.rings(K)[j]:yr.rings(K)[j] + 1] * a[:, j:j + 1] for j in range(K * K)]
+    up, down = w[0], w[-1]
+    for j in range(1, K * K):
+        up, down = up + w[j], down + w[K * K - 1 - j]
+    assert not torch.equal(up, down)
 
 
 # ---- the library's surface without a device -----------------------------------------------------------------------------

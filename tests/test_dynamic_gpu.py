@@ -1,5 +1,6 @@
 """GPU tests of propagate2d_dynamic (DySPN's step, DESIGN.md section 4.23): the forward and every gradient against the fp64
-composition of tests/dynamic_reference.py, bit for bit on dyadic cases across CTA tile seams, the 4-pixel and 1-pixel
+composition of tests/dynamic_reference.py and bit for bit against its kernel_order, bit for bit on dyadic cases across CTA
+tile seams, the 4-pixel and 1-pixel
 paths, the anchor to propagate2d_dilated, the IEEE masks, determinism, the requested gradients and launch counts, the
 memory contract, the DySPN head end to end (INTEGRATION.md section 2h), torch.compile and opcheck."""
 import pytest
@@ -55,7 +56,11 @@ def test_forward_and_gradients_within_tolerance_of_fp64(K, N, samples):
     W = (48, 45)[(case // 2) % 2]
     ins = yr.make_inputs(2, C, 29, W, K, N, samples, seed=case * 31 + N, device='cuda')
     go = torch.randn(2, C, 29, W, device='cuda')
-    within(run(ins, K, go), yr.grads(yr.composition, *ins, K, go, dtype=torch.float64))
+    got = run(ins, K, go)
+    within(got, yr.grads(yr.composition, *ins, K, go, dtype=torch.float64))
+    # and the bits of the kernels' stated order of operations
+    for name, g, r in zip(NAMES, got, yr.kernel_order(*ins, K, go)):
+        assert bits(g, r), name
 
 
 @pytest.mark.parametrize('K', [3, 7])
@@ -88,29 +93,13 @@ def test_vector_and_scalar_paths_give_the_same_bits(K):
     assert all(bits(x, y) for x, y in zip(got, ref))
 
 
-def dyadic_inputs(B, C, H, W, K, N, samples, seed):
-    g = torch.Generator().manual_seed(seed)
-    vals = torch.tensor([0.0, 0.0, 0.0, 0.25, -0.25, 0.5, -0.5])
-    affinity = vals[torch.randint(0, 7, (B, K * K, H, W), generator=g)]
-    attention = torch.tensor([0.0, 0.5, 1.0, 1.0])[torch.randint(0, 4, (B, N * ((K + 1) // 2), H, W), generator=g)]
-    blur = torch.randint(-4, 5, (B, C, H, W), generator=g).float()
-    sparse = conf = None
-    if samples:
-        sparse = torch.randint(0, 5, (B, 1, H, W), generator=g).float()
-        conf = torch.tensor([0.0, 0.5, 1.0])[torch.randint(0, 3, (B, 1, H, W), generator=g)]
-        if samples == 'hard':
-            conf = (sparse > 0).float()
-    go = torch.randint(-2, 3, (B, C, H, W), generator=g).float()
-    return [affinity, attention, blur, sparse, conf], go
-
-
 @pytest.mark.parametrize('K,N', [(3, 3), (5, 2), (7, 2)])
 @pytest.mark.parametrize('samples', [None, 'soft', 'hard'])
 @pytest.mark.parametrize('shape', [(2, 2, 13, 20), (1, 2, 37, 260), (1, 1, 45, 261)])
 def test_dyadic_cases_equal_fp64_bit_for_bit(K, N, samples, shape):
     """(37, 260) crosses three 128 x 16 tiles of the 4-pixel step in x and y, with partial last tiles; (45, 261) runs
     the 1-pixel step across nine 32-wide tiles."""
-    ins, go = dyadic_inputs(*shape, K, N, samples, seed=K * 10 + N + shape[2])
+    ins, go = yr.dyadic_inputs(*shape, K, N, samples, seed=K * 10 + N + shape[2])
     ref = yr.grads(yr.composition, *ins, K, go, dtype=torch.float64)
     # the premise: every intermediate is exact, so fp32 in any order gives fp64's values
     r32 = yr.grads(yr.explicit, *ins, K, go)
