@@ -49,6 +49,10 @@ SIGNATURES = {
     'cspn2d_dyn_fwd_f32': (_i, [_vp] * 6 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_dyn_bwd_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_dyn_bwd_f32': (_i, [_vp] * 11 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_lin_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_lin_fwd_f32': (_i, [_vp] * 4 + [_i] * 6 + [_vp, _sz, _vp]),
+    'cspn2d_lin_bwd_workspace_bytes': (_sz, [_i] * 6),
+    'cspn2d_lin_bwd_f32': (_i, [_vp] * 6 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_paddle_workspace_bytes': (_sz, [_i] * 6),
     'cspn2d_paddle_fwd_f32': (_i, [_vp] * 3 + [_i] * 6 + [_vp, _sz, _vp]),
     'cspn2d_paddle_fwd_gather_f32': (_i, [_vp] * 4 + [_i, _vp] + [_i] * 6 + [_vp, _sz, _vp]),

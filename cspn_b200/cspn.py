@@ -994,6 +994,134 @@ class Affinity_PropagateDynamic(nn.Module):
         return f'prop_time={self.prop_time}, prop_kernel={self.prop_kernel}'
 
 
+# ---- linear three-way scans: SPN's propagation (DESIGN.md section 4.24) ------------------------------------------------
+LINEAR_DIRECTIONS = ('l2r', 'r2l', 't2b', 'b2t')
+
+
+def _linear_mask(directions):
+    """dir_mask of a non-empty subsequence of ('l2r', 'r2l', 't2b', 'b2t')."""
+    if isinstance(directions, str):
+        raise ValueError(f'directions must be a sequence of direction names, got {directions!r}')
+    ds = tuple(directions)
+    idx = [LINEAR_DIRECTIONS.index(d) if d in LINEAR_DIRECTIONS else -1 for d in ds]
+    if not ds or -1 in idx or idx != sorted(set(idx)):
+        raise ValueError(f'directions must be a non-empty subsequence of {LINEAR_DIRECTIONS}, got {directions!r}')
+    return sum(1 << i for i in idx)
+
+
+def _check_linear(feat, gate, directions):
+    """The checks of propagate2d_linear; every refusal comes before anything is allocated.  Returns (mask, gate_mode)."""
+    mask = _linear_mask(directions)
+    nd = len(tuple(directions))
+    if feat.dim() != 4 or min(feat.shape) < 1:
+        raise ValueError(f'feat must be a non-empty (B,C,H,W), got {tuple(feat.shape)}')
+    B, C, H, W = feat.shape
+    if gate.dim() != 4 or tuple(gate.shape[::2]) != (B, H) or gate.shape[3] != W or \
+            not (gate.shape[1] == 3 * nd or (C > 1 and gate.shape[1] == 3 * nd * C)):
+        raise ValueError(f'gate must be (B, 3*nd, H, W) = {(B, 3 * nd, H, W)} or, with C > 1, (B, 3*nd*C, H, W) = '
+                         f'{(B, 3 * nd * C, H, W)}, got {tuple(gate.shape)}')
+    if feat.dtype != torch.float32 or gate.dtype != torch.float32:
+        raise RuntimeError('cspn_b200 is fp32 only')
+    if gate.device != feat.device:
+        raise RuntimeError('feat and gate must be on one device')
+    lateral = max(H if mask & 3 else 0, W if mask & 12 else 0)
+    if B * C > 2 ** 31 - 1 or lateral > 2048 or H * W > 2 ** 31 - 1:
+        raise _lib.CspnError(f'propagate2d_linear takes B*C <= 2^31 - 1 and a lateral extent (H for l2r / r2l, W for t2b / b2t) '
+                             f'<= 2048, got feat {tuple(feat.shape)}')
+    if not feat.is_cuda:
+        raise _lib.CspnError('propagate2d_linear takes CUDA tensors only (there is no host-buffer entry point for it)')
+    return mask, (0 if gate.shape[1] == 3 * nd else 1)
+
+
+def _linear_fwd(feat, gate, mask, mode, keep_planes):
+    """Forward only (no autograd) through cspn2d_lin_fwd_f32, on the current stream.  Returns (out, planes): planes is
+    None for one direction, or when keep_planes is false (they then live in a workspace)."""
+    L = _lib.lib()
+    x, g = feat.contiguous(), gate.contiguous()
+    B, C, H, W = x.shape
+    nd = sum((mask >> i) & 1 for i in range(4))
+    out = torch.empty_like(x)
+    planes = torch.empty((nd, B, C, H, W), dtype=x.dtype, device=x.device) if keep_planes and nd > 1 else None
+    with torch.cuda.device(x.device):
+        ws_bytes = 0 if planes is not None else L.cspn2d_lin_workspace_bytes(B, C, H, W, mask, mode)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
+        rc = L.cspn2d_lin_fwd_f32(_ptr(x), _ptr(g), _ptr(out), _ptr(planes), B, C, H, W, mask, mode, _ptr(ws), ws_bytes,
+                                  _stream(x.device))
+    _lib.check(rc, 'cspn2d_lin_fwd_f32')
+    return out, planes
+
+
+class _Propagate2dLinearFn(torch.autograd.Function):
+    """autograd seam of propagate2d_linear without the torch-op shim: native forward + native backward
+    (cspn2d_lin_bwd_f32) over the saved per-direction planes, differentiable in feat and gate."""
+
+    @staticmethod
+    def forward(ctx, feat, gate, mask, mode):
+        out, planes = _linear_fwd(feat, gate, mask, mode, True)
+        ctx.save_for_backward(feat, gate, out if planes is None else planes)
+        ctx.cfg = (mask, mode)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        feat, gate, planes = ctx.saved_tensors
+        mask, mode = ctx.cfg
+        if not grad_out.is_cuda:
+            raise _lib.CspnError('backward needs CUDA tensors')
+        L = _lib.lib()
+        x, g, p, go = feat.contiguous(), gate.contiguous(), planes.contiguous(), grad_out.contiguous()
+        need_x, need_g = ctx.needs_input_grad[:2]
+        gx = torch.empty_like(x) if need_x else None
+        gg = torch.empty_like(g) if need_g else None
+        B, C, H, W = x.shape
+        with torch.cuda.device(x.device):
+            ws_bytes = L.cspn2d_lin_bwd_workspace_bytes(B, C, H, W, mask, mode)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
+            rc = L.cspn2d_lin_bwd_f32(_ptr(x), _ptr(g), _ptr(p), _ptr(go), _ptr(gx), _ptr(gg), B, C, H, W, mask, mode, _ptr(ws),
+                                      ws_bytes, _stream(x.device))
+        _lib.check(rc, 'cspn2d_lin_bwd_f32')
+        return gx, gg, None, None
+
+
+def propagate2d_linear(feat, gate, directions=LINEAR_DIRECTIONS):
+    """SPN's linear spatial propagation with three-way connections (Liu et al., NIPS 2017), one scan per direction and a
+    node-wise max over the directions.  For 'l2r' (scan index t the column, lateral index i the row):
+        h[i, t] = (1 - g0 - g1 - g2) x[i, t] + g0 h[i-1, t-1] + g1 h[i, t-1] + g2 h[i+1, t-1]
+    with g_j = gate_j[i, t] at the current node, used as given (no abs, no normalisation: SPN's stability condition
+    sum_j |g_j| <= 1 is the caller's to enforce), and reads outside the image 0.  'r2l' reads column t + 1, 't2b' and
+    'b2t' scan rows and read row y -+ 1 at columns x - 1, x, x + 1; tap j is lateral offset j - 1 along increasing index.
+    directions is a non-empty subsequence of ('l2r', 'r2l', 't2b', 'b2t').  gate is (B, 3*nd, H, W), shared by the C
+    channels of feat (B, C, H, W), or (B, 3*nd*C, H, W) with C > 1, one gate per channel; direction block k (the k-th
+    listed direction) is channels [3k*C', 3(k+1)*C') with C' = 1 or C, and channel c uses 3c .. 3c+2 within it, so
+    gate[:, block k] is the gate of a one-direction call.  Several directions are merged node-wise by max: out is h of the
+    first direction that is NaN there, else of the first attaining the maximum (torch.stack(hs).max(0)); the gradient goes
+    to that direction alone.  fp32 CUDA tensors; differentiable in feat and gate with a deterministic backward.
+    DESIGN.md section 4.24 states the order of every operation; INTEGRATION.md section 2i builds an SPN head from it."""
+    mask, mode = _check_linear(feat, gate, directions)
+    if torch.compiler.is_compiling() or _use_torch_op():     # under torch.compile the op is the one traceable route
+        return torch.ops.cspn_b200.propagate2d_linear(feat, gate, mask)[0]
+    if torch.is_grad_enabled() and (feat.requires_grad or gate.requires_grad):
+        return _Propagate2dLinearFn.apply(feat, gate, mask, mode)
+    return _linear_fwd(feat, gate, mask, mode, False)[0]
+
+
+class Affinity_PropagateLinear(nn.Module):
+    """SPN's linear propagation as a module: forward(feat, gate) is propagate2d_linear(feat, gate, directions).  No
+    parameters, no buffers: the gates come from the caller's guidance network (INTEGRATION.md section 2i)."""
+
+    def __init__(self, directions=LINEAR_DIRECTIONS):
+        super().__init__()
+        _linear_mask(directions)
+        self.directions = tuple(directions)
+
+    def forward(self, feat, gate):
+        return propagate2d_linear(feat, gate, self.directions)
+
+    def extra_repr(self):
+        return f'directions={self.directions}'
+
+
 # ---- 3D with a K x K x K affinity kernel (K in {3, 5}) ---------------------------------------------------------------
 KERNEL_SIZES_3D = (3, 5)
 

@@ -1515,6 +1515,95 @@ int cspn2d_dyn_bwd_f32(const float* affinity, const float* attention, const floa
     });
 }
 
+// ---- 2D linear three-way scans, SPN's propagation (DESIGN.md section 4.24) -------------------------------------------
+static bool lin_args_ok(int B, int C, int H, int W, int mask, int gate_mode) {
+    if (!positive(B, C, H, W)) { set_error("non-positive shape B=%d C=%d H=%d W=%d", B, C, H, W); return false; }
+    if (mask < 1 || mask > 15) { set_error("dir_mask must be 1 .. 15 (bits l2r, r2l, t2b, b2t), got %d", mask); return false; }
+    if (gate_mode != CSPN_LIN_GATE_SHARED && gate_mode != CSPN_LIN_GATE_PER_CHANNEL) {
+        set_error("unknown gate_mode %d", gate_mode);
+        return false;
+    }
+    if ((long long)3 * __builtin_popcount(mask) * (gate_mode ? C : 1) > INT32_MAX) { set_error("3 * nd * C gate channels exceed 2^31 - 1"); return false; }
+    return true;
+}
+
+// The alignment of the non-null pointers, the launch limits, the overlaps, then the workspace
+static int check_lin_buffers(int B, int C, int H, int W, int mask, std::vector<Buf> in, std::vector<Buf> outs, const void* ws,
+                             size_t ws_bytes, size_t need) {
+    uintptr_t bits = 0;
+    for (auto* set : {&in, &outs}) {
+        std::vector<Buf> kept;
+        for (const Buf& b : *set)
+            if (b.p) {
+                bits |= reinterpret_cast<uintptr_t>(b.p);
+                kept.push_back(b);
+            }
+        *set = kept;
+    }
+    if (bits & 3) { set_error("tensor pointers must be 4-byte aligned"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const char* why = "";
+    if (!linear2d_launchable(B, C, H, W, mask, &why)) { set_error("unsupported shape: %s", why); return CSPN_ERR_UNSUPPORTED; }
+    const int rc = check_disjoint(in, outs);
+    if (rc != CSPN_OK) return rc;
+    if (need && (!ws || ws_bytes < need)) {
+        set_error("the linear propagation needs %zu workspace bytes, got %zu", need, ws ? ws_bytes : (size_t)0);
+        return CSPN_ERR_WORKSPACE;
+    }
+    return CSPN_OK;
+}
+
+size_t cspn2d_lin_workspace_bytes(int B, int C, int H, int W, int dir_mask, int gate_mode) {
+    if (!lin_args_ok(B, C, H, W, dir_mask, gate_mode)) return 0;
+    return linear2d_workspace_bytes(B, C, H, W, dir_mask);
+}
+
+size_t cspn2d_lin_bwd_workspace_bytes(int B, int C, int H, int W, int dir_mask, int gate_mode) {
+    if (!lin_args_ok(B, C, H, W, dir_mask, gate_mode)) return 0;
+    return linear2d_bwd_workspace_bytes(B, C, H, W, dir_mask, gate_mode ? C : 1);
+}
+
+int cspn2d_lin_fwd_f32(const float* feat, const float* gate, float* out, float* planes, int B, int C, int H, int W, int dir_mask,
+                       int gate_mode, void* workspace, size_t workspace_bytes, cspn_stream_t stream) {
+    begin_call();
+    if (!feat || !gate || !out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!lin_args_ok(B, C, H, W, dir_mask, gate_mode)) return CSPN_ERR_INVALID_ARGUMENT;
+    const int nd = __builtin_popcount(dir_mask), Cg = gate_mode ? C : 1;
+    if (planes && nd == 1) { set_error("planes must be NULL for one direction (its plane is out)"); return CSPN_ERR_INVALID_ARGUMENT; }
+    const long long hw = (long long)H * W;
+    const uintptr_t n_x = span_bytes(B, C, hw), n_p = span_bytes(B, C, nd * hw);
+    const size_t need = planes ? 0 : linear2d_workspace_bytes(B, C, H, W, dir_mask);
+    float* pl = nd > 1 ? (planes ? planes : static_cast<float*>(workspace)) : nullptr;
+    const int rc = check_lin_buffers(B, C, H, W, dir_mask, {{feat, n_x, "feat"}, {gate, span_bytes(B, 3 * nd * Cg, hw), "gate"}},
+                                     {{out, n_x, "out"}, {planes, n_p, "planes"}, {need ? workspace : nullptr, need, "the workspace"}},
+                                     workspace, workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return linear2d_forward(feat, gate, out, pl, B, C, H, W, dir_mask, Cg, (cudaStream_t)stream, launches);
+    });
+}
+
+int cspn2d_lin_bwd_f32(const float* feat, const float* gate, const float* planes, const float* grad_out, float* grad_feat,
+                       float* grad_gate, int B, int C, int H, int W, int dir_mask, int gate_mode, void* workspace, size_t workspace_bytes,
+                       cspn_stream_t stream) {
+    begin_call();
+    if (!feat || !gate || !planes || !grad_out) { set_error("null tensor pointer"); return CSPN_ERR_INVALID_ARGUMENT; }
+    if (!lin_args_ok(B, C, H, W, dir_mask, gate_mode)) return CSPN_ERR_INVALID_ARGUMENT;
+    const int nd = __builtin_popcount(dir_mask), Cg = gate_mode ? C : 1;
+    const long long hw = (long long)H * W;
+    const uintptr_t n_x = span_bytes(B, C, hw), n_g = span_bytes(B, 3 * nd * Cg, hw);
+    const size_t need = (grad_feat || grad_gate) ? linear2d_bwd_workspace_bytes(B, C, H, W, dir_mask, Cg) : 0;
+    const int rc = check_lin_buffers(B, C, H, W, dir_mask,
+                                     {{feat, n_x, "feat"}, {gate, n_g, "gate"}, {planes, span_bytes(B, C, nd * hw), "planes"},
+                                      {grad_out, n_x, "grad_out"}},
+                                     {{grad_feat, n_x, "grad_feat"}, {grad_gate, n_g, "grad_gate"}, {need ? workspace : nullptr, need, "the workspace"}},
+                                     workspace, workspace_bytes, need);
+    if (rc != CSPN_OK) return rc;
+    return on_device_of(feat, "feat", [&](int* launches) {
+        return linear2d_backward(feat, gate, planes, grad_out, grad_feat, grad_gate, B, C, H, W, dir_mask, Cg, workspace,
+                                 (cudaStream_t)stream, launches);
+    });
+}
+
 int cspn2d_describe_plan(int B, int C, int H, int W, int iters, int algo, char* buf, int buf_len) {
     if (!buf || buf_len <= 0) return 0;
     Problem2D p{nullptr, nullptr, nullptr, nullptr, B, C, H, W, 8, iters, 0};

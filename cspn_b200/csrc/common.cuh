@@ -289,4 +289,17 @@ int dynamic2d_backward(const float* aff, const float* att, const float* blur, co
                        const float* grad_out, float* grad_aff, float* grad_att, float* grad_blur, float* grad_sparse, float* grad_conf,
                        int B, int C, int H, int W, int K, int N, void* ws, cudaStream_t st, int* launches);
 
+// Linear three-way scans, SPN's propagation (cspn2d_linear.cu): feat (B, C, H, W), gate (B, 3*nd*Cg, H, W) with Cg 1 or C,
+// mask bits 1 l2r, 2 r2l, 4 t2b, 8 b2t; arguments checked by the caller (sizes, pointers, then launchable).  planes
+// (nd, B, C, H, W) receive every direction's h when nd > 1 (the forward then merges them into out); with nd = 1 h goes to
+// out, and the backward's planes are that output.  The backward's workspace holds grad_x's per-direction planes and the
+// d* bytes (nd > 1) and a shared gate's per-channel gradient (Cg = 1 < C)
+int linear2d_launchable(int B, int C, int H, int W, int mask, const char** why);
+size_t linear2d_workspace_bytes(int B, int C, int H, int W, int mask);
+size_t linear2d_bwd_workspace_bytes(int B, int C, int H, int W, int mask, int Cg);
+int linear2d_forward(const float* feat, const float* gate, float* out, float* planes, int B, int C, int H, int W, int mask, int Cg,
+                     cudaStream_t st, int* launches);
+int linear2d_backward(const float* feat, const float* gate, const float* planes, const float* grad_out, float* grad_feat,
+                      float* grad_gate, int B, int C, int H, int W, int mask, int Cg, void* ws, cudaStream_t st, int* launches);
+
 }  // namespace cspn

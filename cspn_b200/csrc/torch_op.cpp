@@ -43,6 +43,12 @@
 //   propagate2d_dynamic_backward(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence,
 //                                Tensor grad_out, int kernel_size, bool need_affinity, bool need_attention, bool need_blur,
 //                                bool need_sparse, bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor, Tensor)
+//   propagate2d_linear(Tensor feat, Tensor gate, int dir_mask) -> (Tensor, Tensor)
+//       (SPN's three-way scans: feat (B, C, H, W), gate (B, 3*nd, H, W) shared or (B, 3*nd*C, H, W) per channel with C > 1,
+//       dir_mask bits l2r, r2l, t2b, b2t; returns the merged output and the per-direction planes (nd, B, C, H, W), empty
+//       for nd = 1)
+//   propagate2d_linear_backward(Tensor feat, Tensor gate, Tensor planes, Tensor grad_out, int dir_mask, bool need_feat,
+//                               bool need_gate) -> (Tensor, Tensor)   (planes: the forward's planes, its output for nd = 1)
 //   propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor
 //       (own-location gates, K in {3, 5, 7}; guidance (B, K*K-1, H, W) shared, or (B, (K*K-1)*C, H, W) per channel)
 //   propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time,
@@ -99,6 +105,7 @@
 #include <c10/cuda/CUDAStream.h>
 #include <torch/library.h>
 
+#include <algorithm>
 #include <optional>
 #include <tuple>
 #include <utility>
@@ -518,6 +525,56 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> propagate
                                 C, H, W, (int)K, (int)N, ws.ptr(), ws.bytes, current_stream()),
              "cspn2d_dyn_bwd_f32");
     return {grad_or_empty(ga, a), grad_or_empty(gt, at_), grad_or_empty(gd, d), grad_or_empty(gs, d), grad_or_empty(gm, d)};
+}
+
+// Linear three-way scans (SPN): cspn2d_lin_*_f32.  feat (B, C, H, W), gate (B, 3*nd, H, W) or (B, 3*nd*C, H, W) with C > 1.
+// Returns the gate mode.
+int check2d_lin(const at::Tensor& feat, const at::Tensor& gate, int64_t mask) {
+    TORCH_CHECK_VALUE(mask >= 1 && mask <= 15, "dir_mask must be 1 .. 15, got ", mask);
+    TORCH_CHECK_VALUE(feat.dim() == 4 && feat.numel() > 0, "feat must be a non-empty (B,C,H,W), got ", feat.sizes());
+    const int64_t B = feat.size(0), C = feat.size(1), H = feat.size(2), W = feat.size(3), nd = __builtin_popcountll(mask);
+    TORCH_CHECK_VALUE(gate.dim() == 4 && gate.size(0) == B && gate.size(2) == H && gate.size(3) == W &&
+                              (gate.size(1) == 3 * nd || (C > 1 && gate.size(1) == 3 * nd * C)),
+                      "gate must be (B, 3*nd, H, W) or, with C > 1, (B, 3*nd*C, H, W), nd = ", nd, ", feat ", feat.sizes(), ", got ",
+                      gate.sizes());
+    TORCH_CHECK(feat.scalar_type() == at::kFloat && gate.scalar_type() == at::kFloat, "cspn_b200 is fp32 only");
+    TORCH_CHECK(gate.device() == feat.device(), "feat and gate are on different devices");
+    const int64_t lat = std::max<int64_t>((mask & 3) ? H : 0, (mask & 12) ? W : 0);
+    TORCH_CHECK(B * C <= INT32_MAX && lat <= 2048 && gate.size(1) <= INT32_MAX && H * W <= INT32_MAX,
+                "propagate2d_linear takes B*C <= 2^31 - 1 and a lateral extent (H for l2r / r2l, W for t2b / b2t) <= 2048, got feat ",
+                feat.sizes());
+    return gate.size(1) == 3 * nd ? CSPN_LIN_GATE_SHARED : CSPN_LIN_GATE_PER_CHANNEL;
+}
+
+std::tuple<at::Tensor, at::Tensor> propagate2d_linear_cuda(const at::Tensor& feat, const at::Tensor& gate, int64_t mask) {
+    const int mode = check2d_lin(feat, gate, mask);
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor x = feat.contiguous(), g = gate.contiguous();
+    const int B = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3), nd = __builtin_popcount((int)mask);
+    at::Tensor out = at::empty_like(x);
+    at::Tensor planes = nd > 1 ? at::empty({nd, B, C, H, W}, x.options()) : at::zeros({0}, x.options());
+    check_rc(cspn2d_lin_fwd_f32(fptr(x), fptr(g), mptr(out), nd > 1 ? mptr(planes) : nullptr, B, C, H, W, (int)mask, mode, nullptr, 0,
+                                current_stream()),
+             "cspn2d_lin_fwd_f32");
+    return {out, planes};
+}
+
+std::tuple<at::Tensor, at::Tensor> propagate2d_linear_backward_cuda(const at::Tensor& feat, const at::Tensor& gate, const at::Tensor& planes,
+                                                                    const at::Tensor& grad_out, int64_t mask, bool need_x, bool need_g) {
+    const int mode = check2d_lin(feat, gate, mask);
+    check_grad_out(grad_out, feat, "feat");
+    const int64_t nd = __builtin_popcountll(mask);
+    TORCH_CHECK_VALUE(planes.numel() == nd * feat.numel() && planes.scalar_type() == at::kFloat && planes.device() == feat.device(),
+                      "planes must hold the forward's nd = ", nd, " planes of feat's shape, got ", planes.sizes());
+    const c10::cuda::CUDAGuard guard(feat.device());
+    const at::Tensor x = feat.contiguous(), g = gate.contiguous(), p = planes.contiguous(), go = grad_out.contiguous();
+    at::Tensor gx = new_grad(need_x, x), gg = new_grad(need_g, g);
+    const int B = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3);
+    const Workspace ws(cspn2d_lin_bwd_workspace_bytes(B, C, H, W, (int)mask, mode), x);
+    check_rc(cspn2d_lin_bwd_f32(fptr(x), fptr(g), fptr(p), fptr(go), mptr(gx), mptr(gg), B, C, H, W, (int)mask, mode, ws.ptr(), ws.bytes,
+                                current_stream()),
+             "cspn2d_lin_bwd_f32");
+    return {grad_or_empty(gx, x), grad_or_empty(gg, g)};
 }
 
 // 2D 'paddle' (own-location gates), K in {3, 5, 7}.  guidance (B, K*K-1, H, W) is shared by the C channels of feat;
@@ -1161,6 +1218,9 @@ TORCH_LIBRARY(cspn_b200, m) {
     m.def("propagate2d_dynamic_backward(Tensor affinity, Tensor attention, Tensor blur_depth, Tensor? sparse_depth, Tensor? confidence, "
           "Tensor grad_out, int kernel_size, bool need_affinity, bool need_attention, bool need_blur, bool need_sparse, "
           "bool need_confidence) -> (Tensor, Tensor, Tensor, Tensor, Tensor)");
+    m.def("propagate2d_linear(Tensor feat, Tensor gate, int dir_mask) -> (Tensor, Tensor)");
+    m.def("propagate2d_linear_backward(Tensor feat, Tensor gate, Tensor planes, Tensor grad_out, int dir_mask, bool need_feat, "
+          "bool need_gate) -> (Tensor, Tensor)");
     m.def("propagate2d_paddle(Tensor guidance, Tensor feat, int kernel_size, int prop_time) -> Tensor");
     m.def("propagate2d_paddle_backward(Tensor guidance, Tensor feat, Tensor grad_out, int kernel_size, int prop_time, "
           "bool need_guidance, bool need_feat) -> (Tensor, Tensor)");
@@ -1213,6 +1273,8 @@ TORCH_LIBRARY_IMPL(cspn_b200, CUDA, m) {
     m.impl("propagate2d_dilated_backward", &propagate2d_dilated_backward_cuda);
     m.impl("propagate2d_dynamic", &propagate2d_dynamic_cuda);
     m.impl("propagate2d_dynamic_backward", &propagate2d_dynamic_backward_cuda);
+    m.impl("propagate2d_linear", &propagate2d_linear_cuda);
+    m.impl("propagate2d_linear_backward", &propagate2d_linear_backward_cuda);
     m.impl("propagate2d_paddle", &propagate2d_paddle_cuda);
     m.impl("propagate2d_paddle_backward", &propagate2d_paddle_backward_cuda);
     m.impl("propagate3d", &propagate3d_cuda);

@@ -249,6 +249,38 @@ def _register():
 
     lib.register_autograd('cspn_b200::propagate2d_dynamic', backward2d_dynamic, setup_context=setup2d_dynamic)
 
+    @lib.register_fake('cspn_b200::propagate2d_linear')
+    def _(feat, gate, dir_mask):
+        torch._check(1 <= dir_mask <= 15, lambda: 'dir_mask must be 1 .. 15')
+        torch._check(feat.dim() == 4 and gate.dim() == 4, lambda: 'feat and gate must be (B,C,H,W)')
+        nd = sum((dir_mask >> i) & 1 for i in range(4))
+        torch._check(gate.shape[1] == 3 * nd or gate.shape[1] == 3 * nd * feat.shape[1],
+                     lambda: f'{nd} directions need (B,{3 * nd},H,W) or (B,{3 * nd}*C,H,W) gates')
+        out = torch.empty_like(feat, memory_format=torch.contiguous_format)
+        planes = feat.new_empty((nd, *feat.shape)) if nd > 1 else feat.new_empty(0)
+        return out, planes
+
+    @lib.register_fake('cspn_b200::propagate2d_linear_backward')
+    def _(feat, gate, planes, grad_out, dir_mask, need_feat, need_gate):
+        new = lambda need, x: torch.empty_like(x, memory_format=torch.contiguous_format) if need else x.new_empty(0)
+        return new(need_feat, feat), new(need_gate, gate)
+
+    def setup2d_linear(ctx, inputs, output):
+        feat, gate, dir_mask = inputs
+        out, planes = output
+        ctx.mark_non_differentiable(planes)
+        ctx.save_for_backward(feat, gate, planes if dir_mask & (dir_mask - 1) else out)   # one direction: its plane is out
+        ctx.dir_mask = dir_mask
+
+    def backward2d_linear(ctx, grad_out, _grad_planes):
+        feat, gate, planes = ctx.saved_tensors
+        need_f, need_g = ctx.needs_input_grad[:2]
+        gf, gg = torch.ops.cspn_b200.propagate2d_linear_backward(feat, gate, planes, grad_out.contiguous(), ctx.dir_mask, need_f,
+                                                                 need_g)
+        return (gf if need_f else None), (gg if need_g else None), None
+
+    lib.register_autograd('cspn_b200::propagate2d_linear', backward2d_linear, setup_context=setup2d_linear)
+
     @lib.register_fake('cspn_b200::propagate2d_paddle')
     def _(guidance, feat, kernel_size, prop_time):
         torch._check(guidance.dim() == 4 and feat.dim() == 4, lambda: 'guidance and feat must be (B,C,H,W)')

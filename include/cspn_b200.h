@@ -340,6 +340,44 @@ CSPN_API int cspn2d_dyn_bwd_f32(const float* affinity, const float* attention, c
                        float* grad_blur, float* grad_sparse, float* grad_confidence, int B, int C, int H, int W, int K,
                        int iters, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
 
+/* ---- 2D linear three-way scans: SPN's propagation (Liu et al., NIPS 2017; DESIGN.md section 4.24) -------------------
+ * feat [B][C][H][W] is scanned in every direction of dir_mask (bit 0 l2r, 1 r2l, 2 t2b, 3 b2t; nd set bits, 1 .. 4,
+ * taken in that canonical order).  For l2r (scan index t the column, lateral index i the row), with g_j = gate_j[i][t]
+ * used as given (no abs, no normalisation) and reads outside the image 0:
+ *   c = ((1 - g0) - g1) - g2,   h[i][t] = fma(g2, h[i+1][t-1], fma(g1, h[i][t-1], fma(g0, h[i-1][t-1], c * x[i][t])))
+ * r2l reads column t + 1; t2b and b2t scan rows and read row y -+ 1 at columns x - 1, x, x + 1: tap j is lateral offset
+ * j - 1 along increasing index in every direction.  gate_mode CSPN_LIN_GATE_SHARED: gate [B][3*nd][H][W], shared by the
+ * C channels; CSPN_LIN_GATE_PER_CHANNEL: gate [B][3*nd*C][H][W].  Direction block k (the k-th requested direction) is
+ * channels [3k*Cg, 3(k+1)*Cg), Cg = 1 or C, and channel c uses 3c .. 3c+2 within it.  out [B][C][H][W] is h for one
+ * direction, else the node-wise max: h of the first direction that is NaN there, else of the first attaining the maximum.
+ * planes [nd][B][C][H][W] (optional, nd > 1 only; NULL for nd = 1) receives every direction's h; without it the planes go
+ * to the workspace.  The backward takes the planes (for nd = 1 the forward's out), routes grad_out to the direction the
+ * merge picked, runs the adjoint scans in reverse and writes grad_feat [B][C][H][W] and grad_gate (laid out as gate),
+ * whichever is not NULL: grad_feat sums the directions in canonical order, a shared gate's gradient sums the channels
+ * c ascending (DESIGN.md section 4.24 gives every operation's order).
+ * Workspace (bytes, device-independent; the queries return 0 for invalid arguments): forward 4 * nd * B*C*H*W for
+ * nd > 1 (0 when planes is given), else 0; backward, for nd > 1, 8 * nd * B*C*H*W (grad_feat's per-direction planes
+ * and the routed grad_out), and, for a shared gate with C > 1, 12 * nd * B*C*H*W.  Launches: forward 1 (nd = 1) or 2; backward at most 3.  No
+ * atomics and no memsets; the bits depend on the arguments only.
+ * CSPN_ERR_INVALID_ARGUMENT for a null feat / gate / out (planes / grad_out in the backward), planes given with nd = 1,
+ * dir_mask outside 1 .. 15, an unknown gate_mode, a non-positive shape, a pointer that is not 4-byte aligned, and an
+ * output (the workspace included) that overlaps an input or another output; CSPN_ERR_UNSUPPORTED for B*C times the
+ * cluster size (1 .. 8, chosen from the shape) past 2^31 - 1 or a lateral extent (H for l2r / r2l, W for t2b / b2t) past 2048; CSPN_ERR_WORKSPACE for a missing or short workspace.  All
+ * of these come before any device work. */
+#define CSPN_LIN_GATE_SHARED 0
+#define CSPN_LIN_GATE_PER_CHANNEL 1
+
+CSPN_API size_t cspn2d_lin_workspace_bytes(int B, int C, int H, int W, int dir_mask, int gate_mode);
+
+CSPN_API int cspn2d_lin_fwd_f32(const float* feat, const float* gate, float* out, float* planes, int B, int C, int H, int W,
+                       int dir_mask, int gate_mode, void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
+CSPN_API size_t cspn2d_lin_bwd_workspace_bytes(int B, int C, int H, int W, int dir_mask, int gate_mode);
+
+CSPN_API int cspn2d_lin_bwd_f32(const float* feat, const float* gate, const float* planes, const float* grad_out,
+                       float* grad_feat, float* grad_gate, int B, int C, int H, int W, int dir_mask, int gate_mode,
+                       void* workspace, size_t workspace_bytes, cspn_stream_t stream);
+
 /* ---- 2D with the Paddle module's own-location gates, K in {3, 5, 7} (CSPN.cspn with dimNum = 2, demo.py:20-54) -----
  * w_k(p) = |g_k(p)| / sum_j |g_j(p)| at the pixel's own location (IEEE division: a zero sum gives NaN), then iters steps
  * d_{t+1}(p) = sum_k w_k(p) d_t(p + off_k) with zero padding, no centre term and no sparse replacement.  Taps as in the
